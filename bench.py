@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the YOLOv3 hot path on B200 (contract: see task ④).
+"""bench.py — headline benchmark of the YOLOv3 hot path on one or more H100 GPUs.
 
 Workload (BASELINE.json configs[1]): batch=64 416x416 inference, 80 classes, one step =
 forward (75 convs) -> decode (+ score = conf*prob) -> per-image gpu_nms(max_boxes=200,
@@ -8,12 +8,18 @@ score_thresh=0.3, nms_thresh=0.45) over one batch of synthetic images.  Weights 
 and conf bias -2 so that scores straddle the 0.3 threshold.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--size S]
+                  [--dump-outputs DIR]
 
 `value`  : images/s with the batch already resident in HBM, CUDA-event timed, max over ranks.
 `e2e`    : images/s through the public API from pinned HOST float32 images (H2D inside the
            timed region) to host-side detections (D2H inside the timed region).
-`roofline`: the tensor-core conv kernel (74 launches/step): algorithmic conv FLOPs / event-timed
-           duration of those launches, against MEASURED_PEAKS.json's sustained bf16 peak.
+`roofline`: the tensor-core conv kernels (74 launches/step): algorithmic conv FLOPs / event-timed
+           duration of those launches, against MEASURED_PEAKS.json's sustained bf16 peak when that file
+           exists, else the H100 SXM data-sheet figure (989 TFLOP/s dense bf16, 3.35 TB/s HBM3).
+`--dump-outputs DIR`: after the timed device-resident steps, the arrays the last of them returned (decoded boxes,
+           per-image NMS boxes / scores / labels / indices / counts) are written to DIR as float32 .npy files;
+           slots past an image's detection count are zeroed.  Inputs and weights are seeded, so two builds can be
+           compared output for output.
 `cpu_baseline` / `--impl reference`: the CPU oracle port (TensorFlow 1.x cannot be installed in
            this image) timed on the host cores on a bounded sample of the same workload.
 """
@@ -63,7 +69,7 @@ def make_bench_params(seed=2, specs=None):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -104,7 +110,7 @@ def peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(tflops=p.get("bf16_tflops_sustained", p.get("bf16_tflops")), hbm=p.get("hbm_gbs"), src="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet (dense bf16, HBM3), not measured")
 
 
 # --------------------------------------------------------------------------------------
@@ -327,6 +333,24 @@ def latency_b1(pkg, S, iters=30):
             "what": "batch 1, %dx%d, forward + decode + NMS (yb_net_detect), device-resident input, 76 launches" % (S, S)}
 
 
+def dump_outputs(out_dir, result):
+    """Writes detect_raw()'s result tuple as float32 .npy files (labels, indices and counts are small integers, exact in
+    float32).  Slots past an image's detection count hold no result and are written as zeros."""
+    import torch
+    boxes, ob, os_, ol, oi, cnt = (t.cpu() for t in result)
+    valid = torch.arange(ob.shape[1])[None, :] < cnt[:, None].long()
+    zero = torch.zeros((), dtype=torch.float32)
+    arrays = {"decoded_boxes": boxes.float(),
+              "nms_boxes": torch.where(valid[..., None], ob.float(), zero),
+              "nms_scores": torch.where(valid, os_.float(), zero),
+              "nms_labels": torch.where(valid, ol.float(), zero),
+              "nms_indices": torch.where(valid, oi.float(), zero),
+              "nms_counts": cnt.float()}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -341,6 +365,8 @@ def main():
     ap.add_argument("--no-train608", action="store_true")
     ap.add_argument("--train-batch", type=int, default=32)
     ap.add_argument("--train-size", type=int, default=416)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -349,7 +375,7 @@ def main():
                 f"COCO 80-class, random-init cfg-2 weights (BASELINE.json configs[1])")
     config = {"workload": workload, "batch_per_gpu": args.batch, "image": [args.size, args.size], "classes": CLASS_NUM,
               "parallelism": f"replicas x{world} (independent images, no data-path collective)",
-              "l2": "per-step inputs (133 MB) + activations (~6 GB) exceed the 126 MB L2; no explicit flush"}
+              "l2": "per-step inputs (133 MB) + activations (~6 GB) exceed the 50 MB L2; no explicit flush"}
 
     if args.cpu_worker:
         size, passes, warmup, images, threads = (int(v) for v in args.cpu_worker.split(","))
@@ -389,7 +415,7 @@ def main():
     def step_device():
         # forward -> decode -> score -> per-image NMS in one engine call (decode + score filter fused into the
         # detection-head epilogues; bit-identical to forward() + predict_scores() + batched_nms_raw(), tests/test_gpu_path.py)
-        return model.detect_raw(x_dev, **NMS_ARGS)[1:]
+        return model.detect_raw(x_dev, **NMS_ARGS)
 
     def step_device_unfused():
         fms = model.forward(x_dev)
@@ -448,7 +474,7 @@ def main():
     for _ in range(max(args.warmup, 3)):
         out = step_device()
     torch.cuda.synchronize()
-    n_det = int(out[4].sum())
+    n_det = int(out[5].sum())
 
     # ---------------- timed: device-resident ----------------
     sampler = ClockSampler(local_rank)
@@ -458,9 +484,12 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step_device()
+        out = step_device()
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
+    del out
     ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -492,7 +521,7 @@ def main():
     e2e_ms = float(ms2)
 
     # ---------------- roofline: the tensor-core conv kernel, event-timed inside the step ----------------
-    # the same step, its three parts bracketed by events: stem | 74 tcgen05 convs (decode fused into the heads) | NMS
+    # the same step, its three parts bracketed by events: stem | 74 wgmma convs (decode fused into the heads) | NMS
     conv_ms, stem_ms, nms_ms = [], [], []
     res = model.detect_raw(x_dev, **NMS_ARGS)
     for i in range(args.steps + 2):
@@ -522,16 +551,9 @@ def main():
     conv_flop = FWD_GFLOP_416 * scale * 1e9 * B          # all 75 convs: the stem runs inside the first tensor-core launch
     pk = peaks()
     achieved = conv_flop / conv_t / 1e12
-    traffic = None      # DRAM bytes of the same 74 launches, from the committed ncu table (profiles/, not measured here)
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "conv_traffic.json")))
-        if tj.get("batch") == B and tj.get("size") == S:
-            traffic = tj["dram_bytes_per_step"]
-    except Exception:
-        pass
-    roofline = {"bound": "tensor", "kernel": "tcgen05 conv kernels (74 launches per step: conv_halo with the stem fused in for layer 1, conv_halo / conv_igemm 1-CTA and CTA-pair kernels for layers 2..74)",
+    roofline = {"bound": "tensor", "kernel": "wgmma conv kernels (74 launches per step: conv_halo with the stem fused in for layer 1, conv_halo / conv_igemm for layers 2..74)",
                 "achieved": achieved,
-                "peak": pk["tflops"], "unit": "TFLOP/s", "frac": achieved / pk["tflops"], "traffic": traffic,
+                "peak": pk["tflops"], "unit": "TFLOP/s", "frac": achieved / pk["tflops"], "traffic": None,
                 "peak_source": pk["src"], "ms_per_step_conv": conv_t * 1e3, "ms_per_step_stem": float(np.mean(stem_ms)),
                 "ms_per_step_nms": float(np.mean(nms_ms)),
                 "algorithmic_flop_per_step": conv_flop}
@@ -630,10 +652,10 @@ def main():
             torch.cuda.empty_cache()
             return out
 
-        train = bench_train(args.train_batch, args.train_size, max(3, min(args.steps, 8)))
+        train = bench_train(args.train_batch, args.train_size, args.steps)
         train["config"] = "BASELINE.json configs[3] per-GPU shape: batch %d x %d GPU(s), 416x416, bf16, data-parallel" % (args.train_batch, world)
         if world == 1 and not args.no_train608:
-            train608 = bench_train(32, 608, max(3, min(args.steps, 5)))
+            train608 = bench_train(32, 608, args.steps)
             train608["config"] = "BASELINE.json configs[2]: batch=32 608x608 training step, random init, 1 GPU"
 
     if rank != 0:
@@ -649,7 +671,7 @@ def main():
             "e2e": {"value": imgs / (e2e_ms * 1e-3), "unit": "images/s", "h2d_bytes_per_step": x_host.numel() * 4,
                     "d2h_bytes_per_step": int(d2h), "ms_per_step": e2e_ms / args.steps},
             "gpu_launches": args.steps * (74 + 2),
-            "launches_per_step": {"stem (mma.sync) fused into Conv_1's halo producer + conv_halo / conv_igemm (tcgen05: halo-tile, 1-CTA, CTA-pair kernels; decode + score filter in the 3 head epilogues)": 74,
+            "launches_per_step": {"stem (mma.sync) fused into Conv_1's halo producer + conv_halo / conv_igemm (wgmma: halo-tile and implicit-GEMM kernels; decode + score filter in the 3 head epilogues)": 74,
                                   "nms_select + nms_gather": 2},
             "unfused_api_ms_per_step": unfused_ms,
             "detections_per_step": n_det, "clocks": clocks, "roofline": roofline,

@@ -1,12 +1,14 @@
 #!/bin/bash
-# Build libyolob200.so (sm_100a) in-tree.  Usage: ./build.sh [extra nvcc flags]
+# Build libyolob200.so (sm_90a) in-tree.  Usage: ./build.sh [extra nvcc flags]
 set -e
 cd "$(dirname "$0")"
 SRC=yolov3_tensorflow_b200/csrc
 OUT=yolov3_tensorflow_b200/libyolob200.so
 mkdir -p build
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr $*"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr $*"
+# objects compiled with other flags (another architecture, say) are rebuilt
+if [ "$(cat build/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f build/*.o; echo "$FLAGS" > build/flags; fi
 pids=()
 for f in $SRC/*.cu; do
   o=build/$(basename ${f%.cu}).o
@@ -16,5 +18,5 @@ for f in $SRC/*.cu; do
   fi
 done
 for p in "${pids[@]}"; do wait $p; done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o $OUT build/*.o -cudart static
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o $OUT build/*.o -cudart static
 echo "built $OUT"

@@ -1,4 +1,4 @@
-/* yolob200.h — C ABI of libyolob200.so: the B200-native (sm_100a) replacement for the
+/* yolob200.h — C ABI of libyolob200.so: the H100-native (sm_90a) replacement for the
  * TensorFlow ops that wizyoung/YOLOv3_TensorFlow's hot path builds its graph from.
  *
  * The reference has no FFI layer of its own (it is pure Python over TensorFlow), so
@@ -45,7 +45,7 @@ typedef enum yb_wlayout {
 
 int yb_version(void);
 const char* yb_last_error_string(void);
-/* Runtime switches for A/B experiments and tests (DESIGN.md 5b: "YB_CONV_MODE", "YB_CONV_EPI", ...).  The table is
+/* Runtime switches for A/B experiments and tests (DESIGN.md 5b: "YB_HALO", "YB_STEM_FUSE", ...).  The table is
  * seeded once from the equally named environment variables when the library is first used; afterwards only
  * yb_set_option() changes it (value NULL or "" = default).  No entry point calls getenv() on its own. */
 int yb_set_option(const char* key, const char* value);
@@ -84,14 +84,11 @@ typedef struct yb_conv_desc {
  *   out      [n,ho,wo,out_ld] (or the 2x-upsampled buffer)
  *   stat_sum/stat_sqsum nullable float32 [cout_pad]: when given, the per-channel sum and sum of squares of
  *            the raw convolution result (before scale/shift) are atomically accumulated (BN batch statistics).
- * Requires cin % 32 == 0 (the 3-channel stem has its own entry point).  tcgen05 implicit GEMM. */
+ * Requires cin % 32 == 0 (the 3-channel stem has its own entry point).  wgmma implicit GEMM. */
 int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
                   const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,
                   void* stream);
 int yb_conv_cout_pad(int cout);
-/* Profiling aid (tools/conv_trace.py): convs prepared after this call make CTA 0 stamp clock64 at its pipeline events
- * into buf ([10 warps][64 tile iterations][32 slots] + 2 int64, device memory, caller-zeroed); NULL switches it off. */
-int yb_debug_set_conv_trace(long long* buf);
 
 /* First layer (darknet53_body/Conv, 3->32, 3x3 s1; utils/layer_utils.py:35): float32 NHWC image in,
  * `dtype` NHWC out.  w is OHWI float32 [32,3,3,3]. */
@@ -160,7 +157,7 @@ int yb_bn_fold(const float* gamma, const float* beta, const float* mean, const f
 /* dw[cout, k*k*cin] (fp32, OHWI, ACCUMULATED) += sum over output pixels of dz[p,co] * im2col(x)[p,(r,s,ci)].
  * d describes the FORWARD conv (n,h,w,cin,cout,ksize,stride,in_ld,dtype); x is its input activation,
  * dz [n*ho*wo, dz_ld] the gradient w.r.t. its raw output; dz_dilated=1: dz is stored zero-inserted in an
- * [n, 2ho, 2wo, dz_ld] buffer (what the stride-2 dgrad consumes).  tcgen05, MN-major operands, split over pixels. */
+ * [n, 2ho, 2wo, dz_ld] buffer (what the stride-2 dgrad consumes).  wgmma, MN-major operands, split over pixels. */
 int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void* dz, int dz_ld, int dz_dilated, float* dw,
                     void* stream);
 /* wgrad of the 3-channel stem: x float32 [n,h,w,3], dz [n*h*w, 32] 16-bit -> dw [32,3,3,3] accumulated. */

@@ -13,12 +13,12 @@ PARITY PINNING STATUS
   * The TensorFlow *kernels* underneath (conv2d, fused batch-norm,
     non_max_suppression, sigmoid_cross_entropy_with_logits, autodiff) are an
     un-vendored third-party dependency (``tensorflow >= 1.8.0`` unpinned,
-    /root/reference/README.md:24) that cannot be installed here (Python 3.12, no
+    the reference's README.md:24) that cannot be installed here (Python 3.12, no
     network): for those this oracle restates TF's published semantics
     (SURVEY.md Appendix B) and is **parity unpinned**.
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference).
+the reference checkout).
 """
 from __future__ import annotations
 
@@ -260,7 +260,7 @@ def forward(x_nhwc, params, class_num=80, is_training=False, emulate=None, bn_de
 
     emulate in {None,'fp16','bf16'}: round the network input, every conv weight and
     every BN-conv output to that storage type (fp32 accumulate) — the storage model
-    of the B200 engine; detection-head outputs stay fp32.
+    of the GPU engine; detection-head outputs stay fp32.
     Returns numpy arrays (or torch tensors, keeping the autograd graph, if as_torch).
     If is_training, also returns the list of updated (moving_mean, moving_var).
     """

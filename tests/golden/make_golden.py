@@ -1,7 +1,7 @@
 """Generate tests/golden/*.npz by running the REFERENCE'S OWN Python sources
-(/root/reference/model.py, utils/layer_utils.py, utils/nms_utils.py,
+(the reference's model.py, utils/layer_utils.py, utils/nms_utils.py,
 utils/data_utils.py, utils/misc_utils.py) over the numpy-backed TensorFlow shim
-(tf_shim.py).  Run in the build container only (the GPU box has no /root/reference):
+(tf_shim.py).  Needs a checkout of the reference ($YOLOV3_TF_REFERENCE), not a GPU:
 
     python tests/golden/make_golden.py
 
@@ -27,13 +27,15 @@ from tests.synth import gen_inputs, gen_fms  # noqa: E402
 from oracle import yolov3_oracle as O  # noqa: E402  (parameter/input generators + TF-kernel restatement of NMS)
 
 tf, slim = tf_shim.install(nms_fn=O.tf_nms_cpu)
-sys.path.insert(0, "/root/reference")
+# a checkout of wizyoung/YOLOv3_TensorFlow, named by $YOLOV3_TF_REFERENCE
+REF = os.environ["YOLOV3_TF_REFERENCE"]
+sys.path.insert(0, REF)
 import model as ref_model  # noqa: E402
 from utils import nms_utils as ref_nms  # noqa: E402
 from utils import data_utils as ref_data  # noqa: E402
 from utils import misc_utils as ref_misc  # noqa: E402
 
-ANCHORS = ref_misc.parse_anchors("/root/reference/data/yolo_anchors.txt")
+ANCHORS = ref_misc.parse_anchors(os.path.join(REF, "data", "yolo_anchors.txt"))
 assert np.array_equal(ANCHORS, O.COCO_ANCHORS)
 
 

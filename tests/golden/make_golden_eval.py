@@ -16,7 +16,9 @@ if "Inf" not in np.__dict__:
     np.Inf = np.inf                      # the reference predates NumPy 2 (utils/eval_utils.py:376 uses np.Inf)
 from oracle import yolov3_oracle as O  # noqa: E402
 from tests.synth import gen_eval_case  # noqa: E402
-sys.path.insert(0, "/root/reference")
+# a checkout of wizyoung/YOLOv3_TensorFlow, named by $YOLOV3_TF_REFERENCE
+REF = os.environ["YOLOV3_TF_REFERENCE"]
+sys.path.insert(0, REF)
 from utils import eval_utils as ref  # noqa: E402
 
 NMS = dict(max_boxes=20, score_thresh=0.3, nms_thresh=0.45)

@@ -13,10 +13,12 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.modules.setdefault("tensorflow", types.ModuleType("tensorflow"))       # utils/*.py import it at module level
-sys.path.insert(0, "/root/reference")
+# a checkout of wizyoung/YOLOv3_TensorFlow, named by $YOLOV3_TF_REFERENCE
+REF = os.environ["YOLOV3_TF_REFERENCE"]
+sys.path.insert(0, REF)
 from utils import data_aug, data_utils  # noqa: E402
 
-ANCHORS = np.reshape(np.asarray(open("/root/reference/data/yolo_anchors.txt").read().split(","), np.float32), [-1, 2])
+ANCHORS = np.reshape(np.asarray(open(os.path.join(REF, "data", "yolo_anchors.txt")).read().split(","), np.float32), [-1, 2])
 
 
 def main():

@@ -1,5 +1,5 @@
 """A numpy/torch-CPU backed stand-in for the handful of `tensorflow` 1.x symbols that
-/root/reference/{model.py,utils/layer_utils.py,utils/nms_utils.py,utils/misc_utils.py,
+the reference's {model.py,utils/layer_utils.py,utils/nms_utils.py,utils/misc_utils.py,
 utils/data_utils.py} touch, so that the reference's *own Python sources* can be
 executed in this container (TensorFlow itself is not installable here).
 

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 implicit-GEMM conv and the stem, through the C ABI
+"""GPU parity tests of the wgmma implicit-GEMM conv and the stem, through the C ABI
 (yb_conv2d_fwd / yb_stem_conv_fwd).  Reference: plain PyTorch fp32 conv2d on the same
 fp16/bf16-rounded operands.  Tolerance: fp32-accumulation-order noise + one output
 rounding: |err| <= 2^-9 * max(1, |ref|) for fp16 storage (2^-6 for bf16)."""
@@ -14,13 +14,11 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(params=["1cta", "2cta", "mc", "1cta-reg", "2cta-reg", "1cta-eg1", "2cta-eg1", "1cta-eg2", "2cta-eg2"], autouse=True)
 def conv_mode(request):
-    """Every conv test runs against the three tcgen05 kernels: cta_group::1 (128-row tiles), cta_group::2 (a CTA
-    pair per 256-row tile) and the cluster-multicast pair kernel (2x2 / 2x1 pairs; only 256-wide tiles take it,
-    the other shapes fall back to the plain pair kernel), and — for the first two — against both epilogues: the
-    TMA-store / TMA-residual one (default) and the register-store one of round 1 ("-reg"), and with one ("-eg1") or —
-    wherever a kernel exists — two ("-eg2") groups of epilogue warps (the default picks two for 1x1 and Cin <= 64
-    layers).  The library's option
-    table (yb_set_option) overrides the heuristics; it is restored after each test."""
+    """Every conv test runs against the kernel variants: one CTA per tile ("1cta", the default), clusters of 2 CTAs
+    sharing a TMA-multicast weight tile ("2cta") and clusters of 4 ("mc"); for the first two also against the
+    register-store epilogue ("-reg", instead of the shared-memory staging tile) and with one ("-eg1", 64-row tiles) or
+    two ("-eg2", 128-row tiles, the default) consumer warpgroups doing MMA + epilogue.  The library's option table
+    (yb_set_option) selects the variant; it is restored after each test."""
     L = _lib()
     mode, _, epi = request.param.partition("-")
     L.set_option("YB_CONV_MODE", "2cta" if mode == "mc" else mode)
@@ -191,7 +189,7 @@ def test_conv1x1_residual_tail_rows_many_chunks():
 
 
 def test_conv3x3_many_tiles_per_cta_residual():
-    _run_conv(8, 52, 52, 64, 128, 3, 1, residual=True)                  # 169 m-tiles on <= 148 CTAs: residual prefetch across tiles
+    _run_conv(8, 52, 52, 64, 128, 3, 1, residual=True)                  # 169 m-tiles on <= 132 CTAs: persistent CTAs take several tiles
 
 
 def test_conv1x1_cout32_single_chunk():
@@ -253,7 +251,7 @@ def test_pack_weights_layouts():
 ])
 def test_conv3x3_thin(n, h, w, cout, s, res, dtype, conv_mode):
     if conv_mode != "1cta":
-        pytest.skip("independent of the tcgen05 kernel mode")
+        pytest.skip("independent of the igemm kernel variant")
     L = _lib()
     g = torch.Generator().manual_seed(11)
     cin = 32
@@ -284,7 +282,7 @@ def test_conv3x3_thin(n, h, w, cout, s, res, dtype, conv_mode):
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 def test_stem_conv_tensor_core(dtype, conv_mode):
     if conv_mode != "1cta":
-        pytest.skip("independent of the tcgen05 kernel mode")
+        pytest.skip("independent of the igemm kernel variant")
     L = _lib()
     g = torch.Generator().manual_seed(3)
     n, h, w = 2, 40, 56
@@ -329,7 +327,7 @@ def test_stem_conv_tensor_core(dtype, conv_mode):
     torch.testing.assert_close(ssq.double() - 2.0, (of * of).sum(dim=(0, 1, 2)), rtol=1e-4, atol=1e-2)
 
 
-# ------------------------------------------------------------------------- halo-tile tcgen05 conv (csrc/conv_halo.cu)
+# ------------------------------------------------------------------------- halo-tile wgmma conv (csrc/conv_halo.cu)
 @pytest.mark.parametrize("n,h,w,cin,cout,s,res,dtype", [
     (2, 32, 16, 64, 128, 1, False, torch.float16),      # exact tiles
     (2, 32, 16, 32, 64, 1, True, torch.float16),
@@ -345,7 +343,7 @@ def test_stem_conv_tensor_core(dtype, conv_mode):
 ])
 def test_conv3x3_halo(n, h, w, cin, cout, s, res, dtype, conv_mode):
     if conv_mode != "1cta":
-        pytest.skip("independent of the igemm kernel selection")
+        pytest.skip("independent of the igemm kernel variant")
     _run_conv(n, h, w, cin, cout, 3, s, dtype=dtype, residual=res, halo=True)
     _run_conv(n, h, w, cin, cout, 3, s, dtype=dtype, residual=res, halo=True, in_extra=16, out_extra=32, seed=3)
 
@@ -368,7 +366,7 @@ def test_stem_conv1_fused(n, h, w, dtype, conv_mode):
     separate launches (stem kernel, then Conv_1 on its 16-bit output) and against fp32 convs on the same rounded
     operands: image borders (the stem's SAME padding AND Conv_1's pad-1), partial bottom tiles, both storage types."""
     if conv_mode != "1cta":
-        pytest.skip("independent of the igemm kernel selection")
+        pytest.skip("independent of the igemm kernel variant")
     L = _lib()
     lib, check, ptr, st = L.lib, L.check, L.ptr, L.stream_handle
     g = torch.Generator(device="cpu").manual_seed(5 + h)

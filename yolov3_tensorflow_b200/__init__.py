@@ -1,6 +1,6 @@
 """yolov3_tensorflow_b200 — the YOLOv3 hot path of wizyoung/YOLOv3_TensorFlow
 (model.yolov3.forward/predict, utils.nms_utils.gpu_nms, the darknet weight loader) on
-hand-written sm_100a CUDA kernels behind a C ABI (libyolob200.so, include/yolob200.h).
+hand-written sm_90a CUDA kernels behind a C ABI (libyolob200.so, include/yolob200.h).
 
 Importing the package loads the shared library; it fails loudly if it has not been built.
 """

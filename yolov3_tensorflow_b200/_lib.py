@@ -54,7 +54,6 @@ _SIGS = {
     "yb_device_info": ([C.POINTER(i32)] * 3, i32),
     "yb_conv2d_fwd": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp], i32),
     "yb_conv_cout_pad": ([i32], i32),
-    "yb_debug_set_conv_trace": ([vp], i32),
     "yb_stem_conv_fwd": ([vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
     "yb_conv3x3_thin_fwd": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp], i32),
     "yb_conv3x3_halo_supported": ([C.POINTER(ConvDesc)], i32),

@@ -17,6 +17,24 @@
 
 namespace yb {
 
+// Batch statistics -> (mean, biased var, invstd, scale, shift) and the moving-statistics update.  Shared by the
+// finalize kernel and the fused statistics + apply kernel, which must agree bit for bit: every product and sum is
+// rounded explicitly, so no FMA contraction the compiler may pick differently in the two contexts changes a result.
+__device__ __forceinline__ void bn_batch_coeffs(float su, float sq, float count, float ga, float be, float eps, float& mean,
+                                                float& var, float& invstd, float& sc, float& sh) {
+  mean = __fdiv_rn(su, count);
+  var = fmaxf(__fsub_rn(__fdiv_rn(sq, count), __fmul_rn(mean, mean)), 0.f);   // biased
+  invstd = rsqrtf(__fadd_rn(var, eps));
+  sc = __fmul_rn(ga, invstd);
+  sh = __fsub_rn(be, __fmul_rn(mean, sc));
+}
+__device__ __forceinline__ void bn_moving_update(float& mm, float& mv, float mean, float var, float count, float decay) {
+  const float unb = count > 1.f ? __fdiv_rn(__fmul_rn(var, count), __fsub_rn(count, 1.f)) : var;   // unbiased
+  const float keep = __fsub_rn(1.f, decay);
+  mm = __fadd_rn(__fmul_rn(mm, decay), __fmul_rn(keep, mean));
+  mv = __fadd_rn(__fmul_rn(mv, decay), __fmul_rn(keep, unb));
+}
+
 __global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* __restrict__ sqsum, float count, int c,
                                    const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                    float decay, float* moving_mean, float* moving_var, float* scale, float* shift,
@@ -34,20 +52,13 @@ __global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* _
     save_invstd[i] = invstd;
     return;
   }
-  const float mean = sum[i] / count;
-  float var = sqsum[i] / count - mean * mean;   // biased
-  var = fmaxf(var, 0.f);
-  const float invstd = rsqrtf(var + eps);
-  const float sc = gamma[i] * invstd;
+  float mean, var, invstd, sc, sh;
+  bn_batch_coeffs(sum[i], sqsum[i], count, gamma[i], beta[i], eps, mean, var, invstd, sc, sh);
   scale[i] = sc;
-  shift[i] = beta[i] - mean * sc;
+  shift[i] = sh;
   save_mean[i] = mean;
   save_invstd[i] = invstd;
-  if (moving_mean) {
-    const float unb = count > 1.f ? var * count / (count - 1.f) : var;
-    moving_mean[i] = moving_mean[i] * decay + (1.f - decay) * mean;
-    moving_var[i] = moving_var[i] * decay + (1.f - decay) * unb;
-  }
+  if (moving_mean) bn_moving_update(moving_mean[i], moving_var[i], mean, var, count, decay);
 }
 
 struct RowGeom {
@@ -108,7 +119,7 @@ __device__ __forceinline__ long up_row(long r, int h, int w) {
 
 // ---- streaming kernels: thread = (CPT-channel vector, row lane); per-channel coefficients live in registers, rows are
 // ---- walked R at a time so several vector loads are in flight per thread.
-// Launch shape (profiles/r02_d_kernels_train.md): ONE balanced wave of 148 x BPS co-resident blocks.  The first version
+// Launch shape: ONE balanced wave of (SM count) x BPS co-resident blocks.  The first version
 // launched 4 blocks per SM with 3 resident (a 1/3-occupancy tail wave on the large layers: 0.6 of the HBM peak), spilled
 // (85-register cap against 40 coefficient registers) and fetched the per-channel coefficients with 56 scalar loads per
 // thread whose 32-byte stride makes every warp instruction touch 32 sectors — on the 13x13 / 26x26 layers, where a
@@ -187,14 +198,12 @@ bn_act_apply_kernel(const T* __restrict__ z, long z_ld, const float* __restrict_
       float su[CPT], sq[CPT];
       ldc<CPT>(f.sum + c0, vec, su); ldc<CPT>(f.sqsum + c0, vec, sq);
 #pragma unroll
-      for (int j = 0; j < CPT; ++j) {
-        mean[j] = su[j] / f.count;
-        var[j] = fmaxf(sq[j] / f.count - mean[j] * mean[j], 0.f);   // biased
-        invstd[j] = rsqrtf(var[j] + f.eps);
-      }
+      for (int j = 0; j < CPT; ++j) bn_batch_coeffs(su[j], sq[j], f.count, ga[j], be[j], f.eps, mean[j], var[j], invstd[j], sc[j], sh[j]);
     }
+    if (f.sum == nullptr) {
 #pragma unroll
-    for (int j = 0; j < CPT; ++j) { sc[j] = ga[j] * invstd[j]; sh[j] = be[j] - mean[j] * sc[j]; }
+      for (int j = 0; j < CPT; ++j) { sc[j] = ga[j] * invstd[j]; sh[j] = be[j] - mean[j] * sc[j]; }
+    }
     if (blockIdx.x == 0 && lane_r == 0) {
       stc<CPT>(f.scale + c0, vec, sc); stc<CPT>(f.shift + c0, vec, sh);
       stc<CPT>(f.save_mean + c0, vec, mean); stc<CPT>(f.save_invstd + c0, vec, invstd);
@@ -202,11 +211,7 @@ bn_act_apply_kernel(const T* __restrict__ z, long z_ld, const float* __restrict_
         float mm[CPT], mv[CPT];
         ldc<CPT>(f.moving_mean + c0, vec, mm); ldc<CPT>(f.moving_var + c0, vec, mv);
 #pragma unroll
-        for (int j = 0; j < CPT; ++j) {
-          const float unb = f.count > 1.f ? var[j] * f.count / (f.count - 1.f) : var[j];
-          mm[j] = mm[j] * f.decay + (1.f - f.decay) * mean[j];
-          mv[j] = mv[j] * f.decay + (1.f - f.decay) * unb;
-        }
+        for (int j = 0; j < CPT; ++j) bn_moving_update(mm[j], mv[j], mean[j], var[j], f.count, f.decay);
         stc<CPT>(f.moving_mean + c0, vec, mm); stc<CPT>(f.moving_var + c0, vec, mv);
       }
     }
@@ -269,7 +274,7 @@ bn_bwd_reduce_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__
   const int cvi = threadIdx.x % sg.cv, lane_r = threadIdx.x / sg.cv;
   const int c0 = cvi * CPT;
   // per-channel coefficients live in registers (the first version re-loaded four of them per ELEMENT through the LSU,
-  // which made this kernel 2x slower than bn_bwd_apply on the same data: profiles/r01_k).  The invstd factor of
+  // which made this kernel 2x slower than bn_bwd_apply on the same data).  The invstd factor of
   // zhat = (z - mean) * invstd is folded in once per block at the end.
   float sc[CPT], sh[CPT];
   ldc<CPT>(scale + c0, vec, sc); ldc<CPT>(shift + c0, vec, sh);
@@ -398,7 +403,7 @@ bn_bwd_apply_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__ 
   }
 }
 
-// one balanced wave: at most 148 x bps co-resident blocks, every row lane of a block gets >= 1 row
+// one balanced wave: at most (SM count) x bps co-resident blocks, every row lane of a block gets >= 1 row
 static StreamGeom stream_geom(long rows, int c, int cpt, int bps, int* grid) {
   StreamGeom sg;
   sg.cv = c / cpt;
@@ -415,9 +420,8 @@ static int aligned16(std::initializer_list<const void*> ps) {
   for (const void* q : ps) if (q && (reinterpret_cast<uintptr_t>(q) & 15)) return 0;
   return 1;
 }
-// kernel shape: 8 channels per thread (16-byte accesses) unless YB_BN_CPT=4.  Measured (tools/bn_probe.py, profiles/
-// r02_g_bn_probe.md): CPT 8 streams the large layers at 4.9-5.9 TB/s against 2.9-4.7 TB/s for CPT 4, whose 8-byte
-// accesses double the load/store instructions per byte; on the 13x13 layers the two are within a microsecond.
+// kernel shape: 8 channels per thread (16-byte accesses) unless YB_BN_CPT=4, whose 8-byte accesses double the
+// load/store instructions per byte.
 static int bn_cpt(int c) {
   const char* o = opt("YB_BN_CPT");
   if (c > 1024 || c < 32) return 8;

@@ -26,11 +26,11 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
 int num_sms() {                       // of the CURRENT device (cached per device ordinal)
   static int sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int& s = sms[dev & 63];
   if (s == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     s = v;
   }
   return s;
@@ -52,10 +52,9 @@ int ensure_smem_attr(DeviceOnce& once, const void* kernel, int bytes) {
 // ---- runtime switches (A/B experiments and tests only; DESIGN.md 5b).  Seeded ONCE from the YB_* environment
 // ---- variables, changed afterwards only through yb_set_option(): no getenv() on any call path.
 struct Opt { const char* key; char val[32]; };
-static Opt g_opts[] = {{"YB_CONV_MODE", ""}, {"YB_CONV_MC", ""}, {"YB_CONV_DBG", ""}, {"YB_CONV_BRES", ""},
-                       {"YB_CONV_KPS", ""}, {"YB_CONV_EPI", ""}, {"YB_THIN", ""}, {"YB_STEM_DBG", ""},
+static Opt g_opts[] = {{"YB_CONV_MODE", ""}, {"YB_CONV_MC", ""}, {"YB_CONV_EPI", ""}, {"YB_CONV_EG", ""}, {"YB_THIN", ""}, {"YB_STEM_DBG", ""},
                        {"YB_STEM_WGRAD", ""}, {"YB_WGRAD_TP", ""}, {"YB_DGRAD_S2", ""},
-                       {"YB_HALO", ""}, {"YB_CONV_EG", ""}, {"YB_STEM_FUSE", ""}, {"YB_STEM_WARPS", ""}, {"YB_STEM_EPIG", ""}, {"YB_HALO_DIRECT", ""},
+                       {"YB_HALO", ""}, {"YB_STEM_FUSE", ""},
                        {"YB_BN_CPT", ""}, {"YB_BN_FIN", ""}, {"YB_PACK_MT", ""}, {"YB_WGRAD_EPI", ""}, {"YB_STEM_TRAIN", ""}, {"YB_WGRAD_STREAM", ""}, {"YB_STEM_SPLIT", ""}, {"YB_HEAD_STREAM", ""}};
 static std::once_flag g_opt_once;
 static void seed_opts() {

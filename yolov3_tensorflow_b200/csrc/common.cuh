@@ -1,6 +1,6 @@
-// Common device/host helpers for the sm_100a kernels: error plumbing for the C-ABI,
+// Common device/host helpers for the sm_90a kernels: error plumbing for the C-ABI,
 // and thin inline-PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor) and
-// tcgen05 (TMEM alloc / UMMA / commit / ld).  No CUTLASS: everything is spelled out.
+// wgmma (descriptors / fence / commit / wait).  No CUTLASS: everything is spelled out.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -118,14 +118,12 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must trap (kernel fault) instead of hanging the GPU.
+// Bounded wait: a protocol bug must trap (kernel fault) instead of hanging the GPU.  (No printf here: a function call
+// inside a wgmma main loop makes ptxas serialise every wgmma of the kernel.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("yolob200: mbarrier wait timeout (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 
@@ -168,151 +166,18 @@ __device__ __forceinline__ void bulk_wait_group() {        // at most N most-rec
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---- tcgen05 / TMEM ----
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T ; one thread issues
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread t of the warp gets row (lane base + t), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- 2-CTA (cta_group::2) variants: a CTA pair in a cluster drives one 256-row UMMA ----
+// ---- clusters: TMA multicast, cluster-wide barrier, remote mbarrier arrive ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
+__device__ __forceinline__ void cluster_sync_all() {   // every thread of every CTA of the cluster
+  __syncwarp();
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // shared::cluster address -> same offset in the even CTA of the pair
-// TMA loads issued by BOTH CTAs of the pair; the transaction bytes are credited to the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_im2col_4d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c, int w,
-                                                       int h, int n, uint16_t ow, uint16_t oh) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c), "r"(w),
-      "r"(h), "r"(n), "h"(ow), "h"(oh)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem) {  // whole warp, same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior MMAs of this thread retired) on the barrier at the same offset in both CTAs
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// ---- cluster multicast variants (cta_group::2 + .multicast::cluster): the box lands at the same smem offset in
-// ---- every CTA of `mask`, and each destination's bytes are credited to ITS pair leader's barrier
-__device__ __forceinline__ void tma_load_2d_2sm_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                   uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "h"(mask), "r"(c0),
-      "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_im2col_4d_2sm_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c, int w,
-                                                          int h, int n, uint16_t ow, uint16_t oh, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5, %6, %7}], [%2], {%8, %9}, %3;"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "h"(mask), "r"(c),
-      "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mask(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// arrive on the barrier at the same offset in CTA `cta` of the cluster
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n"
@@ -323,27 +188,48 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta)
       "r"(cta)
       : "memory");
 }
+// the box lands at the same shared-memory offset in every CTA of `mask`; each destination's bytes are credited to the
+// barrier at the same offset in that CTA
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5}], [%2], %3;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
+      : "memory");
+}
 
-// UMMA shared-memory matrix descriptor for a K-major tile whose rows are exactly one
-// swizzle span wide (64 x 16-bit = 128 B for SWIZZLE_128B, 32 x 16-bit = 64 B for
-// SWIZZLE_64B): 8-row groups are `sbo` bytes apart.  Field layout (PTX ISA "shared
-// memory descriptor", same as cute::UMMA::SmemDescriptor): [0,14) addr>>4, [16,30)
-// LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) layout (2 = 128B, 4 = 64B swizzle).
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
+// ---- wgmma (warpgroup MMA, operands in shared memory, fp32 accumulators in registers) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {   // at most N most-recent wgmma groups of this thread still pending
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int K>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// named barrier over the 128 threads of one warpgroup (ids 1.. : 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// wgmma shared-memory matrix descriptor (PTX ISA "matrix descriptor format"): [0,14) addr>>4, [16,30) LBO>>4,
+// [32,46) SBO>>4, [62,64) layout (1 = 128B, 2 = 64B swizzle).  The swizzle is a function of the shared-memory address
+// bits, so a descriptor may start at any 16-byte-aligned row of a tile the TMA wrote with the same swizzle.
+// K-major tiles whose rows are one swizzle span wide: SBO = bytes between 8-row groups (LBO unused).
+// MN-major tiles: LBO = bytes between 64 / 32-element MN blocks, SBO = bytes between 8-row K groups.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;                        // LBO (unused for swizzled K-major; canonical value 1)
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;                        // descriptor version (Blackwell)
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)(swizzle_bytes == 128 ? 1 : 2) << 62;
   return d;
 }
-// UMMA instruction descriptor, kind::f16, fp32 accumulate, A and B K-major.
-// [4,6) D fmt (1=f32), [7,10) A fmt, [10,13) B fmt (0=f16, 1=bf16), [15] A major, [16] B major,
-// [17,23) N>>3, [24,29) M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, int is_bf16) {
-  return (1u << 4) | ((uint32_t)is_bf16 << 7) | ((uint32_t)is_bf16 << 10) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t swizzle_bytes) {
+  return make_smem_desc(saddr, 16, sbo_bytes, swizzle_bytes);
 }
 #endif  // __CUDACC__
 

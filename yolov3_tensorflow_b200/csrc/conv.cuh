@@ -13,12 +13,9 @@ struct ConvParams {
   int kh, kw;             // filter window (ksize x ksize for the forward convs; 1x1 .. 2x2 for the stride-2 dgrad classes)
   int scatter;            // 0, or 1 + 2a + b: output pixel (p, q) is stored at (2p + a, 2q + b) of a [n, 2P, 2Q] grid
   int im2col;             // 1: A via im2col TMA, 0: A via 2D tiled TMA
-  int two_cta;            // 1: cta_group::2 kernel (256-row tiles per CTA pair)
-  int b_resident;         // 1-CTA kernel: the whole [BN, K] weight tile stays in shared memory (single n-tile, fits)
-  int epi_groups;         // 1 | 2 sets of four epilogue warps (2: two tiles' epilogues run concurrently; short-K layers)
-  int kps;                // 1-CTA kernel: k-blocks per barrier phase (one empty/full handshake per kps k-blocks)
-  int dbg;                // timing experiments only (YB_CONV_DBG bitmask: 1 skip A loads, 2 skip B loads, 4 skip MMAs)
-  int mc_m, mc_n;         // cluster of mc_m x mc_n pairs with TMA multicast (1,1: plain pair kernel)
+  int consumers;          // consumer warpgroups per CTA: 64 output rows each (1 | 2)
+  int cluster;            // CTAs per cluster sharing one multicast weight tile (1 | 2 | 4)
+  int epi_reg;            // 1: accumulator fragments stored straight from registers (no staging tile)
   int num_m_tiles, num_n_tiles;
   const float* scale;     // [cout_pad]
   const float* shift;     // [cout_pad]
@@ -29,11 +26,7 @@ struct ConvParams {
   int out_fp32, leaky, upsample;
   float* stat_sum;        // nullable: BN batch statistics of the raw conv result
   float* stat_sqsum;
-  int epi_tma;            // 1: 16-bit output tiles leave through shared memory + TMA stores (tmO), the residual comes in by TMA (tmR)
-  CUtensorMap tmO;        // [M, cout] view of the output slice, box 32 rows x 32 channels, SWIZZLE_64B
-  CUtensorMap tmR;        // same view of the residual
   DetParams det;          // det.on: decode + NMS candidate filter instead of the fp32 feature-map store (detection heads)
-  long long* trace;       // debugging only (yb_debug_set_conv_trace): CTA 0 stamps clock64 at its pipeline events, else NULL
 };
 
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
@@ -65,7 +58,6 @@ struct HaloParams {
   const float* stem_scale;     // [32]
   const float* stem_shift;     // [32]
   int in_h, in_w;              // image size (= the stem's output size)
-  int direct;                  // 1: direct 256-bit register stores (no residual, 32-byte aligned dense rows)
 };
 bool conv_halo_supported(const yb_conv_desc* d);
 int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,

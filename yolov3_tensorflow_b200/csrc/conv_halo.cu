@@ -4,20 +4,21 @@
 //
 // Why: with 32 / 64 input channels an im2col row is 64 / 128 bytes and one k-block is one filter tap, so the generic
 // implicit-GEMM kernel (conv_igemm.cu) issues 9 TMA requests of 128 rows per 128-pixel tile — every input pixel is
-// fetched 9x from L2, the TMA row rate (not bandwidth, not the MMA) paces the layer, and these five layers cost 1.4 ms
-// of a 6.2 ms step (profiles/r02_b) against a ~0.5 ms HBM bound.  Here:
-//   * a tile is 16 x 8 output pixels (UMMA M = 128: sixteen 8-row groups, group g = output row g);
+// fetched 9x from L2 and the TMA row rate (not bandwidth, not the MMA) paces the layer.  Here:
+//   * a tile is 16 x 8 output pixels (M = 128: sixteen 8-row groups, group g = output row g; two consumer warpgroups
+//     own output rows 0..7 and 8..15 and issue wgmma m64nCOUTk16);
 //   * stride 1: ONE tiled TMA load brings the (16+2) x (8+2) input halo [18][10][Cin] into shared memory (borders and
 //     the bottom tail zero-filled by the TMA), 1.4x instead of 9x the tile's pixels;
 //     stride 2: four loads with traversal stride 2 bring the four (row, col)-parity planes of the 33 x 17 halo, so
 //     that every tap again reads a dense window of one plane;
-//   * tap (r, s) needs NO data movement: its A operand is the same shared-memory tile, addressed by a UMMA descriptor
+//   * tap (r, s) needs NO data movement: its A operand is the same shared-memory tile, addressed by a wgmma descriptor
 //     that starts (dr * plane_width + ds) rows further down and uses the plane width as the 8-row-group stride (SBO).
 //     The 128B / 64B swizzle is a function of the shared-memory address bits, so a descriptor may start at any row of
-//     a TMA-written tile (tools/probes/umma_shift_probe.cu, profiles/r01_j_umma_shift_probe.txt);
+//     a TMA-written tile;
 //   * all 9 taps' weights [Cout][9 * Cin] stay resident in shared memory for the whole persistent CTA;
-//   * the epilogue is the staging-tile + coalesced-store one of conv_igemm.cu, with pixel (not row) addressing.
-// Warp roles: warp 0 TMA producer, warp 1 MMA issuer, warps 2..5 epilogue; accumulators double-buffered in TMEM.
+//   * the epilogue is the staging-tile one of conv_igemm.cu, with pixel (not row) addressing.
+// Warp roles: warp 0 TMA producer, warps 4..11 (warpgroups 1, 2) MMA + epilogue, fp32 accumulators in registers; the
+// producer keeps up to NST halo tiles in flight ahead of the MMAs.
 // Inference only (folded BN): scale/shift + leaky + optional residual, 16-bit NHWC in and out.
 #include <cudaTypedefs.h>
 #include <string.h>
@@ -26,6 +27,7 @@
 
 #include "common.cuh"
 #include "conv.cuh"
+#include "wgmma.cuh"
 
 namespace yb {
 
@@ -36,7 +38,8 @@ int make_tmap_tiled4d(CUtensorMap* tm, const void* base, int dtype, int n, int h
                       int box_w, int box_h, int estride);
 
 static constexpr int HT_H = 16, HT_W = 8;       // output tile
-static constexpr int HALO_THREADS = 192;
+static constexpr int HALO_THREADS = 384;         // warp 0: TMA, warpgroups 1, 2: MMA + epilogue
+static constexpr int HALO_EPI_LD = 33;          // staging row pitch in floats
 
 template <int CIN, int COUT, int STRIDE>
 struct HaloCfg {
@@ -52,15 +55,14 @@ struct HaloCfg {
                                               : (ph(0) * pw(0) + ph(1) * pw(1) + ph(2) * pw(2) + ph(3) * pw(3)) * ROWB;
   static constexpr int B_TAP_BYTES = COUT * ROWB;                        // one tap's [COUT][CIN] weight tile
   static constexpr int B_BYTES = 9 * B_TAP_BYTES;
-  static constexpr int EPI_BYTES = 4 * 2 * 2048;                         // 4 warps x 2 staging tiles of [32][32] 16-bit
-  static constexpr int MISC_BYTES = 1024;                                // barriers, TMEM slot, scale / shift
+  static constexpr int EPI_BYTES = 2 * 64 * HALO_EPI_LD * 4;              // a [64][33] fp32 staging tile per consumer warpgroup
+  static constexpr int MISC_BYTES = 1024;                                // barriers
   static constexpr int BUDGET = 227 * 1024 - 1024 /*alignment slack*/;
   static constexpr int NST_RAW = (BUDGET - B_BYTES - EPI_BYTES - MISC_BYTES - 2 * COUT * 4) / STAGE_BYTES;
   static constexpr int NST = NST_RAW > 6 ? 6 : NST_RAW;
   static_assert(NST >= 1, "halo conv: configuration does not fit shared memory");
   static constexpr int SMEM_BYTES = 1024 + B_BYTES + NST * STAGE_BYTES + EPI_BYTES + MISC_BYTES + 2 * COUT * 4;
-  static constexpr int TMEM_COLS = 2 * COUT;                             // 128 or 256
-  static constexpr uint32_t SWIZZLE = CIN == 64 ? 2u : 4u;               // UMMA layout_type: 128B / 64B
+  static constexpr uint32_t SWIZZLE = ROWB;                              // 128B / 64B: a pixel row is one swizzle span
   // tap (r, s) -> plane and row/col offset inside it.  stride 2 (pad 1 + VALID): input row 2i + r - 1:
   //   r = 0 -> odd-row plane, offset 0; r = 1 -> even-row plane, offset 0; r = 2 -> odd-row plane, offset 1
   static constexpr int tap_plane(int r, int s) { return STRIDE == 1 ? 0 : (((r == 1) ? 2 : 0) | ((s == 1) ? 1 : 0)); }
@@ -73,7 +75,7 @@ struct HaloCfg {
 // needed on 33 x 17 pixels; their 35 x 19-pixel float32 input halo arrives by one 3D TMA load, STEMW producer warps
 // compute the stem on mma.sync (m16n8k16: A = the 27 -> 32 patch values gathered straight from the halo, B = the stem
 // weights held in registers), apply BN + leaky and store the 16-bit results into the swizzled plane tiles the
-// tcgen05 descriptors of Conv_1 read.  Stem pixels outside the image are Conv_1's zero padding (utils/layer_utils.py:15-16).
+// wgmma descriptors of Conv_1 read.  Stem pixels outside the image are Conv_1's zero padding (utils/layer_utils.py:15-16).
 struct StemCfg {
   static constexpr int SH = 2 * HT_H + 1, SW = 2 * HT_W + 1;             // stem pixels per tile: 33 x 17
   static constexpr int NPX = SH * SW;                                     // 561
@@ -89,12 +91,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-// 256-bit global store (sm_100: STG.E.ENL2.256): one full 32-byte sector per lane
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
 }
 __device__ __forceinline__ void mma16816_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1, bool bf16) {
   if (bf16)
@@ -112,29 +108,22 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// EPIG = 2: a second group of four epilogue warps drains the other accumulator stage (tiles alternate between the groups);
-// it uses the DIRECT epilogue only (no residual, dense 32-byte aligned rows: every lane stores its pixel's chunk as two
-// 256-bit st.global — with out_ld = 64 a lane owns a whole 128-byte line — so the groups need no staging tiles).
-template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, int EPIG = 1>
-__global__ void __launch_bounds__(64 + 128 * EPIG + 32 * STEMW, 1)
+template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0>
+__global__ void __launch_bounds__(HALO_THREADS + 32 * STEMW, 1)
 conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ HaloParams p) {
   using C = HaloCfg<CIN, COUT, STRIDE>;
-  constexpr int NTHREADS = 64 + 128 * EPIG + 32 * STEMW;
-  constexpr int PROD_WARP0 = 2 + 4 * EPIG;       // first stem-producer warp
+  constexpr int PROD_WARP0 = HALO_THREADS / 32;  // first stem-producer warp
   static_assert(STEMW == 0 || (CIN == 32 && STRIDE == 2), "the fused stem feeds Conv_1 (32 -> 64, stride 2)");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // pointer arithmetic: stays in the shared space
   uint8_t* sB = smem;                                        // [9][COUT][CIN]   swizzled, resident
   uint8_t* sA = smem + C::B_BYTES;                           // [NST][planes]    swizzled halo tiles
-  uint8_t* sE = sA + C::NST * C::STAGE_BYTES;                // [4 warps][2][2 KB] epilogue staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sE + C::EPI_BYTES);
+  float* sE = reinterpret_cast<float*>(sA + C::NST * C::STAGE_BYTES);   // [2 warpgroups][64][HALO_EPI_LD] staging
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sE) + C::EPI_BYTES);
   uint64_t* full_bar = bars;            // [NST]
-  uint64_t* empty_bar = bars + 8;       // [NST]
-  uint64_t* tfull_bar = bars + 16;      // [2]
-  uint64_t* tempty_bar = bars + 18;     // [2]
+  uint64_t* empty_bar = bars + 8;       // [NST] one arrive per consumer warp
   uint64_t* b_bar = bars + 20;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 22);
-  float* s_ss = reinterpret_cast<float*>(sE + C::EPI_BYTES + C::MISC_BYTES);   // [2][COUT] scale / shift
+  float* s_ss = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sE) + C::EPI_BYTES + C::MISC_BYTES);   // [2][COUT] scale / shift
   uint64_t* in_full = bars + 24;        // [NIN] float32 input halo landed (TMA -> stem producers)
   uint64_t* in_empty = bars + 26;       // [NIN] stem producers -> TMA
   uint8_t* sIn = reinterpret_cast<uint8_t*>(s_ss + 2 * COUT);                  // [NIN][35][60] float32 (STEMW > 0 only; 128-byte aligned)
@@ -147,24 +136,19 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       for (int i = 0; i < C::NPLANE; ++i) tma_prefetch_desc(&maps.plane[i]);
     }
     tma_prefetch_desc(&maps.w);
-    for (int i = 0; i < C::NST; ++i) { mbar_init(&full_bar[i], STEMW > 0 ? STEMW : 1); mbar_init(&empty_bar[i], 1); }
+    for (int i = 0; i < C::NST; ++i) { mbar_init(&full_bar[i], STEMW > 0 ? STEMW : 1); mbar_init(&empty_bar[i], 8); }
     if (STEMW > 0) {
       tma_prefetch_desc(&maps.in3d);
       for (int i = 0; i < StemCfg::NIN; ++i) { mbar_init(&in_full[i], 1); mbar_init(&in_empty[i], STEMW); }
     }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
     mbar_init(b_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  for (int c = threadIdx.x; c < COUT; c += NTHREADS) {
+  for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_ss[c] = c < p.cout ? __ldg(p.scale + c) : 0.f;
     s_ss[COUT + c] = c < p.cout ? __ldg(p.shift + c) : 0.f;
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -210,43 +194,91 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         if (++stage == C::NST) { stage = 0; phase ^= 1; }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, COUT, std::is_same<T, __nv_bfloat16>::value);
-      const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-      mbar_wait(b_bar, 0);
-      int stage = 0, it = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&tempty_bar[acc], ((it >> 1) & 1) ^ 1);
-        mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * COUT;
-        const uint32_t st_base = a_base + stage * C::STAGE_BYTES;
+  } else if (warp >= 4 && warp < PROD_WARP0) {
+    // ===================== MMA + epilogue: warpgroup cw owns output rows [8 cw, 8 cw + 8) of every tile =====================
+    constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+    const int cw = (warp - 4) >> 2;
+    const int t = threadIdx.x & 127;
+    const int bar_id = 1 + cw;
+    float* stg = sE + cw * 64 * HALO_EPI_LD;
+    const bool has_res = STEMW == 0 && p.res != nullptr;      // (Conv_1 has no shortcut: the residual code is compiled out of the fused kernel)
+    const int er = t >> 1, eh = t & 1;                         // epilogue: this thread's pixel of the chunk and its 16-channel half
+    const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
+    float acc[COUT / 2];
+    mbar_wait(b_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t st_base = a_base + stage * C::STAGE_BYTES;
+      wgmma_fence_operand(acc);
+      wgmma_fence();
 #pragma unroll
-        for (int r = 0; r < 3; ++r) {
+      for (int r = 0; r < 3; ++r) {
 #pragma unroll
-          for (int s = 0; s < 3; ++s) {
-            const int pl = C::tap_plane(r, s);
-            const uint32_t a_tap = st_base + C::poff(pl) + (C::tap_dr(r) * C::pw(pl) + C::tap_ds(s)) * C::ROWB;
-            const uint32_t b_tap = b_base + (r * 3 + s) * C::B_TAP_BYTES;
+        for (int s = 0; s < 3; ++s) {
+          const int pl = C::tap_plane(r, s);
+          const uint32_t a_tap = st_base + C::poff(pl) + ((8 * cw + C::tap_dr(r)) * C::pw(pl) + C::tap_ds(s)) * C::ROWB;
+          const uint32_t b_tap = b_base + (r * 3 + s) * C::B_TAP_BYTES;
 #pragma unroll
-            for (int k = 0; k < CIN / 16; ++k) {
-              const uint64_t adesc = make_kmajor_desc(a_tap + k * 32, C::pw(pl) * C::ROWB, C::SWIZZLE);
-              const uint64_t bdesc = make_kmajor_desc(b_tap + k * 32, 8 * C::ROWB, C::SWIZZLE);
-              umma_f16(d_tmem, adesc, bdesc, idesc, (r | s | k) != 0);
-            }
+          for (int k = 0; k < CIN / 16; ++k)
+            Wgmma<COUT, kBF16, 0, 0>::mma(acc, make_kmajor_desc(a_tap + k * 32, C::pw(pl) * C::ROWB, C::SWIZZLE),
+                                          make_kmajor_desc(b_tap + k * 32, 8 * C::ROWB, C::SWIZZLE), (r | s | k) != 0);
+        }
+      }
+      wgmma_commit();
+      wgmma_fence_operand(acc);
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == C::NST) { stage = 0; phase ^= 1; }
+
+      const int tx = tile % p.tiles_x;
+      const int ty = (tile / p.tiles_x) % p.tiles_y;
+      const int img = tile / (p.tiles_x * p.tiles_y);
+      const int oh = ty * HT_H + 8 * cw + (er >> 3), ow = tx * HT_W + (er & 7);
+      const bool ok = oh < p.ho && ow < p.wo;
+      const long off = ((long)img * p.ho + oh) * p.wo + ow;
+#pragma unroll 1
+      for (int ch = 0; ch < COUT / 32; ++ch) {
+        warpgroup_bar(bar_id);                   // the previous chunk's readers are done with the staging tile
+        wgmma_stage_chunk<COUT>(acc, ch, stg, HALO_EPI_LD, t);
+        warpgroup_bar(bar_id);
+        if (!ok) continue;
+        const int c0 = ch * 32 + eh * 16;
+        const float* src = stg + er * HALO_EPI_LD + eh * 16;
+        float v[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) v[j] = fmaf(src[j], s_ss[c0 + j], s_ss[COUT + c0 + j]);
+        if (p.leaky) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);
+        }
+        if (has_res) {
+          const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + off * p.res_ld + c0);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const uint4 u = __ldg(rp + j);
+            float2 f;
+            f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
+            f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
+            f = Pack2<T>::unpack(u.z); v[8 * j + 4] += f.x; v[8 * j + 5] += f.y;
+            f = Pack2<T>::unpack(u.w); v[8 * j + 6] += f.x; v[8 * j + 7] += f.y;
           }
         }
-        umma_commit(&empty_bar[stage]);
-        umma_commit(&tfull_bar[acc]);
-        if (++stage == C::NST) { stage = 0; phase ^= 1; }
+        uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + off * p.out_ld + c0);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          uint4 pk;
+          pk.x = Pack2<T>::pack(v[8 * j + 0], v[8 * j + 1]);
+          pk.y = Pack2<T>::pack(v[8 * j + 2], v[8 * j + 3]);
+          pk.z = Pack2<T>::pack(v[8 * j + 4], v[8 * j + 5]);
+          pk.w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
+          op[j] = pk;
+        }
       }
     }
-    __syncwarp();
   } else if (STEMW > 0 && warp >= PROD_WARP0) {
     // ===================== stem producers (warps PROD_WARP0 .. PROD_WARP0 + STEMW - 1) =====================
     const int pw_id = warp - PROD_WARP0;
@@ -370,7 +402,7 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         multiply(m0);
         store(m0);
       }
-      fence_proxy_async();                       // generic-proxy plane writes -> visible to tcgen05.mma (async proxy)
+      fence_proxy_async();                       // generic-proxy plane writes -> visible to wgmma (async proxy)
       __syncwarp();
       if (lane == 0) {
         mbar_arrive(&full_bar[stage]);
@@ -379,179 +411,6 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       if (++in_stage == StemCfg::NIN) { in_stage = 0; in_phase ^= 1; }
       if (++stage == C::NST) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int quarter = warp & 3;                  // TMEM lanes [32 q, 32 q + 32): output rows 4q .. 4q+3 of the tile
-    const int grp = (warp - 2) >> 2;               // epilogue group: accumulator stage grp, tiles with iteration % EPIG == grp
-    uint8_t* stage2 = sE + ((warp - 2) & 3) * 4096;          // (staging is used by the non-direct path, EPIG = 1 only)
-    const bool direct = EPIG == 2 || p.direct != 0;
-    const int sw = (lane >> 1) & 3;
-    const int cq = lane & 3, cr0 = lane >> 2;      // coalesced layout: staging row 8k + cr0 (tile row 4q + k, col cr0), piece cq
-    const bool has_res = STEMW == 0 && p.res != nullptr;      // (Conv_1 has no shortcut: the residual code is compiled out of the fused kernel)
-    constexpr int NCH = COUT / 32;
-    uint32_t cnt = 0;
-    int it = grp;
-    uint4 rnext[4];
-    bool prefetched = false;
-    auto pix_base = [&](int tile, long (&off)[4], bool (&ok)[4]) {
-      const int tx = tile % p.tiles_x;
-      const int ty = (tile / p.tiles_x) % p.tiles_y;
-      const int img = tile / (p.tiles_x * p.tiles_y);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int oh = ty * HT_H + 4 * quarter + k, ow = tx * HT_W + cr0;
-        ok[k] = oh < p.ho && ow < p.wo;
-        off[k] = ((long)img * p.ho + oh) * p.wo + ow;
-      }
-    };
-    auto fetch_res = [&](const long (&off)[4], const bool (&ok)[4], int col0) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        rnext[k] = ok[k] ? __ldg(reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + off[k] * p.res_ld + col0 + cq * 8))
-                         : make_uint4(0u, 0u, 0u, 0u);
-    };
-    for (int tile = blockIdx.x + grp * gridDim.x; tile < p.num_tiles; tile += EPIG * gridDim.x, it += EPIG) {
-      const int acc = it & 1;
-      long off[4], noff[4];
-      bool ok[4], nok[4];
-      pix_base(tile, off, ok);
-      const int ntile = tile + EPIG * gridDim.x;
-      const bool has_next = ntile < p.num_tiles;
-      if (has_res && has_next) pix_base(ntile, noff, nok);
-      if (has_res && !prefetched) fetch_res(off, ok, 0);
-      mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-      tcgen05_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * COUT;
-      // all of the tile's TMEM loads in flight at once: tcgen05.ld is latency-bound (~1000 cycles, profiles/r02_b)
-      uint32_t r0[32], r1[32], r2[32], r3[32];
-      tmem_ld_32x32(t_row, r0);
-      tmem_ld_32x32(t_row + 32, r1);
-      if (NCH > 2) { tmem_ld_32x32(t_row + 64, r2); tmem_ld_32x32(t_row + 96, r3); }
-      auto chunk = [&](const uint32_t (&r)[32], const int ch) {
-        uint8_t* buf = stage2 + (cnt & 1u) * 2048;
-        uint4 rcur[4];
-        if (has_res) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) rcur[k] = rnext[k];
-          const bool last = ch + 1 >= NCH;
-          if (!last) fetch_res(off, ok, (ch + 1) * 32);
-          else if (has_next) fetch_res(noff, nok, 0);
-          if (last) prefetched = has_next;
-        }
-        float v[32];
-        const float4* sc4 = reinterpret_cast<const float4*>(s_ss + ch * 32);
-        const float4* sh4 = reinterpret_cast<const float4*>(s_ss + COUT + ch * 32);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 sc = sc4[j];
-          const float4 sh = sh4[j];
-          v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), sc.x, sh.x);
-          v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), sc.y, sh.y);
-          v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), sc.z, sh.z);
-          v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), sc.w, sh.w);
-        }
-        if (p.leaky) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);
-        }
-        uint4* rowp = reinterpret_cast<uint4*>(buf + lane * 64);
-        if (has_res) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int R = 8 * k + cr0;
-            *reinterpret_cast<uint4*>(buf + R * 64 + ((cq ^ ((R >> 1) & 3)) << 4)) = rcur[k];
-          }
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint4 u = rowp[j ^ sw];
-            float2 f;
-            f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
-            f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
-            f = Pack2<T>::unpack(u.z); v[8 * j + 4] += f.x; v[8 * j + 5] += f.y;
-            f = Pack2<T>::unpack(u.w); v[8 * j + 6] += f.x; v[8 * j + 7] += f.y;
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint4 pk;
-          pk.x = Pack2<T>::pack(v[8 * j + 0], v[8 * j + 1]);
-          pk.y = Pack2<T>::pack(v[8 * j + 2], v[8 * j + 3]);
-          pk.z = Pack2<T>::pack(v[8 * j + 4], v[8 * j + 5]);
-          pk.w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
-          rowp[j ^ sw] = pk;
-        }
-        __syncwarp();
-        T* outp = static_cast<T*>(p.out) + ch * 32 + cq * 8;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int R = 8 * k + cr0;
-          const uint4 u = *reinterpret_cast<const uint4*>(buf + R * 64 + ((cq ^ ((R >> 1) & 3)) << 4));
-          if (ok[k]) *reinterpret_cast<uint4*>(outp + off[k] * p.out_ld) = u;
-        }
-        ++cnt;
-      };
-      // direct path: this lane's pixel (tile row 4q + lane / 8, column lane % 8) and its 32 channels of a chunk = 64 bytes
-      long my_off = 0;
-      bool my_ok = false;
-      if (direct) {
-        const int tx = tile % p.tiles_x;
-        const int ty = (tile / p.tiles_x) % p.tiles_y;
-        const int img = tile / (p.tiles_x * p.tiles_y);
-        const int oh = ty * HT_H + 4 * quarter + (lane >> 3), ow = tx * HT_W + (lane & 7);
-        my_ok = oh < p.ho && ow < p.wo;
-        my_off = (((long)img * p.ho + oh) * p.wo + ow) * p.out_ld;
-      }
-      auto chunk_direct = [&](const uint32_t (&r)[32], const int ch) {
-        float v[32];
-        const float4* sc4 = reinterpret_cast<const float4*>(s_ss + ch * 32);
-        const float4* sh4 = reinterpret_cast<const float4*>(s_ss + COUT + ch * 32);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 sc = sc4[j];
-          const float4 sh = sh4[j];
-          v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), sc.x, sh.x);
-          v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), sc.y, sh.y);
-          v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), sc.z, sh.z);
-          v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), sc.w, sh.w);
-        }
-        if (p.leaky) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);
-        }
-        if (my_ok) {
-          uint32_t lo[8], hi[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            lo[j] = Pack2<T>::pack(v[2 * j], v[2 * j + 1]);
-            hi[j] = Pack2<T>::pack(v[16 + 2 * j], v[16 + 2 * j + 1]);
-          }
-          T* dst = static_cast<T*>(p.out) + my_off + ch * 32;
-          st_global_v8(dst, lo);
-          st_global_v8(dst + 16, hi);
-        }
-      };
-      tmem_ld_wait();
-      if (direct) {
-        chunk_direct(r0, 0);
-        chunk_direct(r1, 1);
-        if (NCH > 2) { chunk_direct(r2, 2); chunk_direct(r3, 3); }
-      } else if (EPIG == 1) {
-        chunk(r0, 0);
-        chunk(r1, 1);
-        if (NCH > 2) { chunk(r2, 2); chunk(r3, 3); }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-    }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -567,16 +426,18 @@ static int launch_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t s
   return YB_OK;
 }
 
-template <typename T, int STEM_WARPS, int EPIG>
+static constexpr int STEM_WARPS = 8;           // stem producer warps of the fused kernel (640 threads per CTA)
+
+template <typename T>
 static int launch_stem_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
   using C = HaloCfg<32, 64, 2>;
   constexpr int SMEM = C::SMEM_BYTES + StemCfg::NIN * StemCfg::IN_BYTES;
   static_assert(SMEM <= 227 * 1024, "fused stem + Conv_1 does not fit shared memory");
   static DeviceOnce once;
-  auto kern = conv_halo_kernel<T, 32, 64, 2, STEM_WARPS, EPIG>;
+  auto kern = conv_halo_kernel<T, 32, 64, 2, STEM_WARPS>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), SMEM); if (rc) return rc; }
   const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  kern<<<grid, 64 + 128 * EPIG + 32 * STEM_WARPS, SMEM, st>>>(maps, p);
+  kern<<<grid, HALO_THREADS + 32 * STEM_WARPS, SMEM, st>>>(maps, p);
   YB_CUDA(cudaGetLastError());
   return YB_OK;
 }
@@ -597,7 +458,6 @@ int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const floa
   p->cout = d->cout; p->leaky = d->leaky; p->scale = scale; p->shift = shift;
   p->res = nullptr; p->res_ld = 0; p->out = out; p->out_ld = d->out_ld;
   p->stem_w = stem_w; p->stem_scale = stem_scale; p->stem_shift = stem_shift; p->in_h = d->h; p->in_w = d->w;
-  p->direct = (d->out_ld % 16 == 0 && ((uintptr_t)out & 31) == 0 && opt("YB_HALO_DIRECT")[0] != '0') ? 1 : 0;
   int rc = make_tmap_image3d(&maps->in3d, image, d->n, d->h, d->w, StemCfg::IN_ROWF, StemCfg::IN_ROWS);
   if (rc) return rc;
   const long K = 9L * d->cin;
@@ -605,13 +465,7 @@ int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const floa
 }
 
 int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-  // A/B switches: YB_STEM_WARPS = 8 | 12 producer warps, YB_STEM_EPIG = 1 | 2 epilogue groups
-  const bool w12 = opt("YB_STEM_WARPS")[0] != '8';      // default: twelve producer warps
-  const bool direct_ok = d->out_ld % 16 == 0 && ((uintptr_t)p.out & 31) == 0;
-  const bool eg2 = direct_ok && opt("YB_STEM_EPIG")[0] == '2';
-#define YB_STEM_LAUNCH(T)                                                        \
-  if (eg2) return w12 ? launch_stem_halo<T, 12, 2>(maps, p, st) : launch_stem_halo<T, 8, 2>(maps, p, st); \
-  return w12 ? launch_stem_halo<T, 12, 1>(maps, p, st) : launch_stem_halo<T, 8, 1>(maps, p, st);
+#define YB_STEM_LAUNCH(T) return launch_stem_halo<T>(maps, p, st);
   if (d->dtype == YB_F16) { YB_STEM_LAUNCH(__half) }
   if (d->dtype == YB_BF16) { YB_STEM_LAUNCH(__nv_bfloat16) }
 #undef YB_STEM_LAUNCH
@@ -644,8 +498,6 @@ int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed
   p->num_tiles = p->tiles_x * p->tiles_y * d->n;
   p->cout = d->cout; p->leaky = d->leaky; p->scale = scale; p->shift = shift;
   p->res = res; p->res_ld = d->res_ld; p->out = out; p->out_ld = d->out_ld;
-  // direct 256-bit stores when there is no residual and the rows are 32-byte aligned
-  p->direct = (!res && d->out_ld % 16 == 0 && ((uintptr_t)out & 31) == 0 && opt("YB_HALO_DIRECT")[0] != '0') ? 1 : 0;
   int rc;
   if (d->stride == 1) {
     rc = make_tmap_tiled4d(&maps->plane[0], x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->cin, HT_W + 2, HT_H + 2, 1);

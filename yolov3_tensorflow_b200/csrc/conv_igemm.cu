@@ -1,5 +1,5 @@
 // Fused conv (+BN scale/shift +leaky +residual +2x-upsample +concat-slice store) as an
-// im2col-free implicit GEMM on the 5th-gen tensor cores:
+// im2col-free implicit GEMM on the Hopper tensor cores (wgmma):
 //
 //   D[M = n*ho*wo pixels, N = cout] = A[M, K = k*k*cin] * B[N, K]^T
 //
@@ -9,12 +9,13 @@
 //        come back zero-filled, so no padded copy of the input ever exists (K4 in SURVEY §2.3).
 //        1x1 convs: plain 2D tiled TMA over the [M, in_ld] matrix.
 //   B  : weights packed OHWI = [cout_pad, k*k*cin] K-major, 2D tiled TMA.
-//   D  : fp32 accumulators in TMEM (2 stages x BLOCK_N columns), tcgen05.mma issued by
-//        one thread, operands straight from 128B-swizzled shared memory.
+//   D  : fp32 accumulators in registers: two consumer warpgroups own 64 rows x BN columns each and
+//        issue wgmma.mma_async m64nBNk16 with both operands read from 128B / 64B-swizzled shared memory.
 //
-// Warp roles (192 threads, persistent over tiles): warp0 = TMA producer, warp1 = TMEM
-// allocator + MMA issuer, warps 2..5 = epilogue (TMEM -> registers -> global), so the
-// epilogue of tile i overlaps the mainloop of tile i+1.
+// Warp roles (384 threads, persistent over tiles): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 =
+// MMA + epilogue.  The producer runs ahead through the operand ring, so the next tile's loads overlap this tile's
+// epilogue.  The epilogue stages 32-column chunks of the accumulators through shared memory so that each thread
+// then owns 16 consecutive channels of one pixel (two 16-byte stores per output row).
 //
 // Replaces: slim.conv2d/batch_norm/leaky_relu (utils/layer_utils.py:20, model.py:43-49),
 // tf.add (utils/layer_utils.py:30), tf.pad (:15-16), resize_nearest_neighbor (:86),
@@ -27,58 +28,52 @@
 
 #include "common.cuh"
 #include "conv.cuh"
+#include "wgmma.cuh"
 
 namespace yb {
 
-static constexpr int BLOCK_M = 128;
-static constexpr int UMMA_K = 16;
-static constexpr int NUM_THREADS = 192;         // warp 0 producer, warp 1 MMA, warps 2..5 epilogue (one epilogue group)
-// Epilogue groups (EG): with ONE warp per scheduler the epilogue's ~200 instructions per 32-column chunk issue at
-// IPC ~0.2 (fixed-latency dependencies and nothing to switch to: ~1100 cycles per chunk, profiles/r02_c) and pace every
-// short-K layer.  EG = 2 adds a second set of four epilogue warps: group g drains accumulator stage g (tiles with
-// iteration % 2 == g), so two tiles' epilogues run concurrently, two warps per scheduler.  Its staging tiles cost one
-// operand stage.
-__host__ __device__ constexpr int nthreads(int eg) { return 64 + 128 * eg; }
-__host__ __device__ constexpr int ring_budget(int eg) { return eg == 1 ? 192 * 1024 : 160 * 1024; }   // operand ring
-static constexpr int SMEM_BUDGET = ring_budget(1);
-// Per-epilogue-warp staging: three 2 KB [32 rows][32 channels] SWIZZLE_64B tiles that rotate between the TMA residual
-// load, the in-place epilogue and the TMA store of a chunk (or one 32x33 fp32 transpose tile for the detection heads).
-static constexpr int EPI_TILE_BYTES = 2048;
-static constexpr int EPI_TILES = 3;
-static constexpr int STAGE_BYTES_W = EPI_TILES * EPI_TILE_BYTES;   // 6144 = 12 x 512: every tile is swizzle-atom aligned
-static constexpr int STAGE_FLOATS = STAGE_BYTES_W / 4;
-static constexpr int BAR_BYTES = 512;           // pipeline barriers + 4 x 3 residual barriers + TMEM slot
+static constexpr int WG_ROWS = 64;                // accumulator rows per consumer warpgroup
+static constexpr int RING_BYTES = 196 * 1024;     // operand ring (the rest of the 227 KB: staging, scale / shift, stats)
+static constexpr int EPI_LD = 33;                 // staging row pitch in floats: row walks and column walks are conflict-free
+static constexpr int EPI_FLOATS = WG_ROWS * EPI_LD;
 
-template <int BN, int BK, int EG = 1>
+// NC consumer warpgroups per CTA (tile = 64 NC rows x BN); warpgroup 0 is the TMA producer.
+template <int BN, int BK, int NC>
 struct Cfg {
+  static constexpr int BLOCK_M = WG_ROWS * NC;
+  static constexpr int THREADS = 128 * (NC + 1);
   static constexpr int A_BYTES = BLOCK_M * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int RING = ring_budget(EG);
-  static constexpr int STAGES = (RING / STAGE_BYTES) > 8 ? 8 : (RING / STAGE_BYTES);
-  static constexpr int TMEM_COLS = 2 * BN;  // power of two >= 32 for BN in {64,128,256}
-  static constexpr int SMEM_BYTES = RING + 1024 /*align*/ + 4 * EG * STAGE_BYTES_W + BAR_BYTES + (2 + 2 * EG) * BN * 4;
-  static constexpr uint32_t SWIZZLE = (BK == 64) ? 2u : 4u;   // UMMA layout_type: 128B / 64B
-  static constexpr uint32_t SBO = 8 * BK * 2;                  // bytes between 8-row groups
+  static constexpr int STAGES = (RING_BYTES / STAGE_BYTES) > 8 ? 8 : (RING_BYTES / STAGE_BYTES);
+  // ring | NC x staging tile | NC x [2][BN] statistics | NC x [2][BN] scale / shift | barriers
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + NC * EPI_FLOATS * 4 + NC * 4 * BN * 4 + 256;
+  static constexpr uint32_t SWIZZLE = BK * 2;     // a k-block row is exactly one swizzle span (128B / 64B)
+  static constexpr uint32_t SBO = 8 * BK * 2;     // bytes between 8-row groups
 };
+static_assert(Cfg<256, 64, 2>::SMEM_BYTES <= 227 * 1024, "conv: the widest tile does not fit shared memory");
 
-// debugging aid: CTA 0 stamps clock64 into p.trace[(role * 64 + tile iteration) * 32 + slot], role = warp 0..9 (tools/conv_trace.py)
-__device__ __forceinline__ void trace_stamp(const ConvParams& p, int role, int it, int slot) {
-  if (p.trace != nullptr && blockIdx.x == 0 && it < 64) p.trace[(role * 64 + it) * 32 + slot] = clock64();
+// Work unit -> (m tile, n tile) of this CTA.  A cluster of p.cluster CTAs shares one n-tile (its weight tile is
+// multicast) and takes p.cluster consecutive m-tiles; rank r of the cluster takes the r-th (possibly past the last
+// m-tile: it still takes part in the multicast, its rows are all masked).  Inference walks n fastest (the A tiles
+// stay hot in L2 across their n tiles); with BN statistics on, m runs fastest so a CTA's tiles share their n tile
+// and its per-CTA column sums are flushed to global at most num_n_tiles times.
+__device__ __forceinline__ int num_units(const ConvParams& p) {
+  return (p.num_m_tiles + p.cluster - 1) / p.cluster * p.num_n_tiles;
+}
+__device__ __forceinline__ void unit_coords(const ConvParams& p, int unit, int rank, int& m_idx, int& n_idx) {
+  const int sm_tiles = (p.num_m_tiles + p.cluster - 1) / p.cluster;
+  int sm;
+  if (p.stat_sum != nullptr) { n_idx = unit / sm_tiles; sm = unit - n_idx * sm_tiles; }
+  else { sm = unit / p.num_n_tiles; n_idx = unit - sm * p.num_n_tiles; }
+  m_idx = sm * p.cluster + rank;
 }
 
-// tile index -> (m tile, n tile).  Inference walks n fastest (the A tile stays hot in L2 across its n tiles);
-// with BN statistics on, m runs fastest so a CTA's tiles share their n tile and its per-CTA column sums are
-// flushed to global at most num_n_tiles times.
-__device__ __forceinline__ void tile_coords(const ConvParams& p, int tile, int& m_idx, int& n_idx) {
-  if (p.stat_sum != nullptr) { n_idx = tile / p.num_m_tiles; m_idx = tile - n_idx * p.num_m_tiles; }
-  else { m_idx = tile / p.num_n_tiles; n_idx = tile - m_idx * p.num_n_tiles; }
-}
-// executed by the 128 epilogue threads together (named barrier 1)
+// executed by the 128 threads of one consumer warpgroup: add the per-CTA column sums into the global statistics
 template <int BN>
-__device__ __forceinline__ void stat_flush(const ConvParams& p, float* s_stat, int n0, int et /*0..127*/) {
-  asm volatile("bar.sync 1, 128;" ::: "memory");   // (statistics only run with one epilogue group)
-  for (int c = et; c < BN; c += 128) {
+__device__ __forceinline__ void stat_flush(const ConvParams& p, float* s_stat, int n0, int t, int bar_id) {
+  warpgroup_bar(bar_id);
+  for (int c = t; c < BN; c += 128) {
     if (n0 + c < p.cout) {
       atomicAdd(p.stat_sum + n0 + c, s_stat[c]);
       atomicAdd(p.stat_sqsum + n0 + c, s_stat[BN + c]);
@@ -86,135 +81,21 @@ __device__ __forceinline__ void stat_flush(const ConvParams& p, float* s_stat, i
     s_stat[c] = 0.f;
     s_stat[BN + c] = 0.f;
   }
-  asm volatile("bar.sync 1, 128;" ::: "memory");
+  warpgroup_bar(bar_id);
 }
 
-// executed by the 128 epilogue threads together: (re)load the n-tile's scale/shift into shared memory
-template <int BN>
-__device__ __forceinline__ void load_scale_shift(const ConvParams& p, float* s_ss, int n0, int et /*0..127*/, int group = 0) {
-  asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");   // nobody of this group still reads the previous n-tile's values
-  for (int c = et; c < BN; c += 128) {
-    s_ss[c] = p.scale ? __ldg(p.scale + n0 + c) : 1.f;      // scale = shift = NULL: identity (dgrad convs)
-    s_ss[BN + c] = p.shift ? __ldg(p.shift + n0 + c) : 0.f;
+// 16 consecutive channels of one accumulator row: scale/shift (+leaky) (+residual) -> 16-bit / fp32 global stores
+// (channel-slice, 2x-upsample and parity-scatter aware).
+template <typename T>
+__device__ __forceinline__ void epi_store16(const ConvParams& p, const float* src, const int row, const int col0,
+                                            const float* sc, const float* sh) {
+  float v[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) v[j] = fmaf(src[j], sc[j], sh[j]);
+  if (p.leaky) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);   // == v > 0 ? v : 0.1 v
   }
-  asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Epilogues.  One warp owns 32 accumulator rows (TMEM lanes) and walks the tile's columns in chunks of 32.
-// The chunk loop is ROLLED (two bodies, for the two TMEM read buffers): fully unrolled, the two epilogues of a
-// 256-wide tile were ~15 k SASS instructions of straight-line code executed once per tile, the kernel outgrew the
-// instruction cache (18 k instructions, 290 KB) and the epilogue warps spent most of their time in `no_inst` stalls —
-// 1100 cycles per chunk against a ~250-cycle TMEM-read floor (profiles/r02_b: ncu source page + in-kernel timeline).
-// ---------------------------------------------------------------------------------------------------------------
-
-// One chunk of the register-store epilogue: scale/shift (+leaky) (+residual) -> 16-bit / fp32 global stores
-// (channel-slice, 2x-upsample and parity-scatter aware), optional BN batch statistics.  `r` holds the chunk.
-template <typename T, int BN>
-__device__ __forceinline__ void epi_reg_chunk(const ConvParams& p, const uint32_t (&r)[32], const int ch, const int row,
-                                              const bool row_ok, const int n0, const long (&orow)[4], const int nrep,
-                                              const int lane, float* stage, float* s_stat, const float* s_ss) {
-  const int col0 = n0 + ch * 32;
-  if (p.stat_sum != nullptr) {
-    // BN batch statistics of the raw conv output.  Transpose the warp's 32x32 block through its staging
-    // tile so each lane sums ONE column over the 32 rows, then accumulate per-CTA column sums in shared
-    // memory; they are flushed to global once per (CTA, n-tile) by the caller (global atomics contend badly).
-#pragma unroll
-    for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = row_ok ? __uint_as_float(r[j]) : 0.f;
-    __syncwarp();
-    float cs = 0.f, cs2 = 0.f;
-#pragma unroll
-    for (int rr = 0; rr < 32; ++rr) {
-      const float t = stage[rr * 33 + lane];
-      cs += t;
-      cs2 = fmaf(t, t, cs2);
-    }
-    __syncwarp();
-    atomicAdd(&s_stat[ch * 32 + lane], cs);
-    atomicAdd(&s_stat[BN + ch * 32 + lane], cs2);
-  }
-  if (row_ok) {
-    float v[32];
-    const float4* sc4 = reinterpret_cast<const float4*>(s_ss + ch * 32);
-    const float4* sh4 = reinterpret_cast<const float4*>(s_ss + BN + ch * 32);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 sc = sc4[j];
-      const float4 sh = sh4[j];
-      v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), sc.x, sh.x);
-      v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), sc.y, sh.y);
-      v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), sc.z, sh.z);
-      v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), sc.w, sh.w);
-    }
-    if (p.leaky) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);   // == v > 0 ? v : 0.1 v
-    }
-    if (p.res != nullptr) {
-      const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) +
-                                                       (p.scatter ? orow[0] : (long)row) * p.res_ld + col0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 u = __ldg(rp + j);
-        float2 f;
-        f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
-        f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
-        f = Pack2<T>::unpack(u.z); v[8 * j + 4] += f.x; v[8 * j + 5] += f.y;
-        f = Pack2<T>::unpack(u.w); v[8 * j + 6] += f.x; v[8 * j + 7] += f.y;
-      }
-    }
-    if (p.out_fp32) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = v[j];
-    } else {
-      uint4 pk[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        pk[j].x = Pack2<T>::pack(v[8 * j + 0], v[8 * j + 1]);
-        pk[j].y = Pack2<T>::pack(v[8 * j + 2], v[8 * j + 3]);
-        pk[j].z = Pack2<T>::pack(v[8 * j + 4], v[8 * j + 5]);
-        pk[j].w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
-      }
-      for (int rep = 0; rep < nrep; ++rep) {
-        uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + orow[rep] * p.out_ld + col0);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) op[j] = pk[j];
-      }
-    }
-  }
-  if (p.out_fp32) {
-    // detection heads (cout = 255, fp32): transpose through shared memory so that each store
-    // instruction writes one 128-byte row segment instead of 32 scattered words
-    __syncwarp();
-    const int row_base = row - lane;
-#pragma unroll 1
-    for (int rr = 0; rr < 32; ++rr) {
-      const int r2 = row_base + rr;
-      if (r2 >= p.M) break;
-      if (col0 + lane < p.cout) {
-        const float val = stage[rr * 33 + lane];
-        if (!p.upsample) {
-          static_cast<float*>(p.out)[(long)r2 * p.out_ld + col0 + lane] = val;
-        } else {
-          const int q = r2 % p.Q, pp = (r2 / p.Q) % p.P, img = r2 / (p.Q * p.P);
-          const long W2 = 2L * p.Q;
-          const long base = ((long)img * 2 * p.P + 2 * pp) * W2 + 2 * q;
-          float* o = static_cast<float*>(p.out) + col0 + lane;
-          o[base * p.out_ld] = val; o[(base + 1) * p.out_ld] = val;
-          o[(base + W2) * p.out_ld] = val; o[(base + W2 + 1) * p.out_ld] = val;
-        }
-      }
-    }
-    __syncwarp();
-  }
-}
-
-// Register-store epilogue of one warp over its 32 accumulator rows x BN columns (fp32 heads, 2x-upsample stores,
-// parity scatter, the multicast kernel).  The TMEM load of chunk c+1 is in flight while chunk c is processed.
-template <typename T, int BN>
-__device__ __forceinline__ void epilogue_tile(const ConvParams& p, const int row, const int n0, const uint32_t t_row,
-                                              const int lane, float* stage, float* s_stat, const float* s_ss) {
-  const bool row_ok = row < p.M;
   long orow[4] = {row, 0, 0, 0};
   int nrep = 1;
   if (p.upsample || p.scatter) {
@@ -230,250 +111,153 @@ __device__ __forceinline__ void epilogue_tile(const ConvParams& p, const int row
       nrep = 4;
     }
   }
-  constexpr int NCH = BN / 32;
-  const int nvalid = min(NCH, (p.cout - n0 + 31) >> 5);      // zero-padded weight rows (cout_pad > cout): nothing to store
-  if (nvalid <= 0) return;
-  // chunk c + 1's TMEM load is in flight while chunk c is processed (two buffers: tcgen05.ld itself is fast — 90 cycles
-  // per 32 columns, tools/probes/tmem_ld_probe.cu — more loads in flight bought nothing and cost 64 registers)
-  uint32_t ra[32], rb[32];
-  tmem_ld_32x32(t_row, ra);
-#pragma unroll 1
-  for (int ch = 0; ch < nvalid; ch += 2) {
-    tmem_ld_wait();
-    if (ch + 1 < nvalid) tmem_ld_32x32(t_row + (ch + 1) * 32, rb);
-    epi_reg_chunk<T, BN>(p, ra, ch, row, row_ok, n0, orow, nrep, lane, stage, s_stat, s_ss);
-    if (ch + 1 < nvalid) {
-      tmem_ld_wait();
-      if (ch + 2 < nvalid) tmem_ld_32x32(t_row + (ch + 2) * 32, ra);
-      epi_reg_chunk<T, BN>(p, rb, ch + 1, row, row_ok, n0, orow, nrep, lane, stage, s_stat, s_ss);
+  if (p.out_fp32) {                              // detection heads: cout = 3 (5 + C) need not be a multiple of 16
+    for (int rep = 0; rep < nrep; ++rep) {
+      float* o = static_cast<float*>(p.out) + orow[rep] * p.out_ld + col0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        if (col0 + j < p.cout) o[j] = v[j];
     }
+    return;
   }
-}
-
-
-// Column sums over the 32 rows of a 32x32 block held one row per lane (v[j] = column j of this lane's row): recursive
-// halving, 31 shuffles, no shared memory.  Lane l returns the sum of column l.  v is destroyed.
-template <int W>
-__device__ __forceinline__ void col_sum_step(float (&v)[32], const int lane) {
-  const bool hi = (lane & W) != 0;
+  if (p.res != nullptr) {
+    const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + orow[0] * p.res_ld + col0);
 #pragma unroll
-  for (int j = 0; j < W; ++j) {
-    const float send = hi ? v[j] : v[j + W];
-    const float keep = hi ? v[j + W] : v[j];
-    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, W);
-  }
-}
-__device__ __forceinline__ float warp_col_sum32(float (&v)[32], const int lane) {
-  col_sum_step<16>(v, lane); col_sum_step<8>(v, lane); col_sum_step<4>(v, lane); col_sum_step<2>(v, lane);
-  col_sum_step<1>(v, lane);
-  return v[0];
-}
-
-// Epilogue of one warp over its 32 accumulator rows x BN columns, 16-bit outputs, through shared memory and the TMA:
-//   TMEM -> registers -> scale/shift (+leaky) -> [+ residual tile, fetched by TMA into the same staging tile]
-//   -> 16-bit, written in place into the SWIZZLE_64B staging tile -> cp.async.bulk.tensor store (rows >= M clipped).
-// The first version stored straight from registers: one row per lane, so every 16-byte store instruction touched 32
-// different 128-byte lines (32 L1 wavefronts, half-written sectors) and the residual loads did the same.  Here the LSU
-// only sees conflict-free 16-byte shared-memory accesses; global traffic is full 64-byte row segments issued by the TMA.
-// Three staging tiles rotate per warp: while chunk c is processed, chunk c+1's residual is landing and chunk c-1's
-// store is draining.  `cnt` (chunks processed by this warp so far) indexes tiles and barrier phases across tiles.
-struct EpiTmaState {
-  uint8_t* stage;
-  uint64_t* res_bar;
-  uint32_t cnt;
-  bool prefetched;
-};
-
-template <typename T, int BN>
-__device__ __forceinline__ void epi_tma_chunk(const ConvParams& p, const uint32_t (&r)[32], const int ch, const int nvalid,
-                                              const int m0w, const int n0, const bool row_ok, const bool has_res,
-                                              const int lane, EpiTmaState& st, float* s_stat, const float* s_ss,
-                                              const bool has_next, const int next_m0w, const int next_n0,
-                                              const int tr_role, const int tr_it) {
-  const int sw = (lane >> 1) & 3;                // SWIZZLE_64B: 16-byte chunk j of row r sits at chunk j ^ ((r >> 1) & 3)
-  const uint32_t b = st.cnt % EPI_TILES;
-  uint8_t* buf = st.stage + b * EPI_TILE_BYTES;
-  if (has_res) {
-    // fetch the NEXT chunk's residual (this tile's, or the first of the next tile) into the tile freed two stores ago
-    const bool last = ch + 1 >= nvalid;
-    const int nm = last ? next_m0w : m0w;
-    const int nc = last ? next_n0 : n0 + (ch + 1) * 32;
-    const bool go = last ? (has_next && next_m0w < p.M) : true;
-    if (go && lane == 0) {
-      bulk_wait_group_read<1>();
-      const uint32_t nb = (st.cnt + 1) % EPI_TILES;
-      mbar_arrive_expect_tx(&st.res_bar[nb], EPI_TILE_BYTES);
-      tma_load_2d(st.stage + nb * EPI_TILE_BYTES, &p.tmR, &st.res_bar[nb], nc, nm);
-    }
-    if (last) st.prefetched = go;
-  }
-  float v[32];
-  const float4* sc4 = reinterpret_cast<const float4*>(s_ss + ch * 32);
-  const float4* sh4 = reinterpret_cast<const float4*>(s_ss + BN + ch * 32);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 sc = sc4[j];
-    const float4 sh = sh4[j];
-    v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), sc.x, sh.x);
-    v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), sc.y, sh.y);
-    v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), sc.z, sh.z);
-    v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), sc.w, sh.w);
-  }
-  if (p.leaky) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);   // == v > 0 ? v : 0.1 v
-  }
-  uint4* rowp = reinterpret_cast<uint4*>(buf + lane * 64);
-  if (has_res) {
-    mbar_wait(&st.res_bar[b], (st.cnt / EPI_TILES) & 1);             // residual tile landed (async proxy -> visible)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint4 u = rowp[j ^ sw];
+    for (int j = 0; j < 2; ++j) {
+      const uint4 u = __ldg(rp + j);
       float2 f;
       f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
       f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
       f = Pack2<T>::unpack(u.z); v[8 * j + 4] += f.x; v[8 * j + 5] += f.y;
       f = Pack2<T>::unpack(u.w); v[8 * j + 6] += f.x; v[8 * j + 7] += f.y;
     }
-  } else if (!(p.dbg & 16)) {                    // the store that last read this tile (3 chunks ago) has drained
-    if (lane == 0) bulk_wait_group_read<EPI_TILES - 1>();
-    __syncwarp();
   }
-  // (ablation switches, timing only: dbg & 32 no staging stores, dbg & 16 no fence / TMA store)
-  if (!(p.dbg & 32)) {
+  uint4 pk[2];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 pk;
-      pk.x = Pack2<T>::pack(v[8 * j + 0], v[8 * j + 1]);
-      pk.y = Pack2<T>::pack(v[8 * j + 2], v[8 * j + 3]);
-      pk.z = Pack2<T>::pack(v[8 * j + 4], v[8 * j + 5]);
-      pk.w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
-      rowp[j ^ sw] = pk;
-    }
-  } else {
-    float acc = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc += v[j];
-    if (acc == 123.456f) rowp[0] = make_uint4(1u, 2u, 3u, 4u);     // keeps the arithmetic alive
+  for (int j = 0; j < 2; ++j) {
+    pk[j].x = Pack2<T>::pack(v[8 * j + 0], v[8 * j + 1]);
+    pk[j].y = Pack2<T>::pack(v[8 * j + 2], v[8 * j + 3]);
+    pk[j].z = Pack2<T>::pack(v[8 * j + 4], v[8 * j + 5]);
+    pk[j].w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
   }
-  if (!(p.dbg & 16)) {
-    fence_proxy_async();                         // generic-proxy writes -> visible to the TMA (async proxy)
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_2d(&p.tmO, buf, n0 + ch * 32, m0w);
-      bulk_commit_group();
-    }
+  for (int rep = 0; rep < nrep; ++rep) {
+    uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + orow[rep] * p.out_ld + col0);
+    op[0] = pk[0];
+    op[1] = pk[1];
   }
-  if (lane == 0) trace_stamp(p, tr_role, tr_it, 4 + 3 * (ch & 7));
-  ++st.cnt;
 }
 
+// Register epilogue (YB_CONV_EPI=reg): every thread stores its own accumulator fragments — two adjacent channels of
+// rows r0 and r0 + 8 per 8-column block — straight to global memory, without the staging tile and its barriers.
 template <typename T, int BN>
-__device__ __forceinline__ void epilogue_tile_tma(const ConvParams& p, const int m0w, const int n0, const uint32_t t_row,
-                                                  const int lane, EpiTmaState& st, float* s_stat, const float* s_ss,
-                                                  const bool has_next, const int next_m0w, const int next_n0,
-                                                  const int tr_role = 0, const int tr_it = 64) {
-  if (m0w >= p.M) return;                        // warp-uniform: all 32 rows lie past the last pixel (tail tile)
-  const bool has_res = p.res != nullptr;
-  const bool row_ok = m0w + lane < p.M;
-  constexpr int NCH = BN / 32;
-  const int nvalid = min(NCH, (p.cout - n0) >> 5);           // zero-padded weight rows (cout_pad > cout) are not stored
-  if (nvalid <= 0) return;
-  if (has_res && !st.prefetched && lane == 0) {  // first chunk of the run: nobody fetched its residual ahead of time
-    bulk_wait_group_read<EPI_TILES - 1>();
-    const uint32_t b = st.cnt % EPI_TILES;
-    mbar_arrive_expect_tx(&st.res_bar[b], EPI_TILE_BYTES);
-    tma_load_2d(st.stage + b * EPI_TILE_BYTES, &p.tmR, &st.res_bar[b], n0, m0w);
-  }
-  uint32_t ra[32], rb[32];                       // two TMEM read buffers (see epilogue_tile)
-  tmem_ld_32x32(t_row, ra);
-#pragma unroll 1
-  for (int ch = 0; ch < nvalid; ch += 2) {
-    if (lane == 0) trace_stamp(p, tr_role, tr_it, 2 + 3 * (ch & 7));
-    tmem_ld_wait();
-    if (lane == 0) trace_stamp(p, tr_role, tr_it, 3 + 3 * (ch & 7));
-    if (ch + 1 < nvalid) tmem_ld_32x32(t_row + (ch + 1) * 32, rb);
-    epi_tma_chunk<T, BN>(p, ra, ch, nvalid, m0w, n0, row_ok, has_res, lane, st, s_stat, s_ss, has_next, next_m0w, next_n0,
-                         tr_role, tr_it);
-    if (ch + 1 < nvalid) {
-      if (lane == 0) trace_stamp(p, tr_role, tr_it, 2 + 3 * ((ch + 1) & 7));
-      tmem_ld_wait();
-      if (lane == 0) trace_stamp(p, tr_role, tr_it, 3 + 3 * ((ch + 1) & 7));
-      if (ch + 2 < nvalid) tmem_ld_32x32(t_row + (ch + 2) * 32, ra);
-      epi_tma_chunk<T, BN>(p, rb, ch + 1, nvalid, m0w, n0, row_ok, has_res, lane, st, s_stat, s_ss, has_next, next_m0w,
-                           next_n0, tr_role, tr_it);
+__device__ __forceinline__ void epilogue_reg(const ConvParams& p, const float (&acc)[BN / 2], const int row0, const int n0,
+                                             const float* s_ss, const int t) {
+  const int ncols = min(BN, p.cout - n0);
+  const int rbase = row0 + 16 * (t >> 5) + ((t & 31) >> 2), cq = 2 * (t & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = rbase + 8 * h;
+    if (row >= p.M) continue;
+    long orow[4] = {row, 0, 0, 0};
+    int nrep = 1;
+    if (p.upsample || p.scatter) {
+      const int q = row % p.Q;
+      const int pp = (row / p.Q) % p.P;
+      const int img = row / (p.Q * p.P);
+      const long W2 = 2L * p.Q;
+      const long base = ((long)img * 2 * p.P + 2 * pp) * W2 + 2 * q;
+      if (p.scatter) {
+        orow[0] = base + ((p.scatter - 1) >> 1) * W2 + ((p.scatter - 1) & 1);
+      } else {
+        orow[0] = base; orow[1] = base + 1; orow[2] = base + W2; orow[3] = base + W2 + 1;
+        nrep = 4;
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + cq;                  // column inside the tile
+      if (c >= ncols) continue;
+      float v0 = fmaf(acc[4 * j + 2 * h], s_ss[c], s_ss[BN + c]);
+      float v1 = fmaf(acc[4 * j + 2 * h + 1], s_ss[c + 1], s_ss[BN + c + 1]);
+      if (p.leaky) { v0 = fmaxf(v0, 0.1f * v0); v1 = fmaxf(v1, 0.1f * v1); }
+      const long col = n0 + c;
+      if (p.out_fp32) {
+        for (int rep = 0; rep < nrep; ++rep) {
+          float* o = static_cast<float*>(p.out) + orow[rep] * p.out_ld + col;
+          o[0] = v0;
+          if (c + 1 < ncols) o[1] = v1;
+        }
+        continue;
+      }
+      if (p.res != nullptr) {
+        const float2 r = Pack2<T>::unpack(*reinterpret_cast<const uint32_t*>(static_cast<const T*>(p.res) + orow[0] * p.res_ld + col));
+        v0 += r.x; v1 += r.y;
+      }
+      const uint32_t pk = Pack2<T>::pack(v0, v1);
+      for (int rep = 0; rep < nrep; ++rep)
+        *reinterpret_cast<uint32_t*>(static_cast<T*>(p.out) + orow[rep] * p.out_ld + col) = pk;
     }
   }
 }
 
 // Detection-head epilogue with the decode fused in (yb_net_detect): instead of storing the fp32 feature map
-// (model.py:55-58) for predict_kernel and nms_compact_kernel to re-read, every thread turns its accumulator row — one
-// grid cell, 3 anchors x E = 5 + C logits, all inside this n-tile — into 3 boxes (model.py:82-137, 182-188) and appends
-// the (box, class) pairs with score = sigmoid(conf) * sigmoid(prob) >= thr (test_single_image.py:55,
-// utils/nms_utils.py:30) to the per-(image, class) candidate lists of the NMS (csrc/nms.cu).  Same arithmetic as
-// predict_kernel (decode.cuh), so boxes and scores are bit-identical to the unfused path; the feature maps, the
-// [n, B, C] score tensor and their ~440 MB of HBM round trips at batch 64 never exist.
-//   phase 1: the 3 x 5 box / objectness logits come from three 16-column TMEM reads -> boxes stored, conf kept;
-//            a warp none of whose 96 (row, anchor) pairs reaches conf >= thr is done (score <= conf).
-//   phase 2: the class logits, chunk by chunk: TMEM -> registers -> the thread's own row of the staging tile, then a
-//            ROLLED loop over the columns (column -> (anchor, class) carried as warp-uniform counters), so the code
-//            stays small (see the instruction-cache note above).
+// (model.py:55-58) for predict_kernel and nms_compact_kernel to re-read, every row — one grid cell, 3 anchors x
+// E = 5 + C logits, all inside this n-tile — becomes 3 boxes (model.py:82-137, 182-188) and the (box, class) pairs with
+// score = sigmoid(conf) * sigmoid(prob) >= thr (test_single_image.py:55, utils/nms_utils.py:30) are appended to the
+// per-(image, class) candidate lists of the NMS (csrc/nms.cu).  Same arithmetic as predict_kernel (decode.cuh), so
+// boxes and scores are bit-identical to the unfused path; the feature maps and the [n, B, C] score tensor never exist.
+// The columns arrive chunk by chunk through the staging tile; threads 0..63 of the warpgroup (warps 0 and 1) own one
+// row each and walk its columns with (anchor, element) carried as warp-uniform counters.
 template <int BN, int E>
-__device__ __forceinline__ void epilogue_tile_detect(const ConvParams& p, const int row, const uint32_t t_row,
-                                                     const int lane, const float* s_ss, float* stage) {
+__device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float (&acc)[BN / 2], const int row0, const int t,
+                                                float* stg, const float* s_ss, const int bar_id) {
   static_assert(3 * E <= BN, "all three anchors must lie in one n-tile");
-  static_assert((E % 16) <= 11 && ((2 * E) % 16) <= 11, "an anchor's 5 head logits must fit one aligned 16-column read");
   const DetParams& d = p.det;
-  const bool row_ok = row < p.M;
+  const int lane = t & 31;
+  const bool walker = t < WG_ROWS;                             // warp-uniform
+  const int row = row0 + t;
+  const bool row_ok = walker && row < p.M;
   const int cells = p.P * p.Q;
-  const int img = row_ok ? row / cells : -1 - lane;          // rows past M: distinct dummies, never grouped, never stored
+  const int img = row_ok ? row / cells : -1 - lane;            // rows past M: distinct dummies, never grouped, never stored
   const int cell = row_ok ? row - img * cells : 0;
   const unsigned same = __match_any_sync(0xffffffffu, img);   // lanes of my image (candidate slots are reserved per image)
   const unsigned lt = (1u << lane) - 1u;
   const float offx = (float)(cell % p.Q), offy = (float)(cell / p.Q);
   const int box0 = d.box_off + cell * 3;
-  // ---- phase 1: boxes + objectness ----
-  uint32_t h0[16], h1[16], h2[16];
-  tmem_ld_32x16(t_row + ((0 * E) & ~15), h0);
-  tmem_ld_32x16(t_row + ((1 * E) & ~15), h1);
-  tmem_ld_32x16(t_row + ((2 * E) & ~15), h2);
-  tmem_ld_wait();
-  float conf[3];
-  bool ok[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const uint32_t (&h)[16] = a == 0 ? h0 : (a == 1 ? h1 : h2);
-    constexpr int dummy = 0; (void)dummy;
-    const int o = (a * E) & 15, c0 = a * E;
-    float t[5];
-#pragma unroll
-    for (int k = 0; k < 5; ++k) t[k] = fmaf(__uint_as_float(h[o + k]), s_ss[c0 + k], s_ss[BN + c0 + k]);   // scale 1, shift = bias
-    conf[a] = sigmoid_ref(t[4]);                               // model.py:167
-    ok[a] = row_ok && conf[a] >= d.thr;                        // score = conf * prob <= conf: nothing below thr can pass
-    if (row_ok) {
-      float4 b;
-      decode_axis(t[0], t[2], offx, d.ratio_w, d.anchor_w[a], b.x, b.z);
-      decode_axis(t[1], t[3], offy, d.ratio_h, d.anchor_h[a], b.y, b.w);
-      reinterpret_cast<float4*>(d.boxes)[(long)img * d.B + box0 + a] = b;
-    }
-  }
-  const bool any0 = __any_sync(0xffffffffu, ok[0]), any1 = __any_sync(0xffffffffu, ok[1]), any2 = __any_sync(0xffffffffu, ok[2]);
-  if (!(any0 || any1 || any2)) return;
-  // ---- phase 2: class scores ----
   constexpr int NCH = (3 * E + 31) / 32;
-  float* myrow = stage + lane * 33;
-  int a = 0, e = 0;                                            // (anchor, element) of the current column: warp-uniform
-  float cconf = conf[0];
-  bool cok = ok[0], cany = any0;
-  auto body = [&](const uint32_t (&r)[32], const int ch) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) myrow[j] = __uint_as_float(r[j]);
+  int a = 0, e = 0;
+  float h0 = 0.f, h1 = 0.f, h2 = 0.f, h3 = 0.f;               // the anchor's x, y, w, h logits
+  float cconf = 0.f;
+  bool cok = false, cany = false;
+#pragma unroll 1
+  for (int ch = 0; ch < NCH; ++ch) {
+    warpgroup_bar(bar_id);                                     // the previous chunk's readers are done with the tile
+    wgmma_stage_chunk<BN>(acc, ch, stg, EPI_LD, t);
+    warpgroup_bar(bar_id);
+    if (!walker) continue;
+    const float* myrow = stg + t * EPI_LD;
     const int ncol = min(32, 3 * E - ch * 32);
-#pragma unroll 2
+#pragma unroll 1
     for (int j = 0; j < ncol; ++j) {
       const int col = ch * 32 + j;
-      if (e >= 5 && cany) {
-        const float v = fmaf(myrow[j], s_ss[col], s_ss[BN + col]);
+      const float v = fmaf(myrow[j], s_ss[col], s_ss[BN + col]);   // scale 1, shift = bias
+      if (e < 5) {
+        if (e == 0) h0 = v;
+        else if (e == 1) h1 = v;
+        else if (e == 2) h2 = v;
+        else if (e == 3) h3 = v;
+        else {
+          cconf = sigmoid_ref(v);                              // model.py:167
+          cok = row_ok && cconf >= d.thr;                      // score = conf * prob <= conf: nothing below thr can pass
+          if (row_ok) {
+            float4 b;
+            decode_axis(h0, h2, offx, d.ratio_w, d.anchor_w[a], b.x, b.z);
+            decode_axis(h1, h3, offy, d.ratio_h, d.anchor_h[a], b.y, b.w);
+            reinterpret_cast<float4*>(d.boxes)[(long)img * d.B + box0 + a] = b;
+          }
+          cany = __any_sync(0xffffffffu, cok);
+        }
+      } else if (cany) {
         bool pass = false;
         float sc = 0.f;
         if (cok && v >= d.logit_lo) {
@@ -496,113 +280,62 @@ __device__ __forceinline__ void epilogue_tile_detect(const ConvParams& p, const 
           }
         }
       }
-      if (++e == E) {
-        e = 0; ++a;
-        cconf = a == 1 ? conf[1] : conf[2];
-        cok = a == 1 ? ok[1] : ok[2];
-        cany = a == 1 ? any1 : any2;
-      }
-    }
-  };
-  uint32_t ra[32], rb[32];
-  tmem_ld_32x32(t_row, ra);
-#pragma unroll 1
-  for (int ch = 0; ch < NCH; ch += 2) {
-    tmem_ld_wait();
-    if (ch + 1 < NCH) tmem_ld_32x32(t_row + (ch + 1) * 32, rb);
-    body(ra, ch);
-    if (ch + 1 < NCH) {
-      tmem_ld_wait();
-      if (ch + 2 < NCH) tmem_ld_32x32(t_row + (ch + 2) * 32, ra);
-      body(rb, ch + 1);
+      if (++e == E) { e = 0; ++a; }
     }
   }
 }
 
-template <typename T, int BN, int BK, int EG = 1>
-__global__ void __launch_bounds__(nthreads(EG), 1)
+template <typename T, int BN, int BK, int NC, int DET_E = 0>   // DET_E = 5 + classes: detection head with the decode fused in
+__global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
-  using C = Cfg<BN, BK, EG>;
+  using C = Cfg<BN, BK, NC>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
-  // and every staging-tile access then compiles to LD.E / ST.E + MEMBAR.ALL.CTA instead of LDS / STS (profiles/r02_b)
+  // and every staging-tile access then compiles to generic loads / stores instead of LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int kb_per_tap_ = p.cin / BK;
-  const int num_kb_ = p.kh * p.kw * kb_per_tap_;
-  // operand ring: [nst x A][nst x B], or with resident weights [nst x A][num_kb x B] (B loaded once per CTA)
-  int nst = C::STAGES;
-  const int kps = p.kps;                 // slots per barrier group (1: one handshake per k-block)
-  if (kps > 1) nst = (C::STAGES / kps);  // number of groups; slot index = group * kps + j
-  if (p.b_resident) {
-    nst = (C::RING - num_kb_ * C::B_BYTES) / C::A_BYTES;
-    if (nst > 8) nst = 8;
-  }
   uint8_t* sA = smem;
-  uint8_t* sB = smem + nst * (kps > 1 ? kps : 1) * C::A_BYTES;
-  float* stage_base = reinterpret_cast<float*>(smem + C::RING);              // 4 * EG x STAGE_BYTES_W, 1024-aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::RING + 4 * EG * STAGE_BYTES_W);
-  uint64_t* full_bar = bars;                       // [<=8] TMA -> MMA
-  uint64_t* empty_bar = bars + 8;                  // [<=8] MMA -> TMA
-  uint64_t* tfull_bar = bars + 16;                 // [2] MMA -> epilogue
-  uint64_t* tempty_bar = bars + 18;                // [2] epilogue -> MMA
-  uint64_t* bres_bar = bars + 20;                  // resident weights landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 30);
-  uint64_t* res_bar = bars + 32;                   // [4 * EG warps][EPI_TILES] residual tile landed (TMA)
-  float* s_stat = reinterpret_cast<float*>(smem + C::RING + 4 * EG * STAGE_BYTES_W + BAR_BYTES);   // [2][BN] per-CTA column sums / sums of squares
-  float* s_ss = s_stat + 2 * BN;                   // [EG][2][BN] scale / shift of each epilogue group's current n-tile
+  uint8_t* sB = smem + C::STAGES * C::A_BYTES;
+  float* s_epi = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);   // [NC][64][EPI_LD] staging tiles
+  float* s_stat = s_epi + NC * EPI_FLOATS;               // [NC][2][BN] per-CTA column sums / sums of squares
+  float* s_ss = s_stat + NC * 2 * BN;                    // [NC][2][BN] scale / shift of each warpgroup's current n-tile
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_ss + NC * 2 * BN);   // [STAGES] TMA -> MMA
+  uint64_t* empty_bar = full_bar + 8;                    // [STAGES] MMA -> TMA: one arrive per consumer warp of the cluster
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  const int wg = threadIdx.x >> 7;
+  const int cs = p.cluster;                              // CTAs per cluster (1: no cluster, no multicast)
+  const uint32_t rank = cs > 1 ? cluster_ctarank() : 0u;
+  const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
+  const int nunits = num_units(p);
   const int kb_per_tap = p.cin / BK;
   const int num_kb = p.kh * p.kw * kb_per_tap;
-  if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[10 * 64 * 32] = clock64();
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 4 * NC * cs);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);  // one arrive per epilogue warp
-    }
-    mbar_init(bres_bar, 1);
-    for (int i = 0; i < 4 * EG * EPI_TILES; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[10 * 64 * 32 + 1] = clock64();
+  if (cs > 1) cluster_sync_all();                        // every peer's barriers exist before the first multicast
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    int stage = 0;
-    uint32_t phase = 0;
-    if (p.b_resident && lane == 0 && (int)blockIdx.x < num_tiles) {
-      mbar_arrive_expect_tx(bres_bar, (uint32_t)(num_kb * C::B_BYTES));
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int tap = kb / kb_per_tap;
-        tma_load_2d(sB + kb * C::B_BYTES, &tmB, bres_bar, tap * p.cin + (kb - tap * kb_per_tap) * BK, 0);
-      }
-    }
-    // One lane runs the whole loop: a k-block costs one barrier wait, one expect_tx and two TMA issues.  The filter
-    // tap / channel-chunk coordinates are carried as counters — the first version recomputed them with three integer
-    // divisions per k-block and re-converged the warp every iteration, which (single thread, dependent instructions)
-    // cost about as much as the k-block's MMAs (profiles/r01_j).
-    if (lane == 0) {
-      const bool ld_a = !(p.dbg & 1), ld_b = !p.b_resident && !(p.dbg & 2);
-      const uint32_t tx_bytes = (ld_a ? C::A_BYTES : 0) + (ld_b ? C::B_BYTES : 0);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    // One thread runs the whole loop: a k-block costs one barrier wait, one expect_tx and two TMA issues.  The filter
+    // tap / channel-chunk coordinates are carried as counters instead of being divided out of the k-block index.
+    // In a cluster every CTA loads its own A tile and 1/cs of the shared weight tile, multicast to all cs CTAs.
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int b_rows = BN / cs;
+      const uint16_t mask = (uint16_t)((1u << cs) - 1u);
+      for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
         int m_idx, n_idx;
-        tile_coords(p, tile, m_idx, n_idx);
-        const int m0 = m_idx * BLOCK_M;
+        unit_coords(p, unit, rank, m_idx, n_idx);
+        const int m0 = m_idx * C::BLOCK_M;
         const int n0 = n_idx * BN;
         // first output pixel of the tile -> (image, row, col); base input pixel of the filter window
         const int q = m0 % p.Q;
@@ -611,515 +344,128 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int w_base = q * p.stride - p.pad;
         const int h_base = pp * p.stride - p.pad;
         int c0 = 0, tw = 0, th = 0, kcol = 0;                  // channel chunk, tap (tw, th), column in the packed weights
-        trace_stamp(p, 0, (tile - blockIdx.x) / gridDim.x, 0);
-        for (int kb = 0; kb < num_kb; kb += kps) {
-          // one handshake per group of kps k-blocks: the short-K-block layers (Cin = 32: two 32-cycle MMAs per
-          // k-block) were bound by ~230-440 ns of barrier round trip per k-block (profiles/r01_k_layers_infer.md)
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (tx_bytes) mbar_arrive_expect_tx(&full_bar[stage], tx_bytes * kps);
-          else mbar_arrive(&full_bar[stage]);
-          for (int j = 0; j < kps; ++j) {
-            const int slot = stage * kps + j;
-            if (ld_a) {
-              if (p.im2col) {
-                tma_load_im2col_4d(sA + slot * C::A_BYTES, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
-                                   (uint16_t)th);
-              } else {
-                tma_load_2d(sA + slot * C::A_BYTES, &tmA, &full_bar[stage], c0, m0);
-              }
-            }
-            if (ld_b) tma_load_2d(sB + slot * C::B_BYTES, &tmB, &full_bar[stage], kcol, n0);
-            c0 += BK; kcol += BK;
-            if (c0 == p.cin) { c0 = 0; if (++tw == p.kw) { tw = 0; ++th; } }
-          }
-          if (++stage == nst) { stage = 0; phase ^= 1; }
-        }
-        trace_stamp(p, 0, (tile - blockIdx.x) / gridDim.x, 1);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_f16(BLOCK_M, BN, sizeof(T) == 2 && std::is_same<T, __nv_bfloat16>::value);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    if (lane == 0) {
-      if (p.b_resident && (int)blockIdx.x < num_tiles) mbar_wait(bres_bar, 0);
-      const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        trace_stamp(p, 1, it, 0);
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);  // epilogue drained this accumulator
-        tcgen05_fence_after();
-        trace_stamp(p, 1, it, 1);
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; kb += kps) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          if (kb == 0) trace_stamp(p, 1, it, 2);
-          for (int j = 0; j < kps; ++j) {
-            const int slot = stage * kps + j;
-            const uint32_t a_addr = a_base + slot * C::A_BYTES;
-            const uint32_t b_addr = b_base + (p.b_resident ? kb : slot) * C::B_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t adesc = make_kmajor_desc(a_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              const uint64_t bdesc = make_kmajor_desc(b_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              if (!(p.dbg & 4)) umma_f16(d_tmem, adesc, bdesc, idesc, (kb | j | k) != 0);
-            }
-          }
-          umma_commit(&empty_bar[stage]);                             // smem slots reusable once these MMAs retire
-          if (kb + kps >= num_kb) umma_commit(&tfull_bar[acc]);       // accumulator complete
-          if (++stage == nst) { stage = 0; phase ^= 1; }
-        }
-        trace_stamp(p, 1, it, 3);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int quarter = warp & 3;  // TMEM lanes [32*quarter, 32*quarter+32) are this warp's
-    const int grp = (warp - 2) >> 2;               // epilogue group: drains accumulator stage grp, tiles with iteration % EG == grp
-    const int et = (threadIdx.x - 64) & 127;
-    s_ss += grp * 2 * BN;
-    int cur_n0 = -1, ss_n0 = -1;
-    if (p.stat_sum != nullptr) {
-      for (int c = et; c < 2 * BN; c += 128) s_stat[c] = 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-    int it = grp;
-    uint8_t* my_stage = reinterpret_cast<uint8_t*>(stage_base) + (warp - 2) * STAGE_BYTES_W;
-    EpiTmaState epi_st{my_stage, res_bar + (warp - 2) * EPI_TILES, 0u, false};
-    for (int tile = blockIdx.x + grp * gridDim.x; tile < num_tiles; tile += EG * gridDim.x, it += EG) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      int m_idx, n_idx;
-      tile_coords(p, tile, m_idx, n_idx);
-      const int m0 = m_idx * BLOCK_M;
-      const int n0 = n_idx * BN;
-      if (p.stat_sum != nullptr && n0 != cur_n0) {
-        if (cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
-        cur_n0 = n0;
-      }
-      if (n0 != ss_n0) { load_scale_shift<BN>(p, s_ss, n0, et, grp); ss_n0 = n0; }
-      const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN;
-      if (p.epi_tma) {
-        const int ntile = tile + EG * gridDim.x;
-        int nm = 0, nn = 0;
-        if (ntile < num_tiles) tile_coords(p, ntile, nm, nn);
-        if (lane == 0) trace_stamp(p, warp, it, 0);
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        tcgen05_fence_after();
-        if (lane == 0) trace_stamp(p, warp, it, 1);
-        if (!(p.dbg & 8))
-          epilogue_tile_tma<T, BN>(p, m0 + quarter * 32, n0, t_row, lane, epi_st, s_stat, s_ss, ntile < num_tiles,
-                                   nm * BLOCK_M + quarter * 32, nn * BN, warp, it);
-        if (lane == 0) trace_stamp(p, warp, it, 31);
-      } else {
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        tcgen05_fence_after();
-        if (!(p.dbg & 8))
-          epilogue_tile<T, BN>(p, m0 + quarter * 32 + lane, n0, t_row, lane, reinterpret_cast<float*>(my_stage), s_stat, s_ss);
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-    }
-    if (p.epi_tma && lane == 0) bulk_wait_group<0>();       // every TMA store of this warp has completed
-    if (p.stat_sum != nullptr && cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ----------------------------------------------------------------------------------
-// 2-CTA variant: a cluster of two CTAs (one SM pair) computes a 256 x BN tile with
-// tcgen05.mma.cta_group::2 (UMMA M = 256).  Each CTA loads only ITS 128 rows of A and
-// ITS half of the B tile, so the L2 -> shared fill per FLOP is half that of the 1-CTA
-// kernel (profiles/r01_a: the 1-CTA kernel is fill-bound at ~8 TB/s).  The leader CTA
-// (cluster rank 0) issues the MMAs; tcgen05.commit multicasts barrier arrivals to both
-// CTAs; each CTA drains its own 128 TMEM lanes in its own epilogue warps.
-// ----------------------------------------------------------------------------------
-template <int BN, int BK, int EG = 1>
-struct Cfg2 {
-  static constexpr int A_BYTES = BLOCK_M * BK * 2;         // this CTA's 128 rows
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;        // this CTA's half of the BN weight rows
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (ring_budget(EG) / STAGE_BYTES) > 8 ? 8 : (ring_budget(EG) / STAGE_BYTES);
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 4 * EG * STAGE_BYTES_W + BAR_BYTES + (2 + 2 * EG) * BN * 4;
-  static constexpr uint32_t SWIZZLE = (BK == 64) ? 2u : 4u;
-  static constexpr uint32_t SBO = 8 * BK * 2;
-};
-
-template <typename T, int BN, int BK, int DET_E = 0, int EG = 1>   // DET_E = 5 + classes: detection head with the decode fused in
-__global__ void __launch_bounds__(nthreads(EG), 1)
-conv_igemm_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const __grid_constant__ ConvParams p) {
-  using C = Cfg2<BN, BK, EG>;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
-  // and every staging-tile access then compiles to LD.E / ST.E + MEMBAR.ALL.CTA instead of LDS / STS (profiles/r02_b)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + C::STAGES * C::A_BYTES;
-  float* stage_base = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);   // 4 * EG x STAGE_BYTES_W, 1024-aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES + 4 * EG * STAGE_BYTES_W);
-  uint64_t* full_bar = bars;                        // [STAGES] used in the leader only
-  uint64_t* empty_bar = bars + C::STAGES;           // [STAGES] one per CTA (multicast commit)
-  uint64_t* tfull_bar = bars + 2 * C::STAGES;       // [2] one per CTA (multicast commit)
-  uint64_t* tempty_bar = bars + 2 * C::STAGES + 2;  // [2] used in the leader only (8 arrivals: 4 warps x 2 CTAs)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 30);
-  uint64_t* res_bar = bars + 32;                    // [4 warps][EPI_TILES] residual tile landed (TMA), CTA-local
-  float* s_stat = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 4 * EG * STAGE_BYTES_W + BAR_BYTES);
-  float* s_ss = s_stat + 2 * BN;                   // [EG][2][BN]
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();          // 0 = leader
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;   // m tiles are 256 rows here
-  const int kb_per_tap = p.cin / BK;
-  const int num_kb = p.kh * p.kw * kb_per_tap;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);
-    }
-    for (int i = 0; i < 4 * EG * EPI_TILES; ++i) mbar_init(&res_bar[i], 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm<C::TMEM_COLS>(tmem_slot);
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();                               // peer barriers are initialised before any remote arrive / TMA
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    int stage = 0;
-    uint32_t phase = 0;
-    if (lane == 0) {   // single-lane loop, tap / chunk coordinates as counters (see the 1-CTA kernel)
-      const bool ld_a = !(p.dbg & 1), ld_b = !(p.dbg & 2);
-      const uint32_t tx_bytes = 2 * ((ld_a ? C::A_BYTES : 0) + (ld_b ? C::B_BYTES : 0));
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        int m_idx, n_idx;
-        tile_coords(p, tile, m_idx, n_idx);
-        const int m0 = m_idx * (2 * BLOCK_M) + (int)rank * BLOCK_M;   // this CTA's 128 rows
-        const int n0 = n_idx * BN + (int)rank * (BN / 2);             // this CTA's half of B
-        const int q = m0 % p.Q;
-        const int pp = (m0 / p.Q) % p.P;
-        const int img = m0 / (p.Q * p.P);
-        const int w_base = q * p.stride - p.pad;
-        const int h_base = pp * p.stride - p.pad;
-        int c0 = 0, tw = 0, th = 0, kcol = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          if (ld_a) {
-            if (p.im2col) {
-              tma_load_im2col_4d_2sm(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, w_base, h_base, img,
-                                     (uint16_t)tw, (uint16_t)th);
-            } else {
-              tma_load_2d_2sm(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, m0);
-            }
+          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+          if (p.im2col) {
+            tma_load_im2col_4d(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
+                               (uint16_t)th);
+          } else {
+            tma_load_2d(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, m0);
           }
-          if (ld_b) tma_load_2d_2sm(sB + stage * C::B_BYTES, &tmB, &full_bar[stage], kcol, n0);
+          if (cs == 1) {
+            tma_load_2d(sB + stage * C::B_BYTES, &tmB, &full_bar[stage], kcol, n0);
+          } else {
+            tma_load_2d_multicast(sB + stage * C::B_BYTES + rank * b_rows * BK * 2, &tmB, &full_bar[stage], kcol,
+                                  n0 + (int)rank * b_rows, mask);
+          }
           c0 += BK; kcol += BK;
           if (c0 == p.cin) { c0 = 0; if (++tw == p.kw) { tw = 0; ++th; } }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(2 * BLOCK_M, BN, std::is_same<T, __nv_bfloat16>::value);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      if (lane == 0) {
-        const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-        for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-          const int acc = it & 1;
-          const uint32_t acc_phase = (it >> 1) & 1;
-          mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-          tcgen05_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * BN;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tcgen05_fence_after();
-            const uint32_t a_addr = a_base + stage * C::A_BYTES;
-            const uint32_t b_addr = b_base + stage * C::B_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t adesc = make_kmajor_desc(a_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              const uint64_t bdesc = make_kmajor_desc(b_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              if (!(p.dbg & 4)) umma_f16_2sm(d_tmem, adesc, bdesc, idesc, (kb | k) != 0);
-            }
-            umma_commit_2sm(&empty_bar[stage]);                       // frees the slot in BOTH CTAs
-            if (kb == num_kb - 1) umma_commit_2sm(&tfull_bar[acc]);   // accumulator ready in BOTH CTAs
-            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-      __syncwarp();
-    }
   } else {
-    // ===================== epilogue (warps 2..5, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int grp = (warp - 2) >> 2;               // epilogue group (see nthreads())
-    const int et = (threadIdx.x - 64) & 127;
-    s_ss += grp * 2 * BN;
-    int cur_n0 = -1, ss_n0 = -1;
-    if (p.stat_sum != nullptr) {
-      for (int c = et; c < 2 * BN; c += 128) s_stat[c] = 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-    int it = grp;
-    uint8_t* my_stage = reinterpret_cast<uint8_t*>(stage_base) + (warp - 2) * STAGE_BYTES_W;
-    EpiTmaState epi_st{my_stage, res_bar + (warp - 2) * EPI_TILES, 0u, false};
-    for (int tile = cluster_id + grp * num_clusters; tile < num_tiles; tile += EG * num_clusters, it += EG) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      int m_idx, n_idx;
-      tile_coords(p, tile, m_idx, n_idx);
-      const int m0 = m_idx * (2 * BLOCK_M) + (int)rank * BLOCK_M;
-      const int n0 = n_idx * BN;
-      if (p.stat_sum != nullptr && n0 != cur_n0) {
-        if (cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
-        cur_n0 = n0;
-      }
-      if (n0 != ss_n0) { load_scale_shift<BN>(p, s_ss, n0, et, grp); ss_n0 = n0; }
-      const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      if constexpr (DET_E > 0) {
-        if (!(p.dbg & 8)) epilogue_tile_detect<BN, DET_E>(p, m0 + quarter * 32 + lane, t_row, lane, s_ss, reinterpret_cast<float*>(my_stage));
-      } else if (p.epi_tma) {
-        const int ntile = tile + EG * num_clusters;
-        int nm = 0, nn = 0;
-        if (ntile < num_tiles) tile_coords(p, ntile, nm, nn);
-        if (!(p.dbg & 8))
-          epilogue_tile_tma<T, BN>(p, m0 + quarter * 32, n0, t_row, lane, epi_st, s_stat, s_ss, ntile < num_tiles,
-                                   nm * (2 * BLOCK_M) + (int)rank * BLOCK_M + quarter * 32, nn * BN);
-      } else if (!(p.dbg & 8)) {
-        epilogue_tile<T, BN>(p, m0 + quarter * 32 + lane, n0, t_row, lane, reinterpret_cast<float*>(my_stage), s_stat, s_ss);
-      }
-      tcgen05_fence_before();
+    // ===================== MMA + epilogue (warpgroup cw: rows [64 cw, 64 cw + 64) of every tile) =====================
+    constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int lane = t & 31;
+    const int bar_id = 1 + cw;
+    float* stg = s_epi + cw * EPI_FLOATS;
+    float* sst = s_stat + cw * 2 * BN;
+    float* sss = s_ss + cw * 2 * BN;
+    if (p.stat_sum != nullptr)
+      for (int c = t; c < 2 * BN; c += 128) sst[c] = 0.f;   // (first read after the scale / shift barriers below)
+    // a stage is released on the empty barrier of every CTA of the cluster: any of them may multicast into it next
+    auto release = [&](int st) {
       __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], 0);    // the leader's MMA warp waits for both CTAs
-    }
-    if (p.epi_tma && lane == 0) bulk_wait_group<0>();       // every TMA store of this warp has completed
-    if (p.stat_sum != nullptr && cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();                               // nobody exits while the peer may still signal / read its smem
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<C::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ----------------------------------------------------------------------------------
-// Cluster-multicast variant of the pair kernel, BN = 256: a cluster of CM x CN CTA pairs computes a
-// (CM*256) x (CN*256) super-tile.  The A tile of an m-tile is needed by the CN pairs of its row, the B tile of an
-// n-tile by the CM pairs of its column: each CTA fetches only 1/CN of its A rows and 1/CM of its B rows and the
-// TMA multicasts the box to the CTAs that share it, so the L2 -> shared-memory fill per FLOP drops by another
-// (1/CN + 1/CM)/2 (2x2: half of the pair kernel, a quarter of the 1-CTA kernel).
-// ----------------------------------------------------------------------------------
-template <typename T, int BK, int CM, int CN>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_igemm_mc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const __grid_constant__ ConvParams p) {
-  constexpr int BN = 256;
-  constexpr int CSIZE = 2 * CM * CN;
-  using C = Cfg2<BN, BK>;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
-  // and every staging-tile access then compiles to LD.E / ST.E + MEMBAR.ALL.CTA instead of LDS / STS (profiles/r02_b)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + C::STAGES * C::A_BYTES;
-  float* stage_base = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);   // 4 x STAGE_BYTES_W, 1024-aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES + 4 * STAGE_BYTES_W);
-  uint64_t* full_bar = bars;                        // [STAGES] used in the leader only
-  uint64_t* empty_bar = bars + C::STAGES;           // [STAGES] one per CTA (multicast commit)
-  uint64_t* tfull_bar = bars + 2 * C::STAGES;       // [2] one per CTA (multicast commit)
-  uint64_t* tempty_bar = bars + 2 * C::STAGES + 2;  // [2] used in the leader only (8 arrivals: 4 warps x 2 CTAs)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 30);
-  uint64_t* res_bar = bars + 32;                    // [4 warps][EPI_TILES] residual tile landed (TMA), CTA-local
-  float* s_stat = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 4 * STAGE_BYTES_W + BAR_BYTES);
-  float* s_ss = s_stat + 2 * BN;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const uint32_t rank = crank & 1;                  // 0 = leader of its pair
-  const int pid = crank >> 1, pn = pid % CN, pm = pid / CN;
-  const int cluster_id = blockIdx.x / CSIZE;
-  const int num_clusters = gridDim.x / CSIZE;
-  const int SM_T = (p.num_m_tiles + CM - 1) / CM, SN_T = p.num_n_tiles / CN;   // super-tiles
-  const int num_tiles = SM_T * SN_T;
-  const int kb_per_tap = p.cin / BK;
-  const int num_kb = p.kh * p.kw * kb_per_tap;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CM * CN);              // every pair leader of the cluster commits to it
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);
-    }
-    for (int i = 0; i < 4 * EPI_TILES; ++i) mbar_init(&res_bar[i], 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm<C::TMEM_COLS>(tmem_slot);
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();                               // peer barriers are initialised before any remote arrive / TMA
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    int stage = 0;
+      if (lane == 0) {
+        if (cs == 1) mbar_arrive(&empty_bar[st]);
+        else for (int r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
+      }
+    };
+    float acc[BN / 2];
+    int stage = 0, prev = 0;
     uint32_t phase = 0;
-    // multicast masks: A goes to the CTAs with the same (pm, rank), B to those with the same (pn, rank)
-    uint16_t maskA = 0, maskB = 0;
-#pragma unroll
-    for (int j = 0; j < CN; ++j) maskA |= (uint16_t)(1u << (((pm * CN + j) << 1) | rank));
-#pragma unroll
-    for (int j = 0; j < CM; ++j) maskB |= (uint16_t)(1u << (((j * CN + pn) << 1) | rank));
-    constexpr int A_ROWS = BLOCK_M / CN, B_ROWS = (BN / 2) / CM;   // rows this CTA fetches itself
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-      int sm, sn;
-      if (p.stat_sum != nullptr) { sn = tile / SM_T; sm = tile - sn * SM_T; } else { sm = tile / SN_T; sn = tile - sm * SN_T; }
-      const int m_idx = sm * CM + pm, n_idx = sn * CN + pn;
-      const int m0 = m_idx * (2 * BLOCK_M) + (int)rank * BLOCK_M + pn * A_ROWS;   // first A row this CTA fetches
-      const int n0 = n_idx * BN + (int)rank * (BN / 2) + pm * B_ROWS;             // first B row this CTA fetches
-      const int q = m0 % p.Q;
-      const int pp = (m0 / p.Q) % p.P;
-      const int img = m0 / (p.Q * p.P);
-      const int w_base = q * p.stride - p.pad;
-      const int h_base = pp * p.stride - p.pad;
+    int cur_n0 = -1, ss_n0 = -1;
+    const uint32_t a_off = cw * WG_ROWS * BK * 2;
+    for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
+      int m_idx, n_idx;
+      unit_coords(p, unit, rank, m_idx, n_idx);
+      const int m0 = m_idx * C::BLOCK_M;
+      const int n0 = n_idx * BN;
       for (int kb = 0; kb < num_kb; ++kb) {
-        const int tap = kb / kb_per_tap;
-        const int c0 = (kb - tap * kb_per_tap) * BK;
-        if (lane == 0) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);   // both CTAs' bytes
-          uint8_t* adst = sA + stage * C::A_BYTES + pn * A_ROWS * (BK * 2);
-          uint8_t* bdst = sB + stage * C::B_BYTES + pm * B_ROWS * (BK * 2);
-          if (p.im2col) {
-            tma_load_im2col_4d_2sm_mc(adst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)(tap % p.kw),
-                                      (uint16_t)(tap / p.kw), maskA);
-          } else {
-            tma_load_2d_2sm_mc(adst, &tmA, &full_bar[stage], c0, m0, maskA);
-          }
-          tma_load_2d_2sm_mc(bdst, &tmB, &full_bar[stage], tap * p.cin + c0, n0, maskB);
-        }
-        __syncwarp();
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(sA + stage * C::A_BYTES) + a_off;
+        const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          Wgmma<BN, kBF16, 0, 0>::mma(acc, make_kmajor_desc(a_addr + k * 32, C::SBO, C::SWIZZLE),
+                                      make_kmajor_desc(b_addr + k * 32, C::SBO, C::SWIZZLE), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its stage is free
+        if (kb > 0) release(prev);
+        prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(2 * BLOCK_M, BN, std::is_same<T, __nv_bfloat16>::value);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        if (lane == 0) mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        __syncwarp();
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          if (lane == 0) {
-            mbar_wait(&full_bar[stage], phase);
-            tcgen05_fence_after();
-            const uint32_t a_addr = smem_u32(sA + stage * C::A_BYTES);
-            const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t adesc = make_kmajor_desc(a_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              const uint64_t bdesc = make_kmajor_desc(b_addr + k * UMMA_K * 2, C::SBO, C::SWIZZLE);
-              umma_f16_2sm(d_tmem, adesc, bdesc, idesc, (kb | k) != 0);
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      release(prev);
+
+      if (p.stat_sum != nullptr && n0 != cur_n0) {
+        if (cur_n0 >= 0) stat_flush<BN>(p, sst, cur_n0, t, bar_id);
+        cur_n0 = n0;
+      }
+      if (n0 != ss_n0) {
+        warpgroup_bar(bar_id);                   // nobody still reads the previous n-tile's values
+        for (int c = t; c < BN; c += 128) {
+          sss[c] = p.scale ? __ldg(p.scale + n0 + c) : 1.f;      // scale = shift = NULL: identity (dgrad convs)
+          sss[BN + c] = p.shift ? __ldg(p.shift + n0 + c) : 0.f;
+        }
+        warpgroup_bar(bar_id);
+        ss_n0 = n0;
+      }
+      const int row0 = m0 + cw * WG_ROWS;
+      if constexpr (DET_E > 0) {
+        epilogue_detect<BN, DET_E>(p, acc, row0, t, stg, sss, bar_id);
+      } else if (p.epi_reg) {
+        epilogue_reg<T, BN>(p, acc, row0, n0, sss, t);
+      } else {
+        const int nvalid = min(BN / 32, (p.cout - n0 + 31) >> 5);   // zero-padded weight rows (cout_pad > cout): not stored
+        const int er = t >> 1, eh = t & 1;       // this thread's row of the chunk and its 16-column half
+#pragma unroll 1
+        for (int ch = 0; ch < nvalid; ++ch) {
+          warpgroup_bar(bar_id);                 // the previous chunk's readers are done with the staging tile
+          wgmma_stage_chunk<BN>(acc, ch, stg, EPI_LD, t);
+          warpgroup_bar(bar_id);
+          if (p.stat_sum != nullptr) {           // BN batch statistics of the raw conv output: lane = column
+            const int col = t & 31, rg = (t >> 5) * 16;
+            float cs_ = 0.f, cs2 = 0.f;
+#pragma unroll 4
+            for (int rr = 0; rr < 16; ++rr) {
+              if (row0 + rg + rr < p.M) {
+                const float v = stg[(rg + rr) * EPI_LD + col];
+                cs_ += v;
+                cs2 = fmaf(v, v, cs2);
+              }
             }
-            umma_commit_2sm_mask(&empty_bar[stage], (uint16_t)((1u << CSIZE) - 1));     // one of CM*CN arrivals, in every CTA
-            if (kb == num_kb - 1) umma_commit_2sm_mask(&tfull_bar[acc], (uint16_t)(3u << (pid << 1)));   // own pair
+            atomicAdd(&sst[ch * 32 + col], cs_);
+            atomicAdd(&sst[BN + ch * 32 + col], cs2);
           }
-          __syncwarp();
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          if (row0 + er < p.M) {
+            const int cl = ch * 32 + eh * 16;
+            epi_store16<T>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl);
+          }
         }
       }
     }
-  } else {
-    // ===================== epilogue (warps 2..5, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int et = threadIdx.x - 64;
-    int cur_n0 = -1, ss_n0 = -1;
-    if (p.stat_sum != nullptr) {
-      for (int c = et; c < 2 * BN; c += 128) s_stat[c] = 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-    int it = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      int sm, sn;
-      if (p.stat_sum != nullptr) { sn = tile / SM_T; sm = tile - sn * SM_T; } else { sm = tile / SN_T; sn = tile - sm * SN_T; }
-      const int m0 = (sm * CM + pm) * (2 * BLOCK_M) + (int)rank * BLOCK_M;
-      const int n0 = (sn * CN + pn) * BN;
-      if (p.stat_sum != nullptr && n0 != cur_n0) {
-        if (cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
-        cur_n0 = n0;
-      }
-      if (n0 != ss_n0) { load_scale_shift<BN>(p, s_ss, n0, et); ss_n0 = n0; }
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      epilogue_tile<T, BN>(p, m0 + quarter * 32 + lane, n0, tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN, lane,
-                           stage_base + (warp - 2) * STAGE_FLOATS, s_stat, s_ss);   // (register-store epilogue only)
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], crank & ~1u);   // this pair's leader
-    }
-    if (p.stat_sum != nullptr && cur_n0 >= 0) stat_flush<BN>(p, s_stat, cur_n0, et);
+    if (p.stat_sum != nullptr && cur_n0 >= 0) stat_flush<BN>(p, sst, cur_n0, t, bar_id);
   }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();                               // nobody exits while the peer may still signal / read its smem
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<C::TMEM_COLS>(tmem_base);
-  }
+  if (cs > 1) cluster_sync_all();                        // no CTA exits while a peer may still multicast into it or arrive on it
 }
 
 // ----------------------------------------------------------------------------------
@@ -1215,7 +561,7 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
                         int stride, int pad, int bk, int pixels);
 int make_tmap_im2col(CUtensorMap* tm, const void* base, int dtype, int n, int h, int w, int c, long ld, int ksize,
                      int stride, int pad, int bk) {
-  return make_tmap_im2col_px(tm, base, dtype, n, h, w, c, ld, ksize, stride, pad, bk, BLOCK_M);
+  return make_tmap_im2col_px(tm, base, dtype, n, h, w, c, ld, ksize, stride, pad, bk, 128);
 }
 // `pixels` = output pixels gathered per request (rows of the shared-memory box)
 int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int h, int w, int c, long ld, int ksize,
@@ -1247,149 +593,70 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
   return YB_OK;
 }
 
-template <typename T, int BN, int BK, int EG = 1>
+template <typename T, int BN, int BK, int NC, int DET_E = 0>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
-  using C = Cfg<BN, BK, EG>;
+  using C = Cfg<BN, BK, NC>;
   static DeviceOnce once;
-  auto kern = conv_igemm_kernel<T, BN, BK, EG>;
+  auto kern = conv_igemm_kernel<T, BN, BK, NC, DET_E>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, nthreads(EG), C::SMEM_BYTES, st>>>(tmA, tmB, p);
-  YB_CUDA(cudaGetLastError());
-  return YB_OK;
-}
-
-template <typename T, int BN, int BK, int DET_E = 0, int EG = 1>
-static int launch_cfg2(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
-  using C = Cfg2<BN, BK, EG>;
-  static DeviceOnce once;
-  auto kern = conv_igemm_2cta_kernel<T, BN, BK, DET_E, EG>;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int max_clusters = num_sms() / 2;
-  const int clusters = tiles < max_clusters ? tiles : max_clusters;
+  const int cs = p.cluster;
+  const int units = ceil_div(p.num_m_tiles, cs) * p.num_n_tiles;
+  const int max_clusters = num_sms() / cs;
+  const int clusters = units < max_clusters ? units : max_clusters;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(nthreads(EG));
+  cfg.gridDim = dim3(clusters * cs);
+  cfg.blockDim = dim3(C::THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   YB_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
   return YB_OK;
 }
 
-template <typename T, int BK, int CM, int CN>
-static int launch_mc(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
-  using C = Cfg2<256, BK>;
-  constexpr int CSIZE = 2 * CM * CN;
-  static int max_clusters_dev[64];
-  static DeviceOnce once;
-  int dev = 0;
-  YB_CUDA(cudaGetDevice(&dev));
-  int& max_clusters = max_clusters_dev[dev & 63];
-  if (!(once.mask & (1ull << (dev & 63)))) max_clusters = -1;
-  auto kern = conv_igemm_mc_kernel<T, BK, CM, CN>;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CSIZE; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (max_clusters < 0) {
-    { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-    cfg.gridDim = dim3(CSIZE * (num_sms() / CSIZE));
-    int nc = 0;
-    YB_CUDA(cudaOccupancyMaxActiveClusters(&nc, kern, &cfg));
-    max_clusters = nc > 0 ? nc : 1;
-  }
-  const int super_tiles = ((p.num_m_tiles + CM - 1) / CM) * (p.num_n_tiles / CN);
-  const int clusters = super_tiles < max_clusters ? super_tiles : max_clusters;
-  cfg.gridDim = dim3(CSIZE * clusters);
-  YB_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
-  return YB_OK;
-}
-
-static long long* g_conv_trace = nullptr;   // yb_debug_set_conv_trace (tools only)
 int conv_block_k(int cin) { return (cin % 64 == 0) ? 64 : 32; }
-// 1-CTA tile width
 int conv_block_n(int cout_pad) { return (cout_pad % 128 == 0) ? 128 : 64; }
-// 2-CTA (pair) tile width
-int conv_block_n2(int cout_pad) { return (cout_pad % 256 == 0) ? 256 : ((cout_pad % 128 == 0) ? 128 : 64); }
 
-// Launch with prebuilt tensor maps (used by the network plan).  p.two_cta selects the kernel.
+// Launch with prebuilt tensor maps (used by the network plan).
 int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
                 cudaStream_t st) {
   const int bk = conv_block_k(p.cin);
-  if (p.two_cta && p.mc_m * p.mc_n > 1) {
-#define YB_DISPATCH_MC(T)                                                                  \
-  if (bk == 64 && p.mc_m == 2 && p.mc_n == 2) return launch_mc<T, 64, 2, 2>(tmA, tmB, p, st); \
-  if (bk == 64 && p.mc_m == 2 && p.mc_n == 1) return launch_mc<T, 64, 2, 1>(tmA, tmB, p, st);
-    if (dtype == YB_F16) { YB_DISPATCH_MC(__half) }
-    else if (dtype == YB_BF16) { YB_DISPATCH_MC(__nv_bfloat16) }
-#undef YB_DISPATCH_MC
-    set_error("conv_launch: unsupported multicast configuration");
-    return YB_ERR_UNSUPPORTED;
-  }
   if (p.det.on) {
-    // detection head with the decode fused in: pair kernel, one n-tile holding all 3 * E columns
-    const int bn = conv_block_n2(cout_pad);
-#define YB_DISPATCH_DET(T)                                                                                                  \
-  if (bn == 256 && bk == 64 && p.det.E == 85 && p.epi_groups == 2) return launch_cfg2<T, 256, 64, 85, 2>(tmA, tmB, p, st); \
-  if (bn == 256 && bk == 64 && p.det.E == 85) return launch_cfg2<T, 256, 64, 85>(tmA, tmB, p, st);                         \
-  if (bn == 128 && bk == 64 && p.det.E == 25) return launch_cfg2<T, 128, 64, 25>(tmA, tmB, p, st);
-    if (p.two_cta && dtype == YB_F16) { YB_DISPATCH_DET(__half) }
-    else if (p.two_cta && dtype == YB_BF16) { YB_DISPATCH_DET(__nv_bfloat16) }
+    // detection head with the decode fused in: one n-tile holding all 3 * E columns
+#define YB_DISPATCH_DET(T)                                                                            \
+  if (cout_pad == 256 && bk == 64 && p.det.E == 85) return launch_cfg<T, 256, 64, 2, 85>(tmA, tmB, p, st); \
+  if (cout_pad == 128 && bk == 64 && p.det.E == 25) return launch_cfg<T, 128, 64, 2, 25>(tmA, tmB, p, st);
+    if (dtype == YB_F16) { YB_DISPATCH_DET(__half) }
+    else if (dtype == YB_BF16) { YB_DISPATCH_DET(__nv_bfloat16) }
 #undef YB_DISPATCH_DET
-    set_error("conv_launch: no fused-decode kernel for %d classes (tile %d x %d)", p.det.C, bn, bk);
+    set_error("conv_launch: no fused-decode kernel for %d classes (cout_pad %d, block k %d)", p.det.C, cout_pad, bk);
     return YB_ERR_UNSUPPORTED;
   }
-  if (p.two_cta) {
-    const int bn = conv_block_n2(cout_pad);
-#define YB_DISPATCH2(T)                                                         \
-  if (bn == 256 && bk == 64 && p.epi_groups == 2) return launch_cfg2<T, 256, 64, 0, 2>(tmA, tmB, p, st); \
-  if (bn == 256 && bk == 64) return launch_cfg2<T, 256, 64>(tmA, tmB, p, st); \
-  if (bn == 256 && bk == 32) return launch_cfg2<T, 256, 32>(tmA, tmB, p, st); \
-  if (bn == 128 && bk == 64) return launch_cfg2<T, 128, 64>(tmA, tmB, p, st); \
-  if (bn == 128 && bk == 32) return launch_cfg2<T, 128, 32>(tmA, tmB, p, st); \
-  if (bn == 64 && bk == 64) return launch_cfg2<T, 64, 64>(tmA, tmB, p, st);   \
-  if (bn == 64 && bk == 32) return launch_cfg2<T, 64, 32>(tmA, tmB, p, st);
-    if (dtype == YB_F16) { YB_DISPATCH2(__half) }
-    else if (dtype == YB_BF16) { YB_DISPATCH2(__nv_bfloat16) }
-#undef YB_DISPATCH2
-  } else {
-    const int bn = conv_block_n(cout_pad);
-#define YB_DISPATCH(T)                                                         \
-  if (bn == 128 && bk == 64 && p.epi_groups == 2) return launch_cfg<T, 128, 64, 2>(tmA, tmB, p, st); \
-  if (bn == 64 && bk == 64 && p.epi_groups == 2) return launch_cfg<T, 64, 64, 2>(tmA, tmB, p, st);   \
-  if (bn == 64 && bk == 32 && p.epi_groups == 2) return launch_cfg<T, 64, 32, 2>(tmA, tmB, p, st);   \
-  if (bn == 128 && bk == 64) return launch_cfg<T, 128, 64>(tmA, tmB, p, st); \
-  if (bn == 128 && bk == 32) return launch_cfg<T, 128, 32>(tmA, tmB, p, st); \
-  if (bn == 64 && bk == 64) return launch_cfg<T, 64, 64>(tmA, tmB, p, st);   \
-  if (bn == 64 && bk == 32) return launch_cfg<T, 64, 32>(tmA, tmB, p, st);
-    if (dtype == YB_F16) { YB_DISPATCH(__half) }
-    else if (dtype == YB_BF16) { YB_DISPATCH(__nv_bfloat16) }
+  const int bn = conv_block_n(cout_pad);
+  const int nc = p.consumers;
+#define YB_DISPATCH(T)                                                       \
+  if (bn == 128 && bk == 64) return nc == 2 ? launch_cfg<T, 128, 64, 2>(tmA, tmB, p, st) : launch_cfg<T, 128, 64, 1>(tmA, tmB, p, st); \
+  if (bn == 128 && bk == 32) return nc == 2 ? launch_cfg<T, 128, 32, 2>(tmA, tmB, p, st) : launch_cfg<T, 128, 32, 1>(tmA, tmB, p, st); \
+  if (bn == 64 && bk == 64) return nc == 2 ? launch_cfg<T, 64, 64, 2>(tmA, tmB, p, st) : launch_cfg<T, 64, 64, 1>(tmA, tmB, p, st);     \
+  if (bn == 64 && bk == 32) return nc == 2 ? launch_cfg<T, 64, 32, 2>(tmA, tmB, p, st) : launch_cfg<T, 64, 32, 1>(tmA, tmB, p, st);
+  if (dtype == YB_F16) { YB_DISPATCH(__half) }
+  else if (dtype == YB_BF16) { YB_DISPATCH(__nv_bfloat16) }
 #undef YB_DISPATCH
-  }
   set_error("conv_launch: unsupported dtype %d", dtype);
   return YB_ERR_UNSUPPORTED;
 }
 
 // Build maps + params for one conv.  x/w/out pointers are baked into maps/params.
 // win = 0: the forward rule (ksize x ksize, symmetric padding ksize/2); win = 1: kh x kw window at offsets >= 0.
+// det = 1: one n-tile spans the whole padded cout (the fused-decode detection heads).
 static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
                              const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
                              float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
-                             int* cout_pad_out, int force_pair = 0) {
+                             int* cout_pad_out, int det = 0) {
   YB_REQUIRE(win || d->ksize == 1 || d->ksize == 3, "conv: ksize must be 1 or 3 (got %d)", d->ksize);
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2 (got %d)", d->stride);
   YB_REQUIRE(!(d->ksize == 1 && d->stride != 1), "conv: 1x1 stride-2 is not on the YOLOv3 path");
@@ -1414,102 +681,36 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   const int bk = conv_block_k(d->cin);
   if (!win) { kh = d->ksize; kw = d->ksize; }
   const int pad = win ? 0 : d->ksize / 2;
+  const int bn = det ? cout_pad : conv_block_n(cout_pad);
   p->M = d->n * P * Q; p->P = P; p->Q = Q;
-  // a CTA pair per 256-row tile once there are enough tiles to occupy the 74 SM pairs
-  const char* force = opt("YB_CONV_MODE");      // "1cta" / "2cta": testing override
-  // (measured, profiles/r01_b: pairs win 1.4-1.6x on 256-wide tiles — half the L2->smem fill per FLOP — but lose on
-  //  64/128-wide tiles, whose short per-tile pipelines are dominated by the cross-CTA barrier latency)
-  bool two = cout_pad % 256 == 0 && (long)ceil_div(p->M, 2 * BLOCK_M) * (cout_pad / 256) >= 32;
-  if (force && force[0] == '1') two = false;
-  if (force && force[0] == '2') two = true;
-  if (force_pair) two = true;
-  p->two_cta = two ? 1 : 0;
-  // cluster multicast on top of the pair kernel: 2x2 pairs when there are >= 2 n-tiles, 2x1 (share B) otherwise
-  int mc_m = 1, mc_n = 1;
-  const char* mcf = opt("YB_CONV_MC");          // "0": off, "1": force on where legal (testing)
-  if (two && bk == 64 && cout_pad % 256 == 0 && !(mcf && mcf[0] == '0')) {
-    const int mt = ceil_div(p->M, 2 * BLOCK_M), nt = cout_pad / 256;
-    // measured (profiles/r01_e): +10 % per SM but only 120-132 SMs are schedulable in 8-/4-CTA clusters -> no net gain;
-    // the multicast kernel therefore stays opt-in (YB_CONV_MC=1)
-    const bool big = (mcf && mcf[0] == '1');
-    if (big && mt >= 2) { mc_m = 2; mc_n = (nt % 2 == 0) ? 2 : 1; }
-  }
-  p->mc_m = mc_m; p->mc_n = mc_n;
-  p->dbg = opt_int("YB_CONV_DBG", 0);
-  p->trace = g_conv_trace;
+  // Kernel variants (testing / A-B switches; the detection heads always take the default):
+  //   YB_CONV_EG=1        one consumer warpgroup per CTA (64-row tiles) instead of two (128-row tiles)
+  //   YB_CONV_MODE=2cta   clusters of 2 CTAs (YB_CONV_MC=1: 4) along M sharing one TMA-multicast weight tile
+  //   YB_CONV_EPI=reg     accumulators stored straight from registers (not with BN statistics: those sum columns
+  //                       over the staging tile)
+  p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
+  p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
+  p->epi_reg = (!det && !stat_sum && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  const int block_m = 64 * p->consumers;
   memset(&p->det, 0, sizeof(p->det));
-  p->kps = 1;   // set below once the tile shape is known
-  const int bn = two ? conv_block_n2(cout_pad) : conv_block_n(cout_pad);
-  // Two epilogue groups for the layers whose mainloop is shorter than their epilogue (1x1 convs; no BN
-  // statistics, no multicast): the kernels exist for 1-CTA 128x{128,64} / BK 64, 128x64 / BK 32 and the 256-wide pair.
-  {
-    const char* eg = opt("YB_CONV_EG");          // "1": always one group (A/B), "2": two groups wherever a kernel exists
-    const bool have = two ? (bn == 256 && bk == 64) : ((bn == 128 && bk == 64) || (bn == 64));
-    const bool want = (kh * kw == 1 || (eg[0] == '2'));   // (Cin <= 64 3x3 layers are TMA-row bound: the smaller ring costs them 15-25 %, r02_c)
-    p->epi_groups = (have && want && !stat_sum && mc_m * mc_n == 1 && eg[0] != '1') ? 2 : 1;
-  }
-  const int ring = ring_budget(p->epi_groups);
-  {
-    // resident weights (1-CTA kernel): one n-tile, and the [BN, K] tile leaves room for >= 3 A stages
-    const long b_bytes = (long)kh * kw * d->cin * bn * 2;
-    const char* br = opt("YB_CONV_BRES");
-    p->b_resident = (!two && cout_pad == bn && ring - b_bytes >= 3L * BLOCK_M * bk * 2 && (br && br[0] == '1')) ? 1 : 0;   // opt-in: measured no gain (profiles/r01_i)
-  }
-  if (!two && !p->b_resident) {
-    // k-blocks per barrier phase in the 1-CTA kernel: the largest of {4, 3, 2} that divides the k-block count and still
-    // leaves two groups in the ring.  YB_CONV_KPS=0 restores one handshake per k-block.
-    const char* ke = opt("YB_CONV_KPS");
-    const bool on = !(ke && ke[0] == '0');
-    const int num_kb = kh * kw * (d->cin / bk);
-    const long stage_bytes = (long)(BLOCK_M + bn) * bk * 2;
-    int stages = (int)(ring / stage_bytes);
-    if (stages > 8) stages = 8;
-    if (on)
-      for (int c = 4; c >= 2; --c)
-        if (num_kb % c == 0 && stages / c >= 2) { p->kps = c; break; }
-  }
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
   p->kh = kh; p->kw = kw; p->scatter = scatter;
   p->im2col = kh * kw > 1;
-  p->num_m_tiles = ceil_div(p->M, two ? 2 * BLOCK_M : BLOCK_M);
+  p->num_m_tiles = ceil_div(p->M, block_m);
   p->num_n_tiles = cout_pad / bn;
   p->scale = scale; p->shift = shift;
   p->out = out; p->out_ld = d->out_ld; p->res = res; p->res_ld = d->res_ld;
   p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
   p->stat_sum = stat_sum; p->stat_sqsum = stat_sqsum;
   int rc;
-  // 16-bit outputs leave through shared memory + TMA stores (YB_CONV_EPI=reg: the register-store epilogue of round 1);
-  // the multicast kernel, the 2x-upsampling / parity-scatter stores and the fp32 heads keep the register path
-  {
-    // epi_tma: 1 (default) TMA stores / TMA residual loads, 0 register stores (YB_CONV_EPI=reg).  A third variant (staging
-    // tile drained by coalesced st.global, residual prefetched through registers) measured equal on the plain layers
-    // and 1.5x slower on the residual ones (a one-chunk register prefetch cannot hide a DRAM miss): removed (r02_b).
-    // Convs that also produce BN batch statistics keep the register epilogue: its column sums go through the staging tile.
-    // A fourth variant (no staging at all: each lane stores its row's chunk as two 256-bit st.global.v8, residual by
-    // ld.global.v8 one chunk ahead) halved the epilogue's own time (2.9 k vs 4.6 k cycles per 128x128 tile) but not the
-    // layers': the 1x1 layers are then paced by the operand fill, and the residual layers lost 20 % because a register
-    // prefetch cannot hide a DRAM miss the way the TMA's 3-tile rotation does: removed (profiles/r02_c).
-    const char* ep = opt("YB_CONV_EPI");
-    p->epi_tma = (!d->out_fp32 && !d->upsample2x && !scatter && mc_m * mc_n == 1 && !stat_sum && !(ep[0] == 'r')) ? 1 : 0;
-    memset(&p->tmO, 0, sizeof(p->tmO));
-    memset(&p->tmR, 0, sizeof(p->tmR));
-    if (p->epi_tma) {
-      rc = make_tmap_2d(&p->tmO, out, d->dtype, p->M, d->cout, d->out_ld, 32, 32, 0);
-      if (rc) return rc;
-      if (res) {
-        rc = make_tmap_2d(&p->tmR, res, d->dtype, p->M, d->cout, d->res_ld, 32, 32, 0);
-        if (rc) return rc;
-      }
-    }
-  }
   if (p->im2col) {
     rc = make_tmap_im2col_px(tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride, pad, bk,
-                             BLOCK_M / mc_n);
+                             block_m);
   } else {
-    rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, BLOCK_M / mc_n, bk, 0);
+    rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, block_m, bk, 0);
   }
   if (rc) return rc;
-  rc = make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, (two ? bn / 2 : bn) / mc_m, bk, 1);
+  rc = make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, bn / p->cluster, bk, 1);
   if (rc) return rc;
   *cout_pad_out = cout_pad;
   return YB_OK;
@@ -1522,13 +723,13 @@ int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, con
                            cout_pad_out);
 }
 
-// Detection head with the decode fused into the epilogue (yb_net_detect): always the pair kernel with ONE n-tile that
-// holds all 3 * (5 + C) columns; `out` is never written.  YB_ERR_UNSUPPORTED when the class count has no kernel.
+// Detection head with the decode fused into the epilogue (yb_net_detect): ONE n-tile that holds all 3 * (5 + C)
+// columns; `out` is never written.  YB_ERR_UNSUPPORTED when the class count has no kernel.
 int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
                      const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out) {
   const int E = 5 + class_num;
-  const int bn = conv_block_n2(yb_conv_cout_pad(d->cout));
-  if (d->cout != 3 * E || conv_block_k(d->cin) != 64 || !((bn == 256 && E == 85) || (bn == 128 && E == 25))) {
+  const int cout_pad = yb_conv_cout_pad(d->cout);
+  if (d->cout != 3 * E || conv_block_k(d->cin) != 64 || !((cout_pad == 256 && E == 85) || (cout_pad == 128 && E == 25))) {
     set_error("fused decode: no kernel for %d classes", class_num);
     return YB_ERR_UNSUPPORTED;
   }
@@ -1548,10 +749,6 @@ int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const v
 }  // namespace yb
 
 extern "C" int yb_conv_cout_pad(int cout) { return (cout + 63) / 64 * 64; }
-
-// tools/conv_trace.py: convs PREPARED after this call stamp CTA 0's pipeline events (clock64) into `buf`
-// ([10 warps][64 tile iterations][32 slots] + 2 (kernel entry, set-up done) int64, caller-zeroed); NULL switches it off again.
-extern "C" int yb_debug_set_conv_trace(long long* buf) { yb::g_conv_trace = buf; return YB_OK; }
 
 extern "C" int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
                              const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,

@@ -2,7 +2,7 @@
 // layers darknet53_body/Conv_1, Conv_3; utils/layer_utils.py:35-36,27): they are HBM-bound (12-64 B in,
 // 64-128 B out per pixel, <= 1.6 GFLOP/img) and the implicit-GEMM path is a poor fit for them — with 32
 // input channels an im2col row is 64 B, which halves the TMA line rate, and every input pixel is re-fetched
-// 9x from L2 (profiles/r01_b: 630 us per layer against a 140-160 us HBM bound).  Here every input pixel is
+// 9x from L2.  Here every input pixel is
 // read from global memory ONCE per tile into a shared-memory halo tile, the (tiny) weight matrix stays
 // resident in shared memory, and the 9-tap reduction runs out of shared memory on the warp-level tensor
 // path (ldmatrix + mma.sync m16n8k16, fp32 accumulate) — per-warp gathers through ldmatrix row addresses
@@ -114,8 +114,7 @@ conv_thin_kernel(const ThinParams p) {
   }
 
   // stem: the NEXT tile's halo (float32 image) is fetched into registers while the current tile is processed — a
-  // tile's 540 scalar loads were issued and awaited serially before, 43 % of the kernel (profiles/r01_j: 665 -> 379 us
-  // with the loads removed)
+  // tile's 540 scalar loads would otherwise be issued and awaited serially
   constexpr int HN = STEM ? C::HH * C::HW * 3 : 1;
   constexpr int NL = (HN + THIN_THREADS - 1) / THIN_THREADS;
   float pre[NL];

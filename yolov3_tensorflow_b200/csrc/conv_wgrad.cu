@@ -2,16 +2,15 @@
 //
 //   dW[co, (r,s), ci] = sum_p  dz[p, co] * x[n(p), h(p)*stride + r - pad, w(p)*stride + s - pad, ci]
 //
-//   M = co (128 per tile), N = ci chunk of one filter tap (BNW = 32..128), K = pixels.
+//   M = co (128 per tile, 64 per consumer warpgroup), N = ci chunk of one filter tap (BNW = 32..128), K = pixels.
 //   A = dz^T   : 2D tiled TMA boxes {64 co x 64 pixels} -> smem rows = pixels, 128 B of co
-//                per row: the canonical *MN-major* 128B-swizzled UMMA layout.
+//                per row: the canonical *MN-major* 128B-swizzled wgmma layout.
 //   B = x_col^T: TMA im2col boxes {BCH channels x 64 pixels} of filter tap (r,s) — the same
 //                zero-filled border/stride handling as the forward conv — also MN-major.
-//   D = fp32 in TMEM; every CTA reduces one pixel range (split-K) of one output tile and
+//   D = fp32 in registers (wgmma); every CTA reduces one pixel range (split-K) of one output tile and
 //       adds it into the fp32 gradient with vector atomics.
-//   A CTA accumulates TP filter taps at once (TP x BNW TMEM columns: one kernel row of a 3x3 filter, or all 9 taps
-//   when cin = 32): the dz tile is loaded once per TP taps instead of once per tap — the first version re-read dz
-//   9x and, on the 208x208 / 104x104 layers whose dz + x exceed the L2, ran at HBM speed (profiles/r01_i).
+//   A CTA accumulates TP filter taps at once (one kernel row of a 3x3 filter): the dz tile is loaded once per TP taps
+//   instead of once per tap, which keeps the large early layers, whose dz + x exceed the L2, off HBM speed.
 // Replaces the wgrad half of TF autodiff for slim.conv2d (train.py:112).
 #include <cudaTypedefs.h>
 
@@ -19,6 +18,7 @@
 
 #include "common.cuh"
 #include "conv.cuh"
+#include "wgmma.cuh"
 
 namespace yb {
 
@@ -27,7 +27,7 @@ int make_tmap_2d(CUtensorMap* tm, const void* base, int dtype, long rows, long c
 int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int h, int w, int c, long ld, int ksize,
                         int stride, int pad, int bk, int pixels);
 
-static constexpr int WG_THREADS = 192;
+static constexpr int WG_THREADS = 384;  // warpgroup 0: TMA producer (one thread), warpgroups 1, 2: 64 output channels each
 static constexpr int WG_BKP = 64;     // pixels per pipeline stage
 static constexpr int WG_BM = 128;     // output channels per tile
 
@@ -50,44 +50,25 @@ struct WCfg {
   static constexpr int B_BYTES = BNW * WG_BKP * 2;             // one tap
   static constexpr int STAGE_BYTES = A_BYTES + TP * B_BYTES;
   static constexpr int STAGES = (192 * 1024 / STAGE_BYTES) > 8 ? 8 : (192 * 1024 / STAGE_BYTES);
-  static constexpr int ACC_COLS = TP * BNW;
-  static constexpr int TMEM_COLS = ACC_COLS <= 32 ? 32 : ACC_COLS <= 64 ? 64 : ACC_COLS <= 128 ? 128 : ACC_COLS <= 256 ? 256 : 512;
-  static_assert(ACC_COLS <= 512, "accumulators exceed TMEM");
+  static_assert(TP * BNW <= 192, "accumulators exceed the register budget");
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-  static constexpr uint32_t B_ROW = BCH * 2;                 // bytes per pixel row of a B box
-  static constexpr uint32_t B_SWZ = BCH == 64 ? 2u : 4u;     // 128B / 64B swizzle
+  static constexpr uint32_t B_ROW = BCH * 2;                 // bytes per pixel row of a B box (= its swizzle span)
 };
-
-// MN-major operand descriptor: rows (K index) are `row_bytes` apart, 8-row groups `8*row_bytes` (SBO),
-// successive 64/32-element MN blocks `lbo` bytes apart.
-__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                      uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
 
 template <typename T, int BNW, int TP>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const WgradParams p) {
   using C = WCfg<BNW, TP>;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
-  // and every staging-tile access then compiles to LD.E / ST.E + MEMBAR.ALL.CTA instead of LDS / STS (profiles/r02_b)
+  // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array (an integer round trip makes the pointer generic)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + C::STAGES * C::A_BYTES;              // [stage][tap in group][B_BYTES]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
   uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* done_bar = bars + 2 * C::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 1);
+  uint64_t* empty_bar = bars + C::STAGES;                    // one arrive per consumer warp
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   // tile coordinates: blockIdx.x = pixel split, blockIdx.y = n tile (tap group, ci chunk), blockIdx.z = co tile
   const int tap0 = (blockIdx.y / p.n_chunks) * TP;
   const int ci0 = (blockIdx.y % p.n_chunks) * BNW;
@@ -96,114 +77,102 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int kb1 = min(kb0 + p.kb_per_split, p.num_kb);
   const int nkb = kb1 - kb0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(done_bar, 1);
+    for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (nkb <= 0) return;
 
-  if (nkb > 0) {
-    if (warp == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {   // single-thread loop; the pixel coordinates of the 64-pixel block advance as counters
       int stage = 0; uint32_t phase = 0;
-      if (lane == 0) {   // single-lane loop; the pixel coordinates of the 64-pixel block advance as counters
-        const long pstart = (long)kb0 * WG_BKP;
-        int q = (int)(pstart % p.wo), pp = (int)((pstart / p.wo) % p.ho), img = (int)(pstart / ((long)p.wo * p.ho));
-        const bool two_a = co0 + 64 < p.cout;   // second 64-channel block exists (else its rows are masked anyway)
-        const uint32_t tx_bytes = TP * C::B_BYTES + (two_a ? C::A_BYTES : C::A_BYTES / 2);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          const long p0 = (long)kb * WG_BKP;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          uint8_t* a = sA + stage * C::A_BYTES;
-          if (p.a_dilated) {
-            tma_load_im2col_4d(a, &tmA, &full_bar[stage], co0, 2 * q, 2 * pp, img, 0, 0);
-            if (two_a) tma_load_im2col_4d(a + WG_BKP * 128, &tmA, &full_bar[stage], co0 + 64, 2 * q, 2 * pp, img, 0, 0);
-          } else {
-            tma_load_2d(a, &tmA, &full_bar[stage], co0, (int)p0);
-            if (two_a) tma_load_2d(a + WG_BKP * 128, &tmA, &full_bar[stage], co0 + 64, (int)p0);
-          }
-#pragma unroll
-          for (int t = 0; t < TP; ++t) {
-            uint8_t* b = sB + (stage * TP + t) * C::B_BYTES;
-            const int tap = tap0 + t;
-            const int th = TP == 9 ? t / 3 : (TP == 3 ? tap0 / 3 : tap / p.ksize);
-            const int tw = TP == 9 ? t % 3 : (TP == 3 ? t : tap % p.ksize);
-#pragma unroll
-            for (int j = 0; j < C::NB; ++j)
-              tma_load_im2col_4d(b + j * WG_BKP * C::B_ROW, &tmB, &full_bar[stage], ci0 + j * C::BCH,
-                                 q * p.stride - p.pad, pp * p.stride - p.pad, img, (uint16_t)tw, (uint16_t)th);
-          }
-          q += WG_BKP;
-          while (q >= p.wo) { q -= p.wo; if (++pp == p.ho) { pp = 0; ++img; } }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      const long pstart = (long)kb0 * WG_BKP;
+      int q = (int)(pstart % p.wo), pp = (int)((pstart / p.wo) % p.ho), img = (int)(pstart / ((long)p.wo * p.ho));
+      const bool two_a = co0 + 64 < p.cout;   // second 64-channel block exists (else its rows are masked anyway)
+      const uint32_t tx_bytes = TP * C::B_BYTES + (two_a ? C::A_BYTES : C::A_BYTES / 2);
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const long p0 = (long)kb * WG_BKP;
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
+        uint8_t* a = sA + stage * C::A_BYTES;
+        if (p.a_dilated) {
+          tma_load_im2col_4d(a, &tmA, &full_bar[stage], co0, 2 * q, 2 * pp, img, 0, 0);
+          if (two_a) tma_load_im2col_4d(a + WG_BKP * 128, &tmA, &full_bar[stage], co0 + 64, 2 * q, 2 * pp, img, 0, 0);
+        } else {
+          tma_load_2d(a, &tmA, &full_bar[stage], co0, (int)p0);
+          if (two_a) tma_load_2d(a + WG_BKP * 128, &tmA, &full_bar[stage], co0 + 64, (int)p0);
         }
-      }
-      __syncwarp();
-    } else if (warp == 1) {
-      // kind::f16, fp32 accumulate, A and B both MN-major (bits 15/16)
-      constexpr uint32_t idesc = make_idesc_f16(WG_BM, BNW, std::is_same<T, __nv_bfloat16>::value) | (1u << 15) | (1u << 16);
-      int stage = 0; uint32_t phase = 0;
-      if (lane == 0) {
-        const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = a_base + stage * C::A_BYTES;
 #pragma unroll
-          for (int t = 0; t < TP; ++t) {
-            const uint32_t b_addr = b_base + (stage * TP + t) * C::B_BYTES;
+        for (int t = 0; t < TP; ++t) {
+          uint8_t* b = sB + (stage * TP + t) * C::B_BYTES;
+          const int tap = tap0 + t;
+          const int th = TP == 9 ? t / 3 : (TP == 3 ? tap0 / 3 : tap / p.ksize);
+          const int tw = TP == 9 ? t % 3 : (TP == 3 ? t : tap % p.ksize);
 #pragma unroll
-            for (int k = 0; k < WG_BKP / 16; ++k) {
-              const uint64_t adesc = make_mnmajor_desc(a_addr + k * 16 * 128, WG_BKP * 128, 1024, 2u);
-              const uint64_t bdesc = make_mnmajor_desc(b_addr + k * 16 * C::B_ROW, WG_BKP * C::B_ROW, 8 * C::B_ROW, C::B_SWZ);
-              umma_f16(tmem_base + t * BNW, adesc, bdesc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == kb1 - 1) umma_commit(done_bar);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          for (int j = 0; j < C::NB; ++j)
+            tma_load_im2col_4d(b + j * WG_BKP * C::B_ROW, &tmB, &full_bar[stage], ci0 + j * C::BCH,
+                               q * p.stride - p.pad, pp * p.stride - p.pad, img, (uint16_t)tw, (uint16_t)th);
         }
-      }
-      __syncwarp();
-    } else {
-      // epilogue: rows = output channels, columns = input channels of this tap
-      const int quarter = warp & 3;
-      const int co = co0 + quarter * 32 + lane;
-      mbar_wait(done_bar, 0);
-      tcgen05_fence_after();
-      const long ktot = (long)p.ksize * p.ksize * p.cin;
-#pragma unroll 1
-      for (int t = 0; t < TP; ++t) {
-        float* dst = p.dw + (long)co * ktot + (long)(tap0 + t) * p.cin + ci0;
-#pragma unroll 1
-        for (int ch = 0; ch < BNW / 32; ++ch) {
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + t * BNW + ch * 32, r);
-          tmem_ld_wait();
-          if (co < p.cout) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                     __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-              atomicAdd(reinterpret_cast<float4*>(dst + ch * 32 + 4 * j), v);
-            }
-          }
-        }
+        q += WG_BKP;
+        while (q >= p.wo) { q -= p.wo; if (++pp == p.ho) { pp = 0; ++img; } }
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
+  } else {
+    // MMA: warpgroup cw owns output channels [co0 + 64 cw, co0 + 64 cw + 64) = A box cw.  Both operands are MN-major
+    // (rows of the shared-memory tiles are pixels = K): A = dz^T one 64-channel swizzle atom wide, B = x_col^T.
+    constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127, lane = t & 31;
+    float acc[TP][BNW / 2];
+    int stage = 0, prev = 0; uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(sA + stage * C::A_BYTES) + cw * WG_BKP * 128;
+#pragma unroll
+      for (int tt = 0; tt < TP; ++tt) wgmma_fence_operand(acc[tt]);
+      wgmma_fence();
+#pragma unroll
+      for (int tt = 0; tt < TP; ++tt) {
+        const uint32_t b_addr = smem_u32(sB + (stage * TP + tt) * C::B_BYTES);
+#pragma unroll
+        for (int k = 0; k < WG_BKP / 16; ++k) {
+          const uint64_t adesc = make_smem_desc(a_addr + k * 16 * 128, WG_BKP * 128, 1024, 128);
+          const uint64_t bdesc = make_smem_desc(b_addr + k * 16 * C::B_ROW, WG_BKP * C::B_ROW, 8 * C::B_ROW, C::B_ROW);
+          Wgmma<BNW, kBF16, 1, 1>::mma(acc[tt], adesc, bdesc, (kb > kb0 || k > 0) ? 1 : 0);
+        }
+      }
+      wgmma_commit();
+#pragma unroll
+      for (int tt = 0; tt < TP; ++tt) wgmma_fence_operand(acc[tt]);
+      wgmma_wait<1>();                           // the previous k-block's MMAs have retired: its stage is free
+      if (kb > kb0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int tt = 0; tt < TP; ++tt) wgmma_fence_operand(acc[tt]);
+    // epilogue: accumulator (row, col) = (output channel, input channel of the tap), column pairs -> float2 atomics
+    const long ktot = (long)p.ksize * p.ksize * p.cin;
+    const int rbase = co0 + 64 * cw + 16 * (t >> 5) + (lane >> 2);
+#pragma unroll
+    for (int tt = 0; tt < TP; ++tt) {
+#pragma unroll
+      for (int i = 0; i < BNW / 2; i += 2) {
+        const int co = rbase + 8 * ((i >> 1) & 1);
+        const int ci = 8 * (i >> 2) + 2 * (lane & 3);
+        if (co < p.cout)
+          atomicAdd(reinterpret_cast<float2*>(p.dw + (long)co * ktot + (long)(tap0 + tt) * p.cin + ci0 + ci),
+                    make_float2(acc[tt][i], acc[tt][i + 1]));
+      }
+    }
   }
 }
 
@@ -257,9 +226,8 @@ stem_wgrad_kernel(const float* __restrict__ x, const void* __restrict__ dz, int 
 }
 
 // Pixel splits (split-K) of one wgrad launch.  One CTA is resident per SM (192 KB of stages), so the grid runs in waves
-// of `sms` CTAs, and every CTA ends with TP x BNW x 128 fp32 atomics that nothing overlaps: measured at ~40 pixel blocks'
-// worth of main loop (profiles/r02_g: the 26x26 256->512 layer ran 13 splits x 24 tiles = 312 CTAs = 2.1 waves of 26
-// blocks, 84 us against 36 us of tensor work).  Returns the split count that minimises waves x (blocks per CTA + epi).
+// of `sms` CTAs, and every CTA ends with TP x BNW x 128 fp32 atomics that nothing overlaps, costed as `epi_blocks` pixel
+// blocks' worth of main loop.  Returns the split count that minimises waves x (blocks per CTA + epi).
 long wgrad_pick_splits(long num_kb, long tiles, long sms, long epi_blocks) {
   long splits = 1;
   double best = 1e30;
@@ -302,13 +270,14 @@ extern "C" int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void*
   p.P = (long)d->n * ho * wo; p.ho = ho; p.wo = wo;
   p.cin = d->cin; p.cout = d->cout; p.ksize = d->ksize; p.stride = d->stride; p.pad = d->ksize / 2;
   p.num_kb = ceil_div(p.P, WG_BKP);
-  const int bnw = d->cin % 128 == 0 ? 128 : (d->cin % 64 == 0 ? 64 : 32);
+  const int taps = d->ksize * d->ksize;
+  // 3x3 convs accumulate one kernel row (3 taps) per CTA, at most 64 input channels per tap: 3 x 64 accumulator columns
+  // are 96 registers per thread.  1x1 convs have one tap and take up to 128 channels.
+  const int bnw = taps == 1 && d->cin % 128 == 0 ? 128 : (d->cin % 64 == 0 ? 64 : 32);
   p.n_chunks = d->cin / bnw;
   p.dw = dw;
-  const int taps = d->ksize * d->ksize;
-  // taps accumulated per CTA: all 9 for cin = 32 (288 TMEM columns), one kernel row otherwise; 1x1 convs have one tap
-  const char* tpf = opt("YB_WGRAD_TP");     // "1": one tap per CTA (the first version; A/B testing)
-  const int tp = (taps == 1 || (tpf && tpf[0] == '1')) ? 1 : (bnw == 32 ? 9 : 3);
+  const char* tpf = opt("YB_WGRAD_TP");     // "1": one tap per CTA (A/B testing)
+  const int tp = (taps == 1 || (tpf && tpf[0] == '1')) ? 1 : 3;
   const int tap_groups = taps / tp;
   const int co_tiles = ceil_div(d->cout, WG_BM);
   const long tiles = (long)tap_groups * p.n_chunks * co_tiles;
@@ -331,11 +300,10 @@ extern "C" int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void*
   dim3 grid((unsigned)splits, (unsigned)(tap_groups * p.n_chunks), (unsigned)co_tiles);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define YB_WG(T)                                                                       \
-  if (bnw == 128) return tp == 3 ? launch_wgrad<T, 128, 3>(tmA, tmB, p, grid, st)     \
-                                 : launch_wgrad<T, 128, 1>(tmA, tmB, p, grid, st);   \
+  if (bnw == 128) return launch_wgrad<T, 128, 1>(tmA, tmB, p, grid, st);              \
   if (bnw == 64) return tp == 3 ? launch_wgrad<T, 64, 3>(tmA, tmB, p, grid, st)       \
                                 : launch_wgrad<T, 64, 1>(tmA, tmB, p, grid, st);     \
-  return tp == 9 ? launch_wgrad<T, 32, 9>(tmA, tmB, p, grid, st) : launch_wgrad<T, 32, 1>(tmA, tmB, p, grid, st);
+  return tp == 3 ? launch_wgrad<T, 32, 3>(tmA, tmB, p, grid, st) : launch_wgrad<T, 32, 1>(tmA, tmB, p, grid, st);
   if (d->dtype == YB_F16) { YB_WG(__half) }
   YB_WG(__nv_bfloat16)
 #undef YB_WG

@@ -133,7 +133,8 @@ extern "C" int yb_pack_conv_weights(const float* src, int layout, int cout, int 
   YB_REQUIRE(layout >= 0 && layout <= 2, "pack: bad layout %d", layout);
   YB_REQUIRE(cout_pad >= cout && cout > 0 && cin > 0 && ksize > 0, "pack: bad shape");
   const long total = (long)cout_pad * ksize * ksize * cin;
-  const int grid = (int)((total + 255) / 256 < 148L * 16 ? (total + 255) / 256 : 148L * 16);
+  const long cap = (long)num_sms() * 16;
+  const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == YB_F16)
     pack_weights_kernel<__half><<<grid, 256, 0, st>>>(src, layout, cout, cin, ksize, cout_pad, static_cast<__half*>(dst));

@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(256) loss_kernel(const LossParams p) {
     if (m == 0.f) {
       // no object in this (cell, anchor) — all but a few hundred of the 10^5 boxes: the class loss and its gradient are
       // object_mask * (...) = 0, so neither the 2 x C logits / targets are read nor C sigmoids evaluated (the kernel was
-      // latency-bound on exactly that loop: 379 us for the 52x52 scale at batch 32, profiles/r02_d_kernels_train.md)
+      // latency-bound on exactly that loop)
       if (p.dfm != nullptr)
         for (int k = lane; k < p.C; k += 32) store_grad<T>(p, box, a, cellrow, 5 + k, 0.f);
       continue;

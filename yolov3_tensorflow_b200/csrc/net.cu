@@ -341,8 +341,7 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
   }
   for (size_t i = first > 1 ? first : 1; i < net->layers.size() && (int)i <= last; ++i) {
     Layer& L = net->layers[i];
-    // (after the r01_j pipeline-loop fixes the tcgen05 kernel runs these two layers in ~455 us against ~500-550 us for
-    //  the mma.sync halo kernel, so the latter is now opt-in: YB_THIN=2)
+    // the mma.sync halo kernel for the Cin = 32 layers is opt-in (YB_THIN=2); by default they take the tensor-core path
     const bool thin_cin32 = opt("YB_THIN")[0] == '2';
     if (thin_cin32 && L.info.ksize == 3 && L.info.cin == 32 && L.info.has_bn && !L.upsample) {
       // Cin = 32: 64-byte im2col rows halve the TMA line rate -> direct halo-tile kernel (csrc/conv_thin.cu)
@@ -372,9 +371,8 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
       if (rc) return rc;
       continue;
     }
-    // halo-tile kernel: measured (profiles/r02_c, batch 64 @416) 302 vs 381 us on Conv_3 (32->64 @208^2) and 244 vs 382 us
-    // on Conv_1 (32->64 /2), but 227 vs 188 us on the 64->128 layers (their weights leave room for two halo stages only):
-    // default on for Cin = 32.  YB_HALO=0: never, YB_HALO=1: wherever supported.
+    // halo-tile kernel: default on for Cin = 32, whose 64-byte im2col rows make the implicit GEMM TMA-row bound; the
+    // 64->128 layers leave room for only two halo stages beside their weights.  YB_HALO=0: never, YB_HALO=1: wherever supported.
     const char* hopt = opt("YB_HALO");
     if (L.halo_ok && hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)) {
       int rc = conv_halo_launch(&L.halo_desc, L.halo_maps, L.halo_params, st);

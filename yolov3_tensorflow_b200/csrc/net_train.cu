@@ -1,8 +1,8 @@
-// Training plan: one step of train.py:105-115 on the B200 engine.
+// Training plan: one step of train.py:105-115 on the H100 engine.
 //   forward  : conv (raw z + BN batch sums in the epilogue) -> bn_finalize -> bn_act_apply
 //              (model.py:30-80 with is_training=True; UPDATE_OPS moving stats, train.py:108-109)
 //   loss     : yb_loss_layer x3, gradients written 16-bit into the backward GEMM operands
-//   backward : per layer, last to first: bn_bwd_reduce/apply -> wgrad (tcgen05) -> dgrad (forward
+//   backward : per layer, last to first: bn_bwd_reduce/apply -> wgrad (wgmma) -> dgrad (forward
 //              kernel on dz with flipped/transposed weights; the residual / second-consumer
 //              contributions are folded into the dgrad epilogue's residual add)
 //   update   : L2 + per-tensor clip_by_norm + momentum over one flat gradient buffer (which the

@@ -157,7 +157,7 @@ __global__ void pack_dgrad_s2_kernel(const float* __restrict__ w, int cout, int 
 
 // All layers in one launch (PackJob, optim.cuh).  The per-layer kernels above walk the DESTINATION linearly, so
 // consecutive threads read the masters with a stride of ks*ks*cin floats (one 32-byte sector per element) and every
-// layer pays its own launch: 74 launches, 0.79 ms per training step for 370 MB of traffic (profiles/r02_d_kernels_train.md).
+// layer pays its own launch (74 launches per training step for 370 MB of traffic).
 template <typename T>
 __global__ void __launch_bounds__(256) pack_dgrad_multi_kernel(const PackJob* __restrict__ jobs, int num_jobs) {
   __shared__ float tile[32][33];

@@ -1,10 +1,10 @@
 """`yolov3` — the reference's model class (model.py:12-365 of wizyoung/YOLOv3_TensorFlow)
-re-hosted on the B200 engine.
+re-hosted on the H100 engine.
 
 Same constructor and method names/arguments as the reference.  The reference methods
 build TF1 graph nodes; these run eagerly: they take/return CUDA `torch.Tensor`s (used
 purely as device-buffer containers, NHWC, float32 at the API surface) and enqueue
-hand-written sm_100a kernels from libyolob200.so on the current CUDA stream.
+hand-written sm_90a kernels from libyolob200.so on the current CUDA stream.
 There is no torch op on the compute path and no CPU fallback.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""utils/nms_utils.py of the reference, re-hosted: `gpu_nms` runs the sm_100a NMS kernels
+"""utils/nms_utils.py of the reference, re-hosted: `gpu_nms` runs the sm_90a NMS kernels
 (libyolob200.so: yb_nms); `py_nms` / `cpu_nms` keep the reference's numpy semantics
 (a *different* algorithm: +1 pixel areas, `<=` keep rule — utils/nms_utils.py:51-123)."""
 from __future__ import annotations
