@@ -214,6 +214,10 @@ __device__ __forceinline__ void wgmma_fence_operand(float (&d)[K]) {
 }
 // named barrier over the 128 threads of one warpgroup (ids 1.. : 0 is __syncthreads)
 __device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// named barrier over `n` threads: wait (sync) / signal without waiting (arrive)
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
 
 // wgmma shared-memory matrix descriptor (PTX ISA "matrix descriptor format"): [0,14) addr>>4, [16,30) LBO>>4,
 // [32,46) SBO>>4, [62,64) layout (1 = 128B, 2 = 64B swizzle).  The swizzle is a function of the shared-memory address

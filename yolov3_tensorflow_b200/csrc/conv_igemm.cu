@@ -9,13 +9,19 @@
 //        come back zero-filled, so no padded copy of the input ever exists (K4 in SURVEY §2.3).
 //        1x1 convs: plain 2D tiled TMA over the [M, in_ld] matrix.
 //   B  : weights packed OHWI = [cout_pad, k*k*cin] K-major, 2D tiled TMA.
-//   D  : fp32 accumulators in registers: two consumer warpgroups own 64 rows x BN columns each and
-//        issue wgmma.mma_async m64nBNk16 with both operands read from 128B / 64B-swizzled shared memory.
+//   D  : fp32 accumulators in registers, wgmma.mma_async m64nBNk16 with both operands read from 128B / 64B-swizzled
+//        shared memory.
 //
 // Warp roles (384 threads, persistent over tiles): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 =
-// MMA + epilogue.  The producer runs ahead through the operand ring, so the next tile's loads overlap this tile's
-// epilogue.  The epilogue stages 32-column chunks of the accumulators through shared memory so that each thread
-// then owns 16 consecutive channels of one pixel (two 16-byte stores per output row).
+// MMA + epilogue.  The producer runs ahead through the operand ring in work-unit order.  Two schedules:
+//   ping-pong (the default): each consumer warpgroup owns whole 128 x BN tiles (two m64 wgmmas per k16 step) and the
+//     two take alternate work units.  A pair of named barriers hands the tensor cores from one warpgroup's main loop
+//     to the other's, so one warpgroup's epilogue runs while the other's MMAs run.
+//   cooperative (fused-decode detection heads, 1x1 convs with 128-column tiles, clusters, 1-warpgroup CTAs, register
+//     epilogue; conv_prepare_core chooses): the NC consumer warpgroups split
+//     every tile by rows (64 each), run the k-loop in lockstep and then the epilogue together.
+// The epilogue stages 32-column chunks of one 64-row accumulator block through shared memory so that each thread then
+// owns 16 consecutive channels of one pixel (two 16-byte stores per output row).
 //
 // Replaces: slim.conv2d/batch_norm/leaky_relu (utils/layer_utils.py:20, model.py:43-49),
 // tf.add (utils/layer_utils.py:30), tf.pad (:15-16), resize_nearest_neighbor (:86),
@@ -37,7 +43,8 @@ static constexpr int RING_BYTES = 196 * 1024;     // operand ring (the rest of t
 static constexpr int EPI_LD = 33;                 // staging row pitch in floats: row walks and column walks are conflict-free
 static constexpr int EPI_FLOATS = WG_ROWS * EPI_LD;
 
-// NC consumer warpgroups per CTA (tile = 64 NC rows x BN); warpgroup 0 is the TMA producer.
+// NC consumer warpgroups per CTA (tile = 64 NC rows x BN); warpgroup 0 is the TMA producer.  Both schedules use the
+// same 128-row tile for NC = 2, so they share the ring and the tensor maps.
 template <int BN, int BK, int NC>
 struct Cfg {
   static constexpr int BLOCK_M = WG_ROWS * NC;
@@ -46,7 +53,9 @@ struct Cfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (RING_BYTES / STAGE_BYTES) > 8 ? 8 : (RING_BYTES / STAGE_BYTES);
-  // ring | NC x staging tile | NC x [2][BN] statistics | NC x [2][BN] scale / shift | barriers
+  // ring | NC x staging tile | NC x [2][BN] statistics | NC x [2][BN] scale / shift | barriers.  A ping-pong warpgroup
+  // stages its 128-row tile one 64-row half after the other through its own 64-row staging tile, so the budget is the
+  // same for both schedules (BN = 128, BK = 64: 6 x 32 KB ring + 2 x 8.4 KB staging + 4 KB = 214 KB).
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + NC * EPI_FLOATS * 4 + NC * 4 * BN * 4 + 256;
   static constexpr uint32_t SWIZZLE = BK * 2;     // a k-block row is exactly one swizzle span (128B / 64B)
   static constexpr uint32_t SBO = 8 * BK * 2;     // bytes between 8-row groups
@@ -96,24 +105,26 @@ __device__ __forceinline__ void epi_store16(const ConvParams& p, const float* sr
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.1f * v[j]);   // == v > 0 ? v : 0.1 v
   }
-  long orow[4] = {row, 0, 0, 0};
+  // output row of copy rep (2x upsample: 4 copies): orow0 + (rep >> 1) * W2 + (rep & 1), computed per copy so that no
+  // row array is live beside a ping-pong warpgroup's 128 accumulators
+  long orow0 = row, W2 = 0;
   int nrep = 1;
   if (p.upsample || p.scatter) {
     const int q = row % p.Q;
     const int pp = (row / p.Q) % p.P;
     const int img = row / (p.Q * p.P);
-    const long W2 = 2L * p.Q;
-    const long base = ((long)img * 2 * p.P + 2 * pp) * W2 + 2 * q;
+    const long w2 = 2L * p.Q;
+    const long base = ((long)img * 2 * p.P + 2 * pp) * w2 + 2 * q;
     if (p.scatter) {
-      orow[0] = base + ((p.scatter - 1) >> 1) * W2 + ((p.scatter - 1) & 1);
+      orow0 = base + ((p.scatter - 1) >> 1) * w2 + ((p.scatter - 1) & 1);
     } else {
-      orow[0] = base; orow[1] = base + 1; orow[2] = base + W2; orow[3] = base + W2 + 1;
+      orow0 = base; W2 = w2;
       nrep = 4;
     }
   }
   if (p.out_fp32) {                              // detection heads: cout = 3 (5 + C) need not be a multiple of 16
     for (int rep = 0; rep < nrep; ++rep) {
-      float* o = static_cast<float*>(p.out) + orow[rep] * p.out_ld + col0;
+      float* o = static_cast<float*>(p.out) + (orow0 + (rep >> 1) * W2 + (rep & 1)) * p.out_ld + col0;
 #pragma unroll
       for (int j = 0; j < 16; ++j)
         if (col0 + j < p.cout) o[j] = v[j];
@@ -121,7 +132,7 @@ __device__ __forceinline__ void epi_store16(const ConvParams& p, const float* sr
     return;
   }
   if (p.res != nullptr) {
-    const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + orow[0] * p.res_ld + col0);
+    const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + orow0 * p.res_ld + col0);
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const uint4 u = __ldg(rp + j);
@@ -141,7 +152,7 @@ __device__ __forceinline__ void epi_store16(const ConvParams& p, const float* sr
     pk[j].w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
   }
   for (int rep = 0; rep < nrep; ++rep) {
-    uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + orow[rep] * p.out_ld + col0);
+    uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + (orow0 + (rep >> 1) * W2 + (rep & 1)) * p.out_ld + col0);
     op[0] = pk[0];
     op[1] = pk[1];
   }
@@ -285,10 +296,18 @@ __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float
   }
 }
 
-template <typename T, int BN, int BK, int NC, int DET_E = 0>   // DET_E = 5 + classes: detection head with the decode fused in
+// named barriers (0 = __syncthreads; 1, 2 = the consumer warpgroups' own barriers): MMA_TURN + w = "warpgroup w may
+// start its next main loop" (ping-pong)
+static constexpr int MMA_TURN_BAR = 3;
+
+// DET_E = 5 + classes: detection head with the decode fused in.  PP: ping-pong schedule (NC = 2, no cluster, staged
+// epilogue, no fused decode; see the top of the file).
+template <typename T, int BN, int BK, int NC, int DET_E = 0, bool PP = false>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
+  static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
+  constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
   using C = Cfg<BN, BK, NC>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
@@ -301,26 +320,28 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   float* s_ss = s_stat + NC * 2 * BN;                    // [NC][2][BN] scale / shift of each warpgroup's current n-tile
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_ss + NC * 2 * BN);   // [STAGES] TMA -> MMA
   uint64_t* empty_bar = full_bar + 8;                    // [STAGES] MMA -> TMA: one arrive per consumer warp of the cluster
+                                                         // (ping-pong: of the one warpgroup that read the stage)
 
-  const int wg = threadIdx.x >> 7;
-  const int cs = p.cluster;                              // CTAs per cluster (1: no cluster, no multicast)
-  const uint32_t rank = cs > 1 ? cluster_ctarank() : 0u;
-  const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
-  const int nunits = num_units(p);
-  const int kb_per_tap = p.cin / BK;
-  const int num_kb = p.kh * p.kw * kb_per_tap;
-
+  // warp-uniform by construction: ptxas then keeps the ping-pong consumer's 128 accumulators out of local memory
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 4 * NC * cs);
+      mbar_init(&empty_bar[i], PP ? 4 : 4 * NC * p.cluster);
     }
     fence_barrier_init();
   }
   __syncthreads();
-  if (cs > 1) cluster_sync_all();                        // every peer's barriers exist before the first multicast
+  if (p.cluster > 1) cluster_sync_all();                 // every peer's barriers exist before the first multicast
+
+  const int cs = PP ? 1 : p.cluster;                     // CTAs per cluster (1: no cluster, no multicast)
+  const uint32_t rank = cs > 1 ? cluster_ctarank() : 0u;
+  const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
+  const int nunits = num_units(p);
+  const int kb_per_tap = p.cin / BK;
+  const int num_kb = p.kh * p.kw * kb_per_tap;
 
   if (wg == 0) {
     // ===================== TMA producer =====================
@@ -366,7 +387,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
   } else {
-    // ===================== MMA + epilogue (warpgroup cw: rows [64 cw, 64 cw + 64) of every tile) =====================
+    // ===================== MMA + epilogue =====================
+    // cooperative: warpgroup cw computes rows [64 cw, 64 cw + 64) of every tile of the CTA;
+    // ping-pong: warpgroup cw computes all 128 rows of every other tile of the CTA (its j-th unit is the CTA's 2j + cw-th)
     constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
     const int cw = wg - 1;
     const int t = threadIdx.x & 127;
@@ -385,36 +408,55 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         else for (int r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
       }
     };
-    float acc[BN / 2];
+    float acc[NH][BN / 2];
     int stage = 0, prev = 0;
     uint32_t phase = 0;
+    // ping-pong: step the ring position over the other warpgroup's unit (the producer fills the ring in unit order)
+    auto skip_unit = [&]() {
+      const int s = stage + num_kb;
+      phase ^= (uint32_t)((s / C::STAGES) & 1);
+      stage = s % C::STAGES;
+    };
+    if (PP && cw == 1) skip_unit();
     int cur_n0 = -1, ss_n0 = -1;
-    const uint32_t a_off = cw * WG_ROWS * BK * 2;
-    for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
+    const uint32_t a_off = PP ? 0u : cw * WG_ROWS * BK * 2;
+    const int unit_step = PP ? 2 * num_clusters : num_clusters;
+    for (int unit = cluster_id + (PP ? cw * num_clusters : 0); unit < nunits; unit += unit_step) {
       int m_idx, n_idx;
       unit_coords(p, unit, rank, m_idx, n_idx);
       const int m0 = m_idx * C::BLOCK_M;
       const int n0 = n_idx * BN;
+      // Ping-pong: wait until the other warpgroup has issued the previous unit's main loop.  Besides keeping the two
+      // main loops from interleaving on the tensor cores, this makes every fill of the ring before this unit's
+      // complete, so a parity wait below cannot match a fill two phases old.
+      if (PP && unit != cluster_id) named_bar_sync(MMA_TURN_BAR + cw, 256);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a_addr = smem_u32(sA + stage * C::A_BYTES) + a_off;
         const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
-        wgmma_fence_operand(acc);
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_fence_operand(acc[h]);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)
-          Wgmma<BN, kBF16, 0, 0>::mma(acc, make_kmajor_desc(a_addr + k * 32, C::SBO, C::SWIZZLE),
-                                      make_kmajor_desc(b_addr + k * 32, C::SBO, C::SWIZZLE), (kb | k) != 0);
+#pragma unroll
+          for (int h = 0; h < NH; ++h)
+            Wgmma<BN, kBF16, 0, 0>::mma(acc[h], make_kmajor_desc(a_addr + h * WG_ROWS * BK * 2 + k * 32, C::SBO, C::SWIZZLE),
+                                        make_kmajor_desc(b_addr + k * 32, C::SBO, C::SWIZZLE), (kb | k) != 0);
         wgmma_commit();
-        wgmma_fence_operand(acc);
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_fence_operand(acc[h]);
         wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its stage is free
         if (kb > 0) release(prev);
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
+      if (PP && unit + num_clusters < nunits) named_bar_arrive(MMA_TURN_BAR + (cw ^ 1), 256);   // the other's turn
       wgmma_wait<0>();
-      wgmma_fence_operand(acc);
+#pragma unroll
+      for (int h = 0; h < NH; ++h) wgmma_fence_operand(acc[h]);
       release(prev);
+      if (PP) skip_unit();
 
       if (p.stat_sum != nullptr && n0 != cur_n0) {
         if (cur_n0 >= 0) stat_flush<BN>(p, sst, cur_n0, t, bar_id);
@@ -429,36 +471,41 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         warpgroup_bar(bar_id);
         ss_n0 = n0;
       }
-      const int row0 = m0 + cw * WG_ROWS;
       if constexpr (DET_E > 0) {
-        epilogue_detect<BN, DET_E>(p, acc, row0, t, stg, sss, bar_id);
-      } else if (p.epi_reg) {
-        epilogue_reg<T, BN>(p, acc, row0, n0, sss, t);
+        epilogue_detect<BN, DET_E>(p, acc[0], m0 + cw * WG_ROWS, t, stg, sss, bar_id);
+      } else if (!PP && p.epi_reg) {
+        epilogue_reg<T, BN>(p, acc[0], m0 + cw * WG_ROWS, n0, sss, t);
       } else {
+        // the accumulator blocks as one row of NH * BN / 32 chunks: one copy of the epilogue serves both halves
+        const float(&acc_all)[NH * BN / 2] = reinterpret_cast<const float(&)[NH * BN / 2]>(acc);
         const int nvalid = min(BN / 32, (p.cout - n0 + 31) >> 5);   // zero-padded weight rows (cout_pad > cout): not stored
         const int er = t >> 1, eh = t & 1;       // this thread's row of the chunk and its 16-column half
 #pragma unroll 1
-        for (int ch = 0; ch < nvalid; ++ch) {
-          warpgroup_bar(bar_id);                 // the previous chunk's readers are done with the staging tile
-          wgmma_stage_chunk<BN>(acc, ch, stg, EPI_LD, t);
-          warpgroup_bar(bar_id);
-          if (p.stat_sum != nullptr) {           // BN batch statistics of the raw conv output: lane = column
-            const int col = t & 31, rg = (t >> 5) * 16;
-            float cs_ = 0.f, cs2 = 0.f;
+        for (int h = 0; h < NH; ++h) {
+          const int row0 = m0 + (PP ? h : cw) * WG_ROWS;
+#pragma unroll 1
+          for (int ch = 0; ch < nvalid; ++ch) {
+            warpgroup_bar(bar_id);               // the previous chunk's readers are done with the staging tile
+            wgmma_stage_chunk<NH * BN>(acc_all, h * (BN / 32) + ch, stg, EPI_LD, t);
+            warpgroup_bar(bar_id);
+            if (p.stat_sum != nullptr) {         // BN batch statistics of the raw conv output: lane = column
+              const int col = t & 31, rg = (t >> 5) * 16;
+              float cs_ = 0.f, cs2 = 0.f;
 #pragma unroll 4
-            for (int rr = 0; rr < 16; ++rr) {
-              if (row0 + rg + rr < p.M) {
-                const float v = stg[(rg + rr) * EPI_LD + col];
-                cs_ += v;
-                cs2 = fmaf(v, v, cs2);
+              for (int rr = 0; rr < 16; ++rr) {
+                if (row0 + rg + rr < p.M) {
+                  const float v = stg[(rg + rr) * EPI_LD + col];
+                  cs_ += v;
+                  cs2 = fmaf(v, v, cs2);
+                }
               }
+              atomicAdd(&sst[ch * 32 + col], cs_);
+              atomicAdd(&sst[BN + ch * 32 + col], cs2);
             }
-            atomicAdd(&sst[ch * 32 + col], cs_);
-            atomicAdd(&sst[BN + ch * 32 + col], cs2);
-          }
-          if (row0 + er < p.M) {
-            const int cl = ch * 32 + eh * 16;
-            epi_store16<T>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl);
+            if (row0 + er < p.M) {
+              const int cl = ch * 32 + eh * 16;
+              epi_store16<T>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl);
+            }
           }
         }
       }
@@ -593,11 +640,11 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
   return YB_OK;
 }
 
-template <typename T, int BN, int BK, int NC, int DET_E = 0>
+template <typename T, int BN, int BK, int NC, int DET_E = 0, bool PP = false>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
   using C = Cfg<BN, BK, NC>;
   static DeviceOnce once;
-  auto kern = conv_igemm_kernel<T, BN, BK, NC, DET_E>;
+  auto kern = conv_igemm_kernel<T, BN, BK, NC, DET_E, PP>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int cs = p.cluster;
   const int units = ceil_div(p.num_m_tiles, cs) * p.num_n_tiles;
@@ -638,14 +685,17 @@ int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorM
   }
   const int bn = conv_block_n(cout_pad);
   const int nc = p.consumers;
+#define YB_DISPATCH_BN_BK(T, BN, BK)                                                          \
+  if (bn == BN && bk == BK) {                                                                 \
+    if (p.pingpong) return launch_cfg<T, BN, BK, 2, 0, true>(tmA, tmB, p, st);               \
+    return nc == 2 ? launch_cfg<T, BN, BK, 2>(tmA, tmB, p, st) : launch_cfg<T, BN, BK, 1>(tmA, tmB, p, st); \
+  }
 #define YB_DISPATCH(T)                                                       \
-  if (bn == 128 && bk == 64) return nc == 2 ? launch_cfg<T, 128, 64, 2>(tmA, tmB, p, st) : launch_cfg<T, 128, 64, 1>(tmA, tmB, p, st); \
-  if (bn == 128 && bk == 32) return nc == 2 ? launch_cfg<T, 128, 32, 2>(tmA, tmB, p, st) : launch_cfg<T, 128, 32, 1>(tmA, tmB, p, st); \
-  if (bn == 64 && bk == 64) return nc == 2 ? launch_cfg<T, 64, 64, 2>(tmA, tmB, p, st) : launch_cfg<T, 64, 64, 1>(tmA, tmB, p, st);     \
-  if (bn == 64 && bk == 32) return nc == 2 ? launch_cfg<T, 64, 32, 2>(tmA, tmB, p, st) : launch_cfg<T, 64, 32, 1>(tmA, tmB, p, st);
+  YB_DISPATCH_BN_BK(T, 128, 64) YB_DISPATCH_BN_BK(T, 128, 32) YB_DISPATCH_BN_BK(T, 64, 64) YB_DISPATCH_BN_BK(T, 64, 32)
   if (dtype == YB_F16) { YB_DISPATCH(__half) }
   else if (dtype == YB_BF16) { YB_DISPATCH(__nv_bfloat16) }
 #undef YB_DISPATCH
+#undef YB_DISPATCH_BN_BK
   set_error("conv_launch: unsupported dtype %d", dtype);
   return YB_ERR_UNSUPPORTED;
 }
@@ -691,6 +741,13 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
   p->epi_reg = (!det && !stat_sum && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  // ping-pong wherever the default variant runs, except
+  //  - the fused-decode heads: their 256-column tile does not fit 128 rows per warpgroup in registers;
+  //  - 1x1 convs with 128-column tiles: their main loop (cin / 64 k-blocks) is too short to hide one warpgroup's
+  //    128 x 128 epilogue, and on H100 they measured 2-7 % slower ping-pong than with two warpgroups sharing the
+  //    epilogue (DESIGN.md §5).  The 1x1 convs with 64-column tiles and every windowed conv gain from it.
+  const bool pp_shape = kh * kw > 1 || bn != 128;
+  p->pingpong = (!det && p->consumers == 2 && p->cluster == 1 && !p->epi_reg && pp_shape) ? 1 : 0;
   const int block_m = 64 * p->consumers;
   memset(&p->det, 0, sizeof(p->det));
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
