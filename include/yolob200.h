@@ -89,6 +89,23 @@ int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, co
                   const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,
                   void* stream);
 int yb_conv_cout_pad(int cout);
+/* Host-only: the implicit-GEMM kernel and persistent grid yb_conv2d_fwd would launch for `d` with the current options
+ * (yb_set_option: YB_CONV_EG, YB_CONV_MODE, YB_CONV_EPI, YB_CONV_PP, YB_CONV_CTAS) on a device with sm_count SMs.
+ * kh = kw = 0: the forward ksize x ksize window; kh, kw in {1, 2}: one parity class of yb_conv2d_dgrad_s2 (d = its
+ * stride-1 descriptor over dz).  with_stats: BN statistics requested.  Work units = ceil(num_m_tiles / cluster) x
+ * num_n_tiles; the CTAs of the grid take them round-robin, and under ping-pong the two consumer warpgroups of a CTA
+ * take every other one of the CTA's units. */
+typedef struct yb_conv_schedule_info {
+  int pingpong;      /* 1: ping-pong (each consumer warpgroup owns whole tiles), 0: cooperative */
+  int consumers;     /* consumer warpgroups per CTA                                             */
+  int cluster;       /* CTAs per cluster                                                        */
+  int block_m, block_n, block_k;
+  int stages;        /* operand-ring depth                                                      */
+  int num_kb;        /* k-blocks per tile                                                       */
+  int num_m_tiles, num_n_tiles;
+  int grid;          /* CTAs launched                                                           */
+} yb_conv_schedule_info;
+int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count, yb_conv_schedule_info* info);
 
 /* First layer (darknet53_body/Conv, 3->32, 3x3 s1; utils/layer_utils.py:35): float32 NHWC image in,
  * `dtype` NHWC out.  w is OHWI float32 [32,3,3,3]. */

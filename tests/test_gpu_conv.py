@@ -12,21 +12,28 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(params=["1cta", "2cta", "mc", "1cta-reg", "2cta-reg", "1cta-eg1", "2cta-eg1", "1cta-eg2", "2cta-eg2"], autouse=True)
+@pytest.fixture(params=["1cta", "2cta", "mc", "1cta-reg", "2cta-reg", "1cta-eg1", "2cta-eg1", "1cta-eg2", "2cta-eg2",
+                        "1cta-pp"], autouse=True)
 def conv_mode(request):
-    """Every conv test runs against the kernel variants: one CTA per tile ("1cta", the default), clusters of 2 CTAs
-    sharing a TMA-multicast weight tile ("2cta") and clusters of 4 ("mc"); for the first two also against the
-    register-store epilogue ("-reg", instead of the shared-memory staging tile) and with one ("-eg1", 64-row tiles) or
-    two ("-eg2", 128-row tiles, the default) consumer warpgroups doing MMA + epilogue.  The library's option table
-    (yb_set_option) selects the variant; it is restored after each test."""
+    """Every conv test runs against the kernel variants: one CTA per tile ("1cta", the default: ping-pong for the
+    windowed convs and the 64-column 1x1 convs, cooperative for the 128-column 1x1 convs), clusters of 2 CTAs sharing a
+    TMA-multicast weight tile ("2cta") and clusters of 4 ("mc"); for the first two also against the register-store
+    epilogue ("-reg", instead of the shared-memory staging tile) and with one consumer warpgroup ("-eg1", 64-row tiles).
+    "-eg2" pins two consumer warpgroups (128-row tiles) sharing every tile: "1cta-eg2" is the cooperative schedule
+    wherever the default would ping-pong (YB_CONV_PP=0), "2cta-eg2" the 2-CTA clusters with the grid capped at one
+    cluster (YB_CONV_CTAS=2), so that it runs many units.  "1cta-pp" is ping-pong wherever the kernel allows it
+    (YB_CONV_PP=1), the 128-column 1x1 convs included.  The library's option table (yb_set_option) selects the variant;
+    it is restored after each test."""
     L = _lib()
     mode, _, epi = request.param.partition("-")
     L.set_option("YB_CONV_MODE", "2cta" if mode == "mc" else mode)
     L.set_option("YB_CONV_MC", "1" if mode == "mc" else "0")
     L.set_option("YB_CONV_EPI", "reg" if epi == "reg" else None)
     L.set_option("YB_CONV_EG", epi[2:] if epi.startswith("eg") else None)
+    L.set_option("YB_CONV_PP", {"1cta-eg2": "0", "1cta-pp": "1"}.get(request.param))
+    L.set_option("YB_CONV_CTAS", "2" if request.param == "2cta-eg2" else None)
     yield request.param
-    for k in ("YB_CONV_MODE", "YB_CONV_MC", "YB_CONV_EPI", "YB_CONV_EG"):
+    for k in ("YB_CONV_MODE", "YB_CONV_MC", "YB_CONV_EPI", "YB_CONV_EG", "YB_CONV_PP", "YB_CONV_CTAS"):
         L.set_option(k, None)
 
 

@@ -20,7 +20,7 @@ def _rel(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp(min=1e-6))
 
 
-@pytest.mark.parametrize("n,h,w,cin,cout,k,s,in_extra", [
+WGRAD_SHAPES = [
     (2, 16, 16, 64, 128, 3, 1, 0),        # BNW=64, two A blocks
     (3, 13, 13, 128, 64, 1, 1, 0),        # 1x1, cout=64 (single A block), BNW=128
     (2, 20, 12, 32, 64, 3, 1, 0),         # cin=32 -> 64B-swizzled B
@@ -28,9 +28,28 @@ def _rel(a, b):
     (2, 13, 13, 256, 255, 1, 1, 0),       # detection head: cout=255, dz_ld=256
     (2, 52, 52, 64, 128, 3, 2, 0),        # stride 2 (plain dz)
     (2, 32, 32, 32, 64, 3, 2, 0),         # layer-1 shape: cin=32, stride 2, all 9 taps in one CTA
-])
-@pytest.mark.parametrize("dtype", [torch.bfloat16])
+]
+
+
+@pytest.mark.parametrize("n,h,w,cin,cout,k,s,in_extra", WGRAD_SHAPES)
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])    # the fp16 training path runs fp16 wgrad
 def test_wgrad_matches_autograd(n, h, w, cin, cout, k, s, in_extra, dtype):
+    _wgrad_vs_autograd(n, h, w, cin, cout, k, s, in_extra, dtype)
+
+
+@pytest.mark.parametrize("n,h,w,cin,cout,k,s,in_extra", [sh for sh in WGRAD_SHAPES if sh[5] == 3])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_wgrad_one_tap_per_cta(n, h, w, cin, cout, k, s, in_extra, dtype):
+    """YB_WGRAD_TP=1: the 3x3 wgrad with one filter tap per CTA instead of one kernel row (three taps)."""
+    L = _L()
+    L.set_option("YB_WGRAD_TP", "1")
+    try:
+        _wgrad_vs_autograd(n, h, w, cin, cout, k, s, in_extra, dtype)
+    finally:
+        L.set_option("YB_WGRAD_TP", None)
+
+
+def _wgrad_vs_autograd(n, h, w, cin, cout, k, s, in_extra, dtype):
     L = _L()
     g = torch.Generator().manual_seed(1)
     in_ld = cin + in_extra
@@ -42,7 +61,7 @@ def test_wgrad_matches_autograd(n, h, w, cin, cout, k, s, in_extra, dtype):
     dz[..., :cout] = (torch.randn((n, ho, wo, cout), generator=g) * 0.1).to(dtype).cuda()
     dw = torch.zeros((cout, k, k, cin), dtype=torch.float32, device="cuda")
     d = L.ConvDesc(n=n, h=h, w=w, cin=cin, cout=cout, ksize=k, stride=s, in_ld=in_ld, out_ld=dz_ld, res_ld=0,
-                   dtype=L.YB_BF16, out_fp32=0, leaky=0, upsample2x=0)
+                   dtype=L.YB_F16 if dtype == torch.float16 else L.YB_BF16, out_fp32=0, leaky=0, upsample2x=0)
     xp = C.c_void_p(xfull.data_ptr() + off * 2)
     for _ in range(2):   # accumulates: run twice, expect 2x
         L.check(L.lib.yb_conv2d_wgrad(C.byref(d), xp, L.ptr(dz), dz_ld, 0, L.ptr(dw), L.stream_handle()), "wgrad")

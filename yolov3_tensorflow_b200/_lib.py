@@ -36,6 +36,11 @@ class ConvDesc(C.Structure):
                                    "dtype", "out_fp32", "leaky", "upsample2x")]
 
 
+class ConvSchedule(C.Structure):   # yb_conv_schedule_info
+    _fields_ = [(n, i32) for n in ("pingpong", "consumers", "cluster", "block_m", "block_n", "block_k", "stages", "num_kb",
+                                   "num_m_tiles", "num_n_tiles", "grid")]
+
+
 class LayerInfo(C.Structure):
     _fields_ = [(n, i32) for n in ("index", "cin", "cout", "ksize", "stride", "has_bn", "in_h", "in_w", "out_h",
                                    "out_w", "is_head", "scope_index", "upsample2x")]
@@ -54,6 +59,7 @@ _SIGS = {
     "yb_device_info": ([C.POINTER(i32)] * 3, i32),
     "yb_conv2d_fwd": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp], i32),
     "yb_conv_cout_pad": ([i32], i32),
+    "yb_conv_schedule": ([C.POINTER(ConvDesc), i32, i32, i32, i32, C.POINTER(ConvSchedule)], i32),
     "yb_stem_conv_fwd": ([vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
     "yb_conv3x3_thin_fwd": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp], i32),
     "yb_conv3x3_halo_supported": ([C.POINTER(ConvDesc)], i32),

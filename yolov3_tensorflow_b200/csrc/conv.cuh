@@ -17,6 +17,7 @@ struct ConvParams {
   int cluster;            // CTAs per cluster sharing one multicast weight tile (1 | 2 | 4)
   int epi_reg;            // 1: accumulator fragments stored straight from registers (no staging tile)
   int pingpong;           // 1: the two consumer warpgroups take whole tiles in turn (csrc/conv_igemm.cu)
+  int ctas;               // > 0: the persistent grid is capped at this many CTAs (YB_CONV_CTAS; launch_cfg)
   int num_m_tiles, num_n_tiles;
   const float* scale;     // [cout_pad]
   const float* shift;     // [cout_pad]

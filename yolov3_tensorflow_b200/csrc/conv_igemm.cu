@@ -640,6 +640,20 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
   return YB_OK;
 }
 
+// Persistent grid in CTAs: one cluster per work unit, at most one CTA per SM, and at most p.ctas CTAs (rounded down to
+// whole clusters, at least one cluster) when YB_CONV_CTAS caps it.
+static int conv_grid(const ConvParams& p, int sms) {
+  const int cs = p.cluster;
+  const int units = ceil_div(p.num_m_tiles, cs) * p.num_n_tiles;
+  int max_clusters = sms / cs;
+  if (p.ctas > 0) {
+    const int cap = p.ctas / cs > 1 ? p.ctas / cs : 1;
+    if (cap < max_clusters) max_clusters = cap;
+  }
+  const int clusters = units < max_clusters ? units : max_clusters;
+  return clusters * cs;
+}
+
 template <typename T, int BN, int BK, int NC, int DET_E = 0, bool PP = false>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
   using C = Cfg<BN, BK, NC>;
@@ -647,12 +661,9 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv
   auto kern = conv_igemm_kernel<T, BN, BK, NC, DET_E, PP>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int cs = p.cluster;
-  const int units = ceil_div(p.num_m_tiles, cs) * p.num_n_tiles;
-  const int max_clusters = num_sms() / cs;
-  const int clusters = units < max_clusters ? units : max_clusters;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(clusters * cs);
+  cfg.gridDim = dim3(conv_grid(p, num_sms()));
   cfg.blockDim = dim3(C::THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = st;
@@ -667,6 +678,14 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv
 
 int conv_block_k(int cin) { return (cin % 64 == 0) ? 64 : 32; }
 int conv_block_n(int cout_pad) { return (cout_pad % 128 == 0) ? 128 : 64; }
+// operand-ring depth of the kernel conv_launch runs for (block n, block k, consumer warpgroups)
+static int conv_stages(int bn, int bk, int nc) {
+#define YB_STAGES(BN, BK) \
+  if (bn == BN && bk == BK) return nc == 2 ? Cfg<BN, BK, 2>::STAGES : Cfg<BN, BK, 1>::STAGES;
+  YB_STAGES(256, 64) YB_STAGES(128, 64) YB_STAGES(128, 32) YB_STAGES(64, 64) YB_STAGES(64, 32)
+#undef YB_STAGES
+  return 0;
+}
 
 // Launch with prebuilt tensor maps (used by the network plan).
 int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
@@ -700,13 +719,11 @@ int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorM
   return YB_ERR_UNSUPPORTED;
 }
 
-// Build maps + params for one conv.  x/w/out pointers are baked into maps/params.
+// Shape checks, tiling and kernel variant of one conv: everything conv_prepare_core decides before it looks at the
+// data pointers.  yb_conv_schedule reports what this picks.
 // win = 0: the forward rule (ksize x ksize, symmetric padding ksize/2); win = 1: kh x kw window at offsets >= 0.
 // det = 1: one n-tile spans the whole padded cout (the fused-decode detection heads).
-static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
-                             const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
-                             float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
-                             int* cout_pad_out, int det = 0) {
+static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, int det, ConvParams* p) {
   YB_REQUIRE(win || d->ksize == 1 || d->ksize == 3, "conv: ksize must be 1 or 3 (got %d)", d->ksize);
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2 (got %d)", d->stride);
   YB_REQUIRE(!(d->ksize == 1 && d->stride != 1), "conv: 1x1 stride-2 is not on the YOLOv3 path");
@@ -714,10 +731,6 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   YB_REQUIRE(d->dtype == YB_F16 || d->dtype == YB_BF16, "conv: dtype must be f16 or bf16");
   YB_REQUIRE(d->h % d->stride == 0 && d->w % d->stride == 0, "conv: h,w must be divisible by stride");
   YB_REQUIRE(d->in_ld >= d->cin && d->in_ld % 8 == 0, "conv: in_ld %d invalid for cin %d", d->in_ld, d->cin);
-  YB_REQUIRE(x && w_packed && out && (scale == nullptr) == (shift == nullptr), "conv: null pointer");   // scale = shift = NULL: identity
-  YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 &&
-                 ((uintptr_t)res & 15) == 0,
-             "conv: pointers must be 16-byte aligned");
   const int cout_pad = yb_conv_cout_pad(d->cout);
   if (!d->out_fp32) {
     YB_REQUIRE(d->cout % 32 == 0, "conv: 16-bit output needs cout %% 32 == 0 (got %d)", d->cout);
@@ -725,10 +738,7 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   } else {
     YB_REQUIRE(d->out_ld >= d->cout, "conv: out_ld %d invalid", d->out_ld);
   }
-  if (res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0 && !d->out_fp32, "conv: res_ld %d invalid", d->res_ld);
-  YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), "conv: stat_sum/stat_sqsum must both be given");
   const int P = d->h / d->stride, Q = d->w / d->stride;
-  const int bk = conv_block_k(d->cin);
   if (!win) { kh = d->ksize; kw = d->ksize; }
   const int pad = win ? 0 : d->ksize / 2;
   const int bn = det ? cout_pad : conv_block_n(cout_pad);
@@ -738,15 +748,22 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   //   YB_CONV_MODE=2cta   clusters of 2 CTAs (YB_CONV_MC=1: 4) along M sharing one TMA-multicast weight tile
   //   YB_CONV_EPI=reg     accumulators stored straight from registers (not with BN statistics: those sum columns
   //                       over the staging tile)
+  //   YB_CONV_PP=0|1      0: the cooperative schedule wherever ping-pong would run; 1: ping-pong wherever the kernel
+  //                       allows it (two consumer warpgroups, no cluster, staged epilogue), the 1x1 convs with
+  //                       128-column tiles included; unset: the shape rule below
+  //   YB_CONV_CTAS=N      persistent grid capped at N CTAs (rounded down to whole clusters, at least one), so that
+  //                       small tests give every CTA and warpgroup many work units; the kernel is unchanged
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
-  p->epi_reg = (!det && !stat_sum && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  p->epi_reg = (!det && !stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  p->ctas = opt_int("YB_CONV_CTAS", 0);
   // ping-pong wherever the default variant runs, except
   //  - the fused-decode heads: their 256-column tile does not fit 128 rows per warpgroup in registers;
   //  - 1x1 convs with 128-column tiles: their main loop (cin / 64 k-blocks) is too short to hide one warpgroup's
   //    128 x 128 epilogue, and on H100 they measured 2-7 % slower ping-pong than with two warpgroups sharing the
   //    epilogue (DESIGN.md §5).  The 1x1 convs with 64-column tiles and every windowed conv gain from it.
-  const bool pp_shape = kh * kw > 1 || bn != 128;
+  const char* pp = opt("YB_CONV_PP");
+  const bool pp_shape = pp[0] == '1' || (pp[0] != '0' && (kh * kw > 1 || bn != 128));
   p->pingpong = (!det && p->consumers == 2 && p->cluster == 1 && !p->epi_reg && pp_shape) ? 1 : 0;
   const int block_m = 64 * p->consumers;
   memset(&p->det, 0, sizeof(p->det));
@@ -755,11 +772,32 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   p->im2col = kh * kw > 1;
   p->num_m_tiles = ceil_div(p->M, block_m);
   p->num_n_tiles = cout_pad / bn;
+  p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
+  return YB_OK;
+}
+
+// Build maps + params for one conv.  x/w/out pointers are baked into maps/params.
+static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
+                             const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
+                             float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
+                             int* cout_pad_out, int det = 0) {
+  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, det, p);
+  if (rc) return rc;
+  YB_REQUIRE(x && w_packed && out && (scale == nullptr) == (shift == nullptr), "conv: null pointer");   // scale = shift = NULL: identity
+  YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 &&
+                 ((uintptr_t)res & 15) == 0,
+             "conv: pointers must be 16-byte aligned");
+  if (res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0 && !d->out_fp32, "conv: res_ld %d invalid", d->res_ld);
+  YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), "conv: stat_sum/stat_sqsum must both be given");
+  const int cout_pad = yb_conv_cout_pad(d->cout);
+  const int bk = conv_block_k(d->cin);
+  const int pad = p->pad;
+  kh = p->kh; kw = p->kw;
+  const int block_m = 64 * p->consumers;
+  const int bn = det ? cout_pad : conv_block_n(cout_pad);
   p->scale = scale; p->shift = shift;
   p->out = out; p->out_ld = d->out_ld; p->res = res; p->res_ld = d->res_ld;
-  p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
   p->stat_sum = stat_sum; p->stat_sqsum = stat_sqsum;
-  int rc;
   if (p->im2col) {
     rc = make_tmap_im2col_px(tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride, pad, bk,
                              block_m);
@@ -806,6 +844,34 @@ int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const v
 }  // namespace yb
 
 extern "C" int yb_conv_cout_pad(int cout) { return (cout + 63) / 64 * 64; }
+
+// host-only view of conv_select + conv_grid (tests): the kernel yb_conv2d_fwd (kh = kw = 0) or one parity class of
+// yb_conv2d_dgrad_s2 (kh x kw window) would launch with the current options on a device with sm_count SMs
+extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count,
+                                yb_conv_schedule_info* info) {
+  YB_REQUIRE(d && info && sm_count > 0, "conv_schedule: bad argument");
+  const int win = kh != 0 || kw != 0;
+  if (win) {
+    YB_REQUIRE(kh >= 1 && kh <= 2 && kw >= 1 && kw <= 2, "conv_schedule: bad window");
+    YB_REQUIRE(d->stride == 1 && !with_stats, "conv_schedule: windows are stride-1 without statistics");
+  }
+  yb::ConvParams p;
+  memset(&p, 0, sizeof(p));
+  const int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, 0, &p);
+  if (rc) return rc;
+  info->pingpong = p.pingpong;
+  info->consumers = p.consumers;
+  info->cluster = p.cluster;
+  info->block_m = 64 * p.consumers;
+  info->block_n = yb::conv_block_n(yb_conv_cout_pad(d->cout));
+  info->block_k = yb::conv_block_k(d->cin);
+  info->stages = yb::conv_stages(info->block_n, info->block_k, p.consumers);
+  info->num_kb = p.kh * p.kw * d->cin / info->block_k;
+  info->num_m_tiles = p.num_m_tiles;
+  info->num_n_tiles = p.num_n_tiles;
+  info->grid = yb::conv_grid(p, sm_count);
+  return YB_OK;
+}
 
 extern "C" int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
                              const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,
