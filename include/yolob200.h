@@ -377,6 +377,37 @@ int yb_net_train_fwd_bwd(yb_net* net, const float* images, const float* y_true_1
  * all-reduce of a finished bucket (detection heads first) while the next bucket's backward is running. */
 int yb_net_train_backward(yb_net* net, const float* images, int first_layer, int last_layer, int flags, void* stream);
 int yb_net_grad_range(yb_net* net, int first_layer, int last_layer, float** ptr, size_t* count);
+/* ---- synchronised batch norm for data-parallel training: the step as per-layer calls with exchange points ----
+ * Each layer runs in two phases.  YB_PHASE_LOCAL computes per-replica sums: forward, the conv and its batch sums
+ * Σz / Σz² (layer 0 also zeroes the per-step sums and, unless YB_TRAIN_FORWARD_ONLY, the flat gradient); backward,
+ * the BN gradient sums Σdact·ẑ / Σdact.  YB_PHASE_GLOBAL consumes them: forward, statistics -> scale / shift, the
+ * moving-statistics update and the activation; backward, dz, the weight gradient (on a side stream) and the input
+ * gradient.  Between the two phases of a BN layer the caller sums the layer's exchange slab (yb_net_bn_exchange_buffer)
+ * across the ranks in place.  A detection conv (no BN) has nothing to exchange: its forward runs in LOCAL, its bias
+ * gradient in backward LOCAL.
+ * Order of one step: forward_layer(0, LOCAL), (0, GLOBAL), ... (74, GLOBAL); train_loss; backward_layer(74, LOCAL),
+ * (74, GLOBAL), ... (0, GLOBAL); then yb_net_train_join and yb_net_train_update.  A call out of this order fails with
+ * YB_ERR_INVALID_ARGUMENT before any device work; forward_layer(0, LOCAL) always starts a new step.
+ * bn_replicas (>= 1, the same for every call of a step) multiplies the rows the statistics cover:
+ * M = bn_replicas * n * out_h * out_w, in the mean / variance, the backward and the unbiased-variance factor of the
+ * moving-statistics update.  Every rank must therefore run the same n, H and W in a step.  With bn_replicas = 1 and
+ * no exchange the calls compute what yb_net_train_fwd_bwd computes.  The flat gradient holds the LOCAL dgamma / dbeta
+ * and rank-local weight gradients whose all-reduce times 1/world is the gradient of the concatenated batch. */
+enum { YB_PHASE_LOCAL = 0, YB_PHASE_GLOBAL = 1 };
+int yb_net_train_forward_layer(yb_net* net, const float* images, int layer, int phase, int bn_replicas, float bn_decay,
+                               float* fm1, float* fm2, float* fm3, int flags, void* stream);
+/* compute_loss of yb_net_train_fwd_bwd on the feature maps the forward wrote: zeroes loss4, then accumulates into it
+ * and writes d(loss)/d(feature maps) for the backward. */
+int yb_net_train_loss(yb_net* net, const float* y_true_1, const float* y_true_2, const float* y_true_3,
+                      const float* anchors9x2, int use_label_smooth, int use_focal_loss, float loss_scale,
+                      double* loss4, void* stream);
+int yb_net_train_backward_layer(yb_net* net, const float* images, int layer, int phase, int bn_replicas, int flags,
+                                void* stream);
+/* makes `stream` wait for the weight-gradient side stream: call before all-reducing a finished gradient range and
+ * after the last backward call. */
+int yb_net_train_join(yb_net* net, void* stream);
+/* BN layer `layer`'s exchange slab, 2 x cout_pad floats: forward [Σz | Σz²], backward [Σdact·ẑ | Σdact]. */
+int yb_net_bn_exchange_buffer(yb_net* net, int layer, int backward, float** ptr, size_t* count);
 /* the flat float32 gradient of all 222 trainable tensors (creation order: per conv w [OHWI], then gamma, beta
  * | bias; each padded to 4 floats) — the buffer a data-parallel wrapper all-reduces. */
 int yb_net_grad_buffer(yb_net* net, float** ptr, size_t* count);

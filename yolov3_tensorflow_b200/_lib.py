@@ -15,6 +15,7 @@ YB_F16, YB_BF16, YB_F32 = 0, 1, 2
 YB_W_HWIO, YB_W_OIHW, YB_W_OHWI = 0, 1, 2
 YB_OPT_SGD, YB_OPT_MOMENTUM, YB_OPT_RMSPROP, YB_OPT_ADAM = 0, 1, 2, 3
 YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
+YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
 
 
 class YoloB200Error(RuntimeError):
@@ -113,6 +114,11 @@ _SIGS = {
     "yb_net_train_fwd_bwd": ([vp, vp, vp, vp, vp, C.POINTER(f32), i32, i32, f32, f32, vp, vp, vp, vp, i32, vp], i32),
     "yb_net_train_backward": ([vp, vp, i32, i32, i32, vp], i32),
     "yb_net_grad_range": ([vp, i32, i32, C.POINTER(vp), C.POINTER(sz)], i32),
+    "yb_net_train_forward_layer": ([vp, vp, i32, i32, i32, f32, vp, vp, vp, i32, vp], i32),
+    "yb_net_train_loss": ([vp, vp, vp, vp, C.POINTER(f32), i32, i32, f32, vp, vp], i32),
+    "yb_net_train_backward_layer": ([vp, vp, i32, i32, i32, i32, vp], i32),
+    "yb_net_train_join": ([vp, vp], i32),
+    "yb_net_bn_exchange_buffer": ([vp, i32, i32, C.POINTER(vp), C.POINTER(sz)], i32),
     "yb_net_grad_buffer": ([vp, C.POINTER(vp), C.POINTER(sz)], i32),
     "yb_net_train_update": ([vp, C.POINTER(Optimizer), vp], i32),
     "yb_net_train_reset_state": ([vp, i32, vp], i32),

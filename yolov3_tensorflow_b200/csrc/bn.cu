@@ -9,6 +9,8 @@
 //   bn_bwd_reduce    : dbeta = sum(dact), dgamma = sum(dact * zhat), dact = dA * leaky'(y)
 //   bn_bwd_apply     : dz = gamma*invstd*(dact - dbeta/M - zhat*dgamma/M), optional
 //                      zero-insertion (dilated) store for the dgrad of stride-2 convs
+// M is the number of rows the statistics cover: n*h*w on one device, replicas*n*h*w under synchronised BN, where
+// the sums are all-reduced across equal-shaped ranks between the producing and the consuming kernel.
 //   col_sum          : bias gradient of the detection convs
 // All are HBM-bound streaming kernels over [rows, C] NHWC 16-bit tensors (C % 8 == 0):
 // a thread owns 8 consecutive channels (one 16-byte load), a block a slab of rows.
@@ -267,7 +269,8 @@ bn_bwd_reduce_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__
                      const float* __restrict__ scale, const float* __restrict__ shift,
                      const float* __restrict__ save_mean, const float* __restrict__ save_invstd, RowGeom g,
                      StreamGeom sg, int leaky, int upsample, int vec, float* __restrict__ dgamma,
-                     float* __restrict__ dbeta, float* __restrict__ partial, unsigned int* __restrict__ ticket) {
+                     float* __restrict__ dbeta, float* __restrict__ partial, unsigned int* __restrict__ ticket,
+                     float* __restrict__ xg, float* __restrict__ xb) {
   using CV = ChanVec<T, CPT>;
   __shared__ float s_g[256][CPT + 1], s_b[256][CPT + 1];
   __shared__ unsigned int s_last;
@@ -345,7 +348,8 @@ bn_bwd_reduce_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__
     float acc = 0.f;
 #pragma unroll
     for (int sl = 0; sl < BN_SLOTS; ++sl) { acc += v[sl]; partial[(long)sl * 2 * g.c + c] = 0.f; }   // re-armed
-    if (c < g.c) dgamma[c] = acc; else dbeta[c - g.c] = acc;
+    if (c < g.c) { dgamma[c] = acc; if (xg) xg[c] = acc; }
+    else { dbeta[c - g.c] = acc; if (xb) xb[c - g.c] = acc; }
   }
   if (threadIdx.x == 0) *ticket = 0u;   // ready for the next launch
 }
@@ -356,11 +360,11 @@ bn_bwd_apply_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__ 
                     const float* __restrict__ gamma, const float* __restrict__ scale, const float* __restrict__ shift,
                     const float* __restrict__ save_mean, const float* __restrict__ save_invstd,
                     const float* __restrict__ dgamma, const float* __restrict__ dbeta, RowGeom g, StreamGeom sg,
-                    int leaky, int upsample, int dilate, int vec, T* __restrict__ dz, long dz_ld) {
+                    int leaky, int upsample, int dilate, int vec, float count, T* __restrict__ dz, long dz_ld) {
   using CV = ChanVec<T, CPT>;
   const int cvi = threadIdx.x % sg.cv, lane_r = threadIdx.x / sg.cv;
   const int c0 = cvi * CPT;
-  const float inv_m = 1.f / (float)g.rows;
+  const float inv_m = 1.f / count;
   // dz = k1*dact + k2*z + k3   with   k1 = gamma*invstd, k2 = -k1*invstd*dgamma/M, k3 = -k1*dbeta/M - k2*mean
   float sc[CPT], sh[CPT], k1[CPT], k2[CPT], k3[CPT];
   ldc<CPT>(scale + c0, vec, sc); ldc<CPT>(shift + c0, vec, sh);
@@ -514,20 +518,32 @@ extern "C" int yb_bn_act_apply(const void* z, long z_ld, const float* scale, con
 }
 
 // yb_bn_finalize + yb_bn_act_apply in one launch (same arguments, same results): the training forward of a BN conv
+namespace yb {
+// count: the rows the sums cover (n*h*w, or replicas*n*h*w when the sums were all-reduced across ranks)
+int bn_stats_act_apply_n(const void* z, long z_ld, const float* sum, const float* sqsum, long count, const float* gamma,
+                         const float* beta, float eps, float decay, float* moving_mean, float* moving_var, float* scale,
+                         float* shift, float* save_mean, float* save_invstd, const void* res, long res_ld, void* out,
+                         long out_ld, int n, int h, int w, int c, int dtype, int leaky, int upsample2x, void* stream) {
+  YB_BN_COMMON_CHECK("bn_stats_act_apply");
+  YB_REQUIRE(count >= (long)n * h * w, "bn_stats_act_apply: count must cover the local rows");
+  YB_REQUIRE(z && out && gamma && beta && scale && shift && save_mean && save_invstd, "bn_stats_act_apply: null pointer");
+  YB_REQUIRE((sum == nullptr) == (sqsum == nullptr), "bn_stats_act_apply: sum/sqsum must both be given (both NULL: frozen BN)");
+  YB_REQUIRE((moving_mean == nullptr) == (moving_var == nullptr), "bn_stats_act_apply: moving_mean/var must both be given");
+  YB_REQUIRE(sum || moving_mean, "bn_stats_act_apply: frozen BN needs the moving statistics");
+  BnFin f{sum, sqsum, gamma, beta, moving_mean, moving_var, scale, shift, save_mean, save_invstd, (float)count, eps, decay};
+  return launch_act_apply(z, z_ld, nullptr, nullptr, res, res_ld, out, out_ld, n, h, w, c, dtype, leaky, upsample2x, &f,
+                          static_cast<cudaStream_t>(stream));
+}
+}  // namespace yb
+
 extern "C" int yb_bn_stats_act_apply(const void* z, long z_ld, const float* sum, const float* sqsum, const float* gamma,
                                      const float* beta, float eps, float decay, float* moving_mean, float* moving_var,
                                      float* scale, float* shift, float* save_mean, float* save_invstd, const void* res,
                                      long res_ld, void* out, long out_ld, int n, int h, int w, int c, int dtype,
                                      int leaky, int upsample2x, void* stream) {
-  YB_BN_COMMON_CHECK("bn_stats_act_apply");
-  YB_REQUIRE(z && out && gamma && beta && scale && shift && save_mean && save_invstd, "bn_stats_act_apply: null pointer");
-  YB_REQUIRE((sum == nullptr) == (sqsum == nullptr), "bn_stats_act_apply: sum/sqsum must both be given (both NULL: frozen BN)");
-  YB_REQUIRE((moving_mean == nullptr) == (moving_var == nullptr), "bn_stats_act_apply: moving_mean/var must both be given");
-  YB_REQUIRE(sum || moving_mean, "bn_stats_act_apply: frozen BN needs the moving statistics");
-  BnFin f{sum, sqsum, gamma, beta, moving_mean, moving_var, scale, shift, save_mean, save_invstd,
-          (float)((long)n * h * w), eps, decay};
-  return launch_act_apply(z, z_ld, nullptr, nullptr, res, res_ld, out, out_ld, n, h, w, c, dtype, leaky, upsample2x, &f,
-                          static_cast<cudaStream_t>(stream));
+  return bn_stats_act_apply_n(z, z_ld, sum, sqsum, (long)n * h * w, gamma, beta, eps, decay, moving_mean, moving_var,
+                              scale, shift, save_mean, save_invstd, res, res_ld, out, out_ld, n, h, w, c, dtype, leaky,
+                              upsample2x, stream);
 }
 
 extern "C" int yb_bn_bwd_reduce_workspace_bytes(size_t* bytes) {
@@ -536,12 +552,15 @@ extern "C" int yb_bn_bwd_reduce_workspace_bytes(size_t* bytes) {
   return YB_OK;
 }
 
-extern "C" int yb_bn_bwd_reduce(const void* dA, long dA_ld, const void* z, long z_ld, const float* scale,
-                                const float* shift, const float* save_mean, const float* save_invstd, int n, int h,
-                                int w, int c, int dtype, int leaky, int upsample2x, float* dgamma, float* dbeta,
-                                void* workspace, void* stream) {
+namespace yb {
+// xg / xb (optional, both or neither, needs a workspace): the final block also stores the two sums there — the
+// exchange slab a synchronised-BN caller all-reduces while dgamma / dbeta keep the local sums
+int bn_bwd_reduce_x(const void* dA, long dA_ld, const void* z, long z_ld, const float* scale, const float* shift,
+                    const float* save_mean, const float* save_invstd, int n, int h, int w, int c, int dtype, int leaky,
+                    int upsample2x, float* dgamma, float* dbeta, void* workspace, float* xg, float* xb, void* stream) {
   YB_BN_COMMON_CHECK("bn_bwd_reduce");
   YB_REQUIRE(dA && z && scale && shift && save_mean && save_invstd && dgamma && dbeta, "bn_bwd_reduce: null pointer");
+  YB_REQUIRE((xg == nullptr) == (xb == nullptr) && (xg == nullptr || workspace), "bn_bwd_reduce: bad exchange slab");
   RowGeom g{(long)n * h * w, h, w, c};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int grid;
@@ -558,21 +577,32 @@ extern "C" int yb_bn_bwd_reduce(const void* dA, long dA_ld, const void* z, long 
 #define YB_RED_LAUNCH(T, CPT, R, BPS)                                                                                  \
   bn_bwd_reduce_kernel<T, CPT, R, BPS><<<grid, 256, 0, st>>>((const T*)dA, dA_ld, (const T*)z, z_ld, scale, shift,      \
                                                              save_mean, save_invstd, g, sg, leaky, upsample2x, vec,   \
-                                                             dgamma, dbeta, partial, ticket)
+                                                             dgamma, dbeta, partial, ticket, xg, xb)
   YB_BN_DTYPES(YB_RED_LAUNCH)
 #undef YB_RED_LAUNCH
   YB_CUDA(cudaGetLastError());
   return YB_OK;
 }
+}  // namespace yb
 
-extern "C" int yb_bn_bwd_apply(const void* dA, long dA_ld, const void* z, long z_ld, const float* gamma,
-                               const float* scale, const float* shift, const float* save_mean,
-                               const float* save_invstd, const float* dgamma, const float* dbeta, int n, int h, int w,
-                               int c, int dtype, int leaky, int upsample2x, int dilate2x, void* dz, long dz_ld,
-                               void* stream) {
+extern "C" int yb_bn_bwd_reduce(const void* dA, long dA_ld, const void* z, long z_ld, const float* scale,
+                                const float* shift, const float* save_mean, const float* save_invstd, int n, int h,
+                                int w, int c, int dtype, int leaky, int upsample2x, float* dgamma, float* dbeta,
+                                void* workspace, void* stream) {
+  return bn_bwd_reduce_x(dA, dA_ld, z, z_ld, scale, shift, save_mean, save_invstd, n, h, w, c, dtype, leaky, upsample2x,
+                         dgamma, dbeta, workspace, nullptr, nullptr, stream);
+}
+
+namespace yb {
+// count: the rows dgamma / dbeta cover (n*h*w, or replicas*n*h*w for all-reduced sums)
+int bn_bwd_apply_n(const void* dA, long dA_ld, const void* z, long z_ld, const float* gamma, const float* scale,
+                   const float* shift, const float* save_mean, const float* save_invstd, const float* dgamma,
+                   const float* dbeta, long count, int n, int h, int w, int c, int dtype, int leaky, int upsample2x,
+                   int dilate2x, void* dz, long dz_ld, void* stream) {
   YB_BN_COMMON_CHECK("bn_bwd_apply");
   YB_REQUIRE(dA && z && gamma && scale && shift && save_mean && save_invstd && dgamma && dbeta && dz,
              "bn_bwd_apply: null pointer");
+  YB_REQUIRE(count >= (long)n * h * w, "bn_bwd_apply: count must cover the local rows");
   RowGeom g{(long)n * h * w, h, w, c};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int grid;
@@ -582,11 +612,21 @@ extern "C" int yb_bn_bwd_apply(const void* dA, long dA_ld, const void* z, long z
 #define YB_APP_LAUNCH(T, CPT, R, BPS)                                                                                  \
   bn_bwd_apply_kernel<T, CPT, R, BPS><<<grid, 256, 0, st>>>((const T*)dA, dA_ld, (const T*)z, z_ld, gamma, scale,      \
                                                             shift, save_mean, save_invstd, dgamma, dbeta, g, sg, leaky, \
-                                                            upsample2x, dilate2x, vec, (T*)dz, dz_ld)
+                                                            upsample2x, dilate2x, vec, (float)count, (T*)dz, dz_ld)
   YB_BN_DTYPES(YB_APP_LAUNCH)
 #undef YB_APP_LAUNCH
   YB_CUDA(cudaGetLastError());
   return YB_OK;
+}
+}  // namespace yb
+
+extern "C" int yb_bn_bwd_apply(const void* dA, long dA_ld, const void* z, long z_ld, const float* gamma,
+                               const float* scale, const float* shift, const float* save_mean,
+                               const float* save_invstd, const float* dgamma, const float* dbeta, int n, int h, int w,
+                               int c, int dtype, int leaky, int upsample2x, int dilate2x, void* dz, long dz_ld,
+                               void* stream) {
+  return bn_bwd_apply_n(dA, dA_ld, z, z_ld, gamma, scale, shift, save_mean, save_invstd, dgamma, dbeta, (long)n * h * w,
+                        n, h, w, c, dtype, leaky, upsample2x, dilate2x, dz, dz_ld, stream);
 }
 
 extern "C" int yb_col_stats(const void* x, long ld, long rows, int c, int dtype, float* sum, float* sqsum, void* stream);

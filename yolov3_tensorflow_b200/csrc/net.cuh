@@ -49,6 +49,7 @@ struct Layer {
   ConvParams d4_params[4];
   int d4_cout_pad[4] = {0, 0, 0, 0};
   size_t st_sum = 0, st_sqsum = 0, st_mean = 0, st_invstd = 0, st_scale = 0, st_shift = 0;   // fp32 [cout_pad] each
+  size_t x_bwd = 0;                  // fp32 [2][cout_pad]: sync-BN backward exchange slab (sum dact*zhat | sum dact)
   size_t w_dgrad = 0;                // [cin_pad, k, k, k_cout] 16-bit (param arena)
   long g_w = -1, g_gamma = -1, g_beta = -1, g_bias = -1;   // float offsets into the flat gradient / velocity buffers
   ConvParams tparams;                // training-mode forward conv (raw z + statistics)
@@ -71,6 +72,7 @@ struct yb_net {
   std::vector<size_t> gbuf_offset;   // gradient mirror of every 16-bit activation buffer
   size_t dfm_off[3] = {0, 0, 0};     // 16-bit [rows, 256] loss gradients of the three detection maps
   size_t stats_off = 0, stats_bytes = 0;   // per-step zeroed BN sums
+  size_t xbwd_off = 0, xbwd_bytes = 0;     // sync-BN backward exchange slabs
   size_t lossws_off = 0, lossws_bytes = 0;
   size_t bnws_off = 0, bnws_bytes = 0;     // two-stage BN-backward reduction scratch (zeroed at bind)
   size_t ones_off = 0, zeros_off = 0;      // fp32 [1024] constants (param arena)
@@ -87,6 +89,10 @@ struct yb_net {
   // side stream of the backward pass: layer L's wgrad runs beside its dgrad (net_train.cu); created on first use
   cudaStream_t side_stream = nullptr;
   cudaEvent_t side_fork = nullptr, side_join = nullptr;
+  bool side_forked = false;           // work on the side stream not yet joined
+  // layered training step (yb_net_train_forward_layer ...): the feature maps the forward wrote, and the next call
+  float* train_fm[3] = {nullptr, nullptr, nullptr};
+  int step_slot = -1, step_replicas = 1;
   ~yb_net() {
     if (side_fork) cudaEventDestroy(side_fork);
     if (side_join) cudaEventDestroy(side_join);

@@ -19,6 +19,18 @@ namespace yb {
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
                  const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
                  ConvParams* p, int* cout_pad_out);
+// bn.cu: the BN kernels with the row count and the backward exchange slab exposed
+int bn_stats_act_apply_n(const void* z, long z_ld, const float* sum, const float* sqsum, long count, const float* gamma,
+                         const float* beta, float eps, float decay, float* moving_mean, float* moving_var, float* scale,
+                         float* shift, float* save_mean, float* save_invstd, const void* res, long res_ld, void* out,
+                         long out_ld, int n, int h, int w, int c, int dtype, int leaky, int upsample2x, void* stream);
+int bn_bwd_reduce_x(const void* dA, long dA_ld, const void* z, long z_ld, const float* scale, const float* shift,
+                    const float* save_mean, const float* save_invstd, int n, int h, int w, int c, int dtype, int leaky,
+                    int upsample2x, float* dgamma, float* dbeta, void* workspace, float* xg, float* xb, void* stream);
+int bn_bwd_apply_n(const void* dA, long dA_ld, const void* z, long z_ld, const float* gamma, const float* scale,
+                   const float* shift, const float* save_mean, const float* save_invstd, const float* dgamma,
+                   const float* dbeta, long count, int n, int h, int w, int c, int dtype, int leaky, int upsample2x,
+                   int dilate2x, void* dz, long dz_ld, void* stream);
 
 static size_t al256(size_t v) { return (v + 255) & ~size_t(255); }
 
@@ -62,6 +74,14 @@ void train_layout(yb_net* net) {
   }
   o = al256(o);
   net->stats_bytes = o - net->stats_off;
+  // backward exchange slabs [sum dact*zhat | sum dact] of synchronised BN (padding zeroed at bind)
+  net->xbwd_off = o;
+  for (auto& L : net->layers) {
+    if (!L.info.has_bn) continue;
+    L.x_bwd = o; o += 2 * (size_t)L.cout_pad * 4;
+  }
+  o = al256(o);
+  net->xbwd_bytes = o - net->xbwd_off;
   for (auto& L : net->layers) {
     if (!L.info.has_bn) continue;
     L.st_mean = o; o = al256(o + (size_t)L.cout_pad * 4);
@@ -149,6 +169,7 @@ int train_bind(yb_net* net, cudaStream_t st) {
   YB_CUDA(cudaGetLastError());
   YB_CUDA(cudaMemsetAsync(net->par + net->zeros_off, 0, 1024 * 4, st));
   YB_CUDA(cudaMemsetAsync(net->act + net->bnws_off, 0, net->bnws_bytes, st));
+  YB_CUDA(cudaMemsetAsync(net->act + net->xbwd_off, 0, net->xbwd_bytes, st));
   const float* ones = fpar(net, net->ones_off);
   const float* zeros = fpar(net, net->zeros_off);
   for (auto& L : net->layers) {
@@ -285,91 +306,234 @@ static int refresh_all_dgrad_weights(yb_net* net, void* stream) {
 
 using namespace yb;
 
+namespace yb {
+
+// ---- one training step as per-layer, two-phase steps -------------------------------------------------------------
+// The fused entry points (yb_net_train_fwd_bwd / yb_net_train_backward) and the layered exports used by synchronised
+// batch norm run the same helpers below.  LOCAL phases produce per-replica sums, GLOBAL phases consume them; under
+// sync BN the caller all-reduces the layer's exchange slab between the two.  `replicas` multiplies the row count the
+// GLOBAL math divides by (every rank runs the same n x h x w in a step); the fused path passes 1.
+
+// forward.  LOCAL: the conv and its batch sums (layer 0 also zeroes the per-step sums and, unless forward-only, the
+// flat gradient); a detection conv is done here.  GLOBAL: sums -> scale/shift (+ moving statistics) -> apply.
+static int train_fwd_layer(yb_net* net, int i, int phase, const float* images, int replicas, float bn_decay,
+                           float* const user_fm[3], int flags, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool bn_frozen = (flags & YB_TRAIN_BN_FROZEN) != 0;
+  const int n = net->n, dt = net->dtype;
+  const float* ones = fpar(net, net->ones_off);
+  const float* zeros = fpar(net, net->zeros_off);
+  Layer& L = net->layers[i];
+  const long rows = (long)n * L.info.out_h * L.info.out_w;
+  int rc;
+  if (phase == YB_PHASE_LOCAL) {
+    if (i == 0) {
+      YB_CUDA(cudaMemsetAsync(net->act + net->stats_off, 0, net->stats_bytes, st));
+      if (!(flags & YB_TRAIN_FORWARD_ONLY)) YB_CUDA(cudaMemsetAsync(net->par + net->grad_off, 0, (size_t)net->grad_count * 4, st));
+      if (opt("YB_STEM_TRAIN")[0] != 'c') {   // warp-level tensor path, batch statistics accumulated by the same kernel
+        return yb_stem_conv_fwd_tc_stats(images, fpar(net, L.w_master), ones, zeros, n, net->h, net->w, dt, 0,
+                                         net->act + L.z_off, fact(net, L.st_sum), fact(net, L.st_sqsum), stream);
+      }
+      // YB_STEM_TRAIN=cuda: the fp32 CUDA-core stem + a column-statistics pass (the first version)
+      rc = yb_stem_conv_fwd(images, fpar(net, L.w_master), ones, zeros, n, net->h, net->w, L.info.cout, dt, 0,
+                            net->act + L.z_off, stream);
+      if (rc) return rc;
+      return yb_col_stats(net->act + L.z_off, L.info.cout, rows, L.info.cout, dt, fact(net, L.st_sum), fact(net, L.st_sqsum), stream);
+    }
+    ConvParams p = L.tparams;
+    if (!L.info.has_bn) {
+      const int which = L.out.buf == net->fm_buf[0] ? 0 : (L.out.buf == net->fm_buf[1] ? 1 : 2);
+      p.out = user_fm[which] ? (void*)user_fm[which] : (void*)(net->act + net->bufs[L.out.buf].offset);
+      net->train_fm[which] = static_cast<float*>(p.out);
+    }
+    return conv_launch(dt, L.cout_pad, L.tmA, L.tmB, p, st);
+  }
+  if (!L.info.has_bn) return YB_OK;
+  if (!bn_frozen) net->fold_dirty = true;
+  const long count = (long)replicas * rows;
+  const void* resp = L.res.buf >= 0 ? ten_ptr2(net, L.res) : nullptr;
+  const long res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
+  if (opt("YB_BN_FIN")[0] != '0') {   // statistics -> scale/shift inside the apply kernel (one launch per BN layer instead of two)
+    return bn_stats_act_apply_n(net->act + L.z_off, L.info.cout, bn_frozen ? nullptr : fact(net, L.st_sum),
+                                bn_frozen ? nullptr : fact(net, L.st_sqsum), count, fpar(net, L.gamma), fpar(net, L.beta),
+                                net->bn_eps, bn_decay, fpar(net, L.mean), fpar(net, L.var), fact(net, L.st_scale),
+                                fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), resp, res_ld,
+                                ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w,
+                                L.info.cout, dt, 1, L.upsample ? 1 : 0, stream);
+  }
+  rc = yb_bn_finalize(bn_frozen ? nullptr : fact(net, L.st_sum), bn_frozen ? nullptr : fact(net, L.st_sqsum), count,
+                      L.info.cout, fpar(net, L.gamma), fpar(net, L.beta),
+                      net->bn_eps, bn_decay, fpar(net, L.mean), fpar(net, L.var), fact(net, L.st_scale),
+                      fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), stream);
+  if (rc) return rc;
+  return yb_bn_act_apply(net->act + L.z_off, L.info.cout, fact(net, L.st_scale), fact(net, L.st_shift), resp, res_ld,
+                         ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1,
+                         L.upsample ? 1 : 0, stream);
+}
+
+// loss + d(loss)/d(feature maps) of the maps the forward wrote (loss4 accumulates; the callers zero it)
+static int train_loss(yb_net* net, const float* const y_true[3], const float* anchors9x2, int use_label_smooth,
+                      int use_focal_loss, float loss_scale, double* loss4, void* stream) {
+  const int n = net->n;
+  for (int s = 0; s < 3; ++s) {
+    const int div = 32 >> s;
+    int rc = yb_loss_layer(net->train_fm[s], y_true[s], n, net->h / div, net->w / div, net->h, net->w, net->class_num,
+                           anchors9x2 + 2 * 3 * (2 - s), use_label_smooth, use_focal_loss, 1.0f / (float)n, loss_scale,
+                           net->act + net->lossws_off, net->lossws_bytes, loss4, net->act + net->dfm_off[s], net->dtype,
+                           (3 * (5 + net->class_num) + 31) / 32 * 32, stream);
+    if (rc) return rc;
+  }
+  return YB_OK;
+}
+
+// makes `stream` wait for the wgrad side stream (no-op when nothing was forked since the last join)
+static int train_join(yb_net* net, cudaStream_t st) {
+  if (!net->side_forked) return YB_OK;
+  YB_CUDA(cudaEventRecord(net->side_join, net->side_stream));
+  YB_CUDA(cudaStreamWaitEvent(st, net->side_join, 0));
+  net->side_forked = false;
+  return YB_OK;
+}
+
+// backward.  LOCAL: the BN gradient sums (dgamma / dbeta; with `exchange` also into the layer's exchange slab), or the
+// bias gradient of a detection conv.  GLOBAL: dz from the sums (the slab's with `exchange`), then wgrad and dgrad.
+//
+// Synchronised BN.  With W ranks of N images each, the loss is a mean over the local batch, so rank r's dA_r is
+// W x the gradient of the global loss (mean over W*N) w.r.t. its rows.  The normalisation over all M = W*n*h*w rows
+// makes the exact input gradient of the concatenated batch, for rank r's rows,
+//   dz_r = gamma*invstd*(dact_r - SUM_ranks(sum dact)/M - zhat_r * SUM_ranks(sum dact*zhat)/M)
+// evaluated with the global-loss dact; using the rank-local dact_r (W x that) gives W x the big-batch dz.  Everything
+// below is linear in dz, so every weight gradient of rank r is W x its share of the big-batch gradient, and the
+// all-reduce (sum) of the flat gradient followed by the optimizer's 1/W gives exactly the big-batch gradient.  The
+// same holds for dgamma / dbeta, which therefore keep the LOCAL sums in the flat gradient.
+static int train_bwd_layer(yb_net* net, int i, int phase, const float* images, int replicas, bool exchange, int flags,
+                           void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool bn_frozen = (flags & YB_TRAIN_BN_FROZEN) != 0;
+  const int n = net->n, dt = net->dtype;
+  Layer& L = net->layers[i];
+  const long rows = (long)n * L.info.out_h * L.info.out_w;
+  float* xg = exchange && L.info.has_bn ? fact(net, L.x_bwd) : nullptr;
+  float* xb = xg ? xg + L.cout_pad : nullptr;
+  int rc;
+  if (phase == YB_PHASE_LOCAL) {
+    if (!L.info.has_bn) return yb_col_sum(net->act + L.dz_off, L.dz_ld, rows, L.info.cout, dt, gradp(net, L.g_bias), stream);
+    return bn_bwd_reduce_x(gten_ptr(net, L.out), net->bufs[L.out.buf].ld, net->act + L.z_off, L.info.cout,
+                           fact(net, L.st_scale), fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), n,
+                           L.info.out_h, L.info.out_w, L.info.cout, dt, 1, L.upsample ? 1 : 0, gradp(net, L.g_gamma),
+                           gradp(net, L.g_beta), net->act + net->bnws_off, xg, xb, stream);
+  }
+  if (L.info.has_bn) {
+    // frozen BN: mean / variance are constants -> dz = gamma * invstd * dact (the batch-statistic terms vanish)
+    const float* zeros = fpar(net, net->zeros_off);
+    const float* sg = bn_frozen ? zeros : (xg ? xg : gradp(net, L.g_gamma));
+    const float* sb = bn_frozen ? zeros : (xb ? xb : gradp(net, L.g_beta));
+    rc = bn_bwd_apply_n(gten_ptr(net, L.out), net->bufs[L.out.buf].ld, net->act + L.z_off, L.info.cout, fpar(net, L.gamma),
+                        fact(net, L.st_scale), fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), sg, sb,
+                        (long)replicas * rows, n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1, L.upsample ? 1 : 0,
+                        L.dz_dilated, net->act + L.dz_off, L.dz_ld, stream);
+    if (rc) return rc;
+  }
+  if (i == 0) return yb_stem_conv_wgrad(images, net->act + L.dz_off, dt, n, net->h, net->w, gradp(net, L.g_w), stream);
+  // Layer L's weight gradient and input gradient both only read dz_L: the wgrad goes to a side stream and runs beside
+  // the dgrad (and the next layer's BN backward).  Both kernels own a whole SM per CTA, so the gain is in the tails:
+  // the SMs a finishing kernel frees — and the ~15 us every wgrad CTA spends flushing fp32 atomics at its end — are
+  // picked up by the other kernel's CTAs instead of idling until the launch boundary.  dz_L and the forward activations
+  // are never rewritten during the backward (one buffer per layer); train_join orders the side stream before whatever
+  // the caller enqueues next (all-reduce of a finished layer range, optimizer, next step's gradient memset).
+  void* wstream = stream;
+  if (opt("YB_WGRAD_STREAM")[0] != '0') {
+    if (net->side_stream == nullptr) {
+      YB_CUDA(cudaStreamCreateWithFlags(&net->side_stream, cudaStreamNonBlocking));
+      YB_CUDA(cudaEventCreateWithFlags(&net->side_fork, cudaEventDisableTiming));
+      YB_CUDA(cudaEventCreateWithFlags(&net->side_join, cudaEventDisableTiming));
+    }
+    YB_CUDA(cudaEventRecord(net->side_fork, st));
+    YB_CUDA(cudaStreamWaitEvent(net->side_stream, net->side_fork, 0));
+    wstream = net->side_stream;
+    net->side_forked = true;
+  }
+  yb_conv_desc d; memset(&d, 0, sizeof(d));
+  d.n = n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
+  d.ksize = L.info.ksize; d.stride = L.info.stride; d.in_ld = net->bufs[L.in.buf].ld; d.dtype = dt;
+  rc = yb_conv2d_wgrad(&d, ten_ptr2(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), wstream);
+  if (rc) return rc;
+  if (L.dgrad_parity) {
+    for (int c = 0; c < 4; ++c) {
+      rc = conv_launch(dt, L.d4_cout_pad[c], L.d4_tmA[c], L.d4_tmB[c], L.d4_params[c], st);
+      if (rc) return rc;
+    }
+    return YB_OK;
+  }
+  return conv_launch(dt, L.d_cout_pad, L.d_tmA, L.d_tmB, L.dparams, st);
+}
+
+// Position of (layer, phase) in the layered step: forward 0..L-1 (LOCAL, GLOBAL each), the loss, backward L-1..0.
+static int fwd_slot(int layer, int phase) { return 2 * layer + phase; }
+static int loss_slot(const yb_net* net) { return 2 * (int)net->layers.size(); }
+static int bwd_slot(const yb_net* net, int layer, int phase) {
+  return loss_slot(net) + 1 + 2 * ((int)net->layers.size() - 1 - layer) + phase;
+}
+static const char* slot_name(const yb_net* net, int s, char* buf, size_t len) {
+  const int nl = (int)net->layers.size();
+  if (s < 0) snprintf(buf, len, "forward layer 0 LOCAL (no step in progress)");
+  else if (s < loss_slot(net)) snprintf(buf, len, "forward layer %d %s", s / 2, s % 2 ? "GLOBAL" : "LOCAL");
+  else if (s == loss_slot(net)) snprintf(buf, len, "the loss");
+  else if (s < bwd_slot(net, 0, 1) + 1) {
+    const int k = s - loss_slot(net) - 1;
+    snprintf(buf, len, "backward layer %d %s", nl - 1 - k / 2, k % 2 ? "GLOBAL" : "LOCAL");
+  } else snprintf(buf, len, "forward layer 0 LOCAL (the step is complete)");
+  return buf;
+}
+// Host-side order check: a step starts at forward layer 0 LOCAL (always accepted) and every other call must be the
+// next one.  A failed or out-of-order call leaves the step unfinished; starting again at layer 0 recovers.
+static int check_slot(yb_net* net, const char* what, int s, int replicas) {
+  const bool start = s == 0;
+  if (!start && s != net->step_slot) {
+    char want[96], got[96];
+    set_error("%s: out of order: called for %s, expected %s", what, slot_name(net, s, got, sizeof(got)),
+              slot_name(net, net->step_slot, want, sizeof(want)));
+    return YB_ERR_INVALID_ARGUMENT;
+  }
+  if (!start && replicas != net->step_replicas) {
+    set_error("%s: bn_replicas %d differs from the %d this step started with", what, replicas, net->step_replicas);
+    return YB_ERR_INVALID_ARGUMENT;
+  }
+  return YB_OK;
+}
+static int advance(yb_net* net, int s, int replicas, int rc) {
+  net->step_slot = rc == YB_OK ? s + 1 : -1;
+  net->step_replicas = replicas;
+  return rc;
+}
+
+}  // namespace yb
+
 extern "C" int yb_net_train_fwd_bwd(yb_net* net, const float* images, const float* y_true_1, const float* y_true_2,
                                     const float* y_true_3, const float* anchors9x2, int use_label_smooth,
                                     int use_focal_loss, float bn_decay, float loss_scale, float* fm1, float* fm2,
                                     float* fm3, double* loss4, int flags, void* stream) {
   const int forward_only = flags & YB_TRAIN_FORWARD_ONLY;
-  const bool bn_frozen = (flags & YB_TRAIN_BN_FROZEN) != 0;
   YB_REQUIRE(net && net->training && net->act && net->par, "train_fwd_bwd: not a bound training plan");
   YB_REQUIRE(images, "train_fwd_bwd: null images");
   YB_REQUIRE(forward_only || (y_true_1 && y_true_2 && y_true_3 && anchors9x2 && loss4), "train_fwd_bwd: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int n = net->n, dt = net->dtype;
-  const float* ones = fpar(net, net->ones_off);
-  const float* zeros = fpar(net, net->zeros_off);
   float* user_fm[3] = {fm1, fm2, fm3};
   const float* y_true[3] = {y_true_1, y_true_2, y_true_3};
   int rc;
-  YB_CUDA(cudaMemsetAsync(net->act + net->stats_off, 0, net->stats_bytes, st));
-  if (!forward_only) {
-    YB_CUDA(cudaMemsetAsync(net->par + net->grad_off, 0, (size_t)net->grad_count * 4, st));
-    YB_CUDA(cudaMemsetAsync(loss4, 0, 4 * sizeof(double), st));
-  }
+  net->step_slot = -1;
+  if (!forward_only) YB_CUDA(cudaMemsetAsync(loss4, 0, 4 * sizeof(double), st));
   // ------------------------------------------------ forward (is_training=True)
-  float* fm_ptr[3] = {nullptr, nullptr, nullptr};
-  const bool fuse_fin = opt("YB_BN_FIN")[0] != '0';
-  const bool stem_tc = opt("YB_STEM_TRAIN")[0] != 'c';
-  for (size_t i = 0; i < net->layers.size(); ++i) {
-    Layer& L = net->layers[i];
-    const long rows = (long)n * L.info.out_h * L.info.out_w;
-    if (i == 0) {
-      if (stem_tc) {   // warp-level tensor path, batch statistics accumulated by the same kernel (the sums were zeroed above)
-        rc = yb_stem_conv_fwd_tc_stats(images, fpar(net, L.w_master), ones, zeros, n, net->h, net->w, dt, 0,
-                                       net->act + L.z_off, fact(net, L.st_sum), fact(net, L.st_sqsum), stream);
-        if (rc) return rc;
-      } else {         // YB_STEM_TRAIN=cuda: the fp32 CUDA-core stem + a column-statistics pass (the first version)
-        rc = yb_stem_conv_fwd(images, fpar(net, L.w_master), ones, zeros, n, net->h, net->w, L.info.cout, dt, 0,
-                              net->act + L.z_off, stream);
-        if (rc) return rc;
-        rc = yb_col_stats(net->act + L.z_off, L.info.cout, rows, L.info.cout, dt, fact(net, L.st_sum), fact(net, L.st_sqsum), stream);
-        if (rc) return rc;
-      }
-    } else {
-      ConvParams p = L.tparams;
-      if (!L.info.has_bn) {
-        const int which = L.out.buf == net->fm_buf[0] ? 0 : (L.out.buf == net->fm_buf[1] ? 1 : 2);
-        p.out = user_fm[which] ? (void*)user_fm[which] : (void*)(net->act + net->bufs[L.out.buf].offset);
-        fm_ptr[which] = static_cast<float*>(p.out);
-      }
-      rc = conv_launch(dt, L.cout_pad, L.tmA, L.tmB, p, st);
-      if (rc) return rc;
-    }
-    if (L.info.has_bn) {
-      const void* resp = L.res.buf >= 0 ? ten_ptr2(net, L.res) : nullptr;
-      const long res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
-      if (fuse_fin) {     // statistics -> scale/shift inside the apply kernel (one launch per BN layer instead of two)
-        rc = yb_bn_stats_act_apply(net->act + L.z_off, L.info.cout, bn_frozen ? nullptr : fact(net, L.st_sum),
-                                   bn_frozen ? nullptr : fact(net, L.st_sqsum), fpar(net, L.gamma), fpar(net, L.beta),
-                                   net->bn_eps, bn_decay, fpar(net, L.mean), fpar(net, L.var), fact(net, L.st_scale),
-                                   fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), resp, res_ld,
-                                   ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w,
-                                   L.info.cout, dt, 1, L.upsample ? 1 : 0, stream);
-        if (rc) return rc;
-        continue;
-      }
-      rc = yb_bn_finalize(bn_frozen ? nullptr : fact(net, L.st_sum), bn_frozen ? nullptr : fact(net, L.st_sqsum), rows,
-                          L.info.cout, fpar(net, L.gamma), fpar(net, L.beta),
-                          net->bn_eps, bn_decay, fpar(net, L.mean), fpar(net, L.var), fact(net, L.st_scale),
-                          fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), stream);
-      if (rc) return rc;
-      rc = yb_bn_act_apply(net->act + L.z_off, L.info.cout, fact(net, L.st_scale), fact(net, L.st_shift), resp, res_ld,
-                           ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1,
-                           L.upsample ? 1 : 0, stream);
+  for (int i = 0; i < (int)net->layers.size(); ++i) {
+    for (int ph = YB_PHASE_LOCAL; ph <= YB_PHASE_GLOBAL; ++ph) {
+      rc = train_fwd_layer(net, i, ph, images, 1, bn_decay, user_fm, flags, stream);
       if (rc) return rc;
     }
   }
-  if (!bn_frozen) net->fold_dirty = true;
   if (forward_only) return YB_OK;
   // ------------------------------------------------ loss + d(loss)/d(feature maps)
-  for (int s = 0; s < 3; ++s) {
-    const int div = 32 >> s;
-    rc = yb_loss_layer(fm_ptr[s], y_true[s], n, net->h / div, net->w / div, net->h, net->w, net->class_num,
-                       anchors9x2 + 2 * 3 * (2 - s), use_label_smooth, use_focal_loss, 1.0f / (float)n, loss_scale,
-                       net->act + net->lossws_off, net->lossws_bytes, loss4, net->act + net->dfm_off[s], dt,
-                       (3 * (5 + net->class_num) + 31) / 32 * 32, stream);
-    if (rc) return rc;
-  }
+  rc = train_loss(net, y_true, anchors9x2, use_label_smooth, use_focal_loss, loss_scale, loss4, stream);
+  if (rc) return rc;
   if (flags & YB_TRAIN_NO_BACKWARD) return YB_OK;
   return yb_net_train_backward(net, images, 0, (int)net->layers.size() - 1, flags, stream);
 }
@@ -380,78 +544,67 @@ extern "C" int yb_net_train_backward(yb_net* net, const float* images, int first
                                      void* stream) {
   YB_REQUIRE(net && net->training && net->act && net->par && images, "train_backward: not a bound training plan");
   YB_REQUIRE(first_layer >= 0 && first_layer <= last_layer && last_layer < (int)net->layers.size(), "train_backward: bad layer range");
-  const bool bn_frozen = (flags & YB_TRAIN_BN_FROZEN) != 0;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int n = net->n, dt = net->dtype;
-  const float* zeros = fpar(net, net->zeros_off);
-  int rc;
-  // Layer L's weight gradient and input gradient both only read dz_L: the wgrad goes to a side stream and runs beside
-  // the dgrad (and the next layer's BN backward).  Both kernels own a whole SM per CTA, so the gain is in the tails:
-  // the SMs a finishing kernel frees — and the ~15 us every wgrad CTA spends flushing fp32 atomics at its end — are
-  // picked up by the other kernel's CTAs instead of idling until the launch boundary.  dz_L and the forward activations
-  // are never rewritten during the backward (one buffer per layer), the join below orders the side stream before
-  // whatever the caller enqueues next (all-reduce of this layer range, optimizer, next step's gradient memset).
-  const bool overlap = opt("YB_WGRAD_STREAM")[0] != '0';
-  bool forked = false;
-  if (overlap && net->side_stream == nullptr) {
-    YB_CUDA(cudaStreamCreateWithFlags(&net->side_stream, cudaStreamNonBlocking));
-    YB_CUDA(cudaEventCreateWithFlags(&net->side_fork, cudaEventDisableTiming));
-    YB_CUDA(cudaEventCreateWithFlags(&net->side_join, cudaEventDisableTiming));
-  }
+  net->step_slot = -1;
   for (int i = last_layer; i >= first_layer; --i) {
-    Layer& L = net->layers[i];
-    const long rows = (long)n * L.info.out_h * L.info.out_w;
-    if (L.info.has_bn) {
-      float* dgamma = gradp(net, L.g_gamma);
-      float* dbeta = gradp(net, L.g_beta);
-      const void* dA = gten_ptr(net, L.out);
-      const long dA_ld = net->bufs[L.out.buf].ld;
-      rc = yb_bn_bwd_reduce(dA, dA_ld, net->act + L.z_off, L.info.cout, fact(net, L.st_scale), fact(net, L.st_shift),
-                            fact(net, L.st_mean), fact(net, L.st_invstd), n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1,
-                            L.upsample ? 1 : 0, dgamma, dbeta, net->act + net->bnws_off, stream);
-      if (rc) return rc;
-      // frozen BN: mean / variance are constants -> dz = gamma * invstd * dact (the batch-statistic terms vanish)
-      rc = yb_bn_bwd_apply(dA, dA_ld, net->act + L.z_off, L.info.cout, fpar(net, L.gamma), fact(net, L.st_scale),
-                           fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), bn_frozen ? zeros : dgamma,
-                           bn_frozen ? zeros : dbeta, n,
-                           L.info.out_h, L.info.out_w, L.info.cout, dt, 1, L.upsample ? 1 : 0, L.dz_dilated,
-                           net->act + L.dz_off, L.dz_ld, stream);
-      if (rc) return rc;
-    } else {
-      rc = yb_col_sum(net->act + L.dz_off, L.dz_ld, rows, L.info.cout, dt, gradp(net, L.g_bias), stream);
-      if (rc) return rc;
-    }
-    if (i == 0) {
-      rc = yb_stem_conv_wgrad(images, net->act + L.dz_off, dt, n, net->h, net->w, gradp(net, L.g_w), stream);
-      if (rc) return rc;
-      break;
-    }
-    yb_conv_desc d; memset(&d, 0, sizeof(d));
-    d.n = n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
-    d.ksize = L.info.ksize; d.stride = L.info.stride; d.in_ld = net->bufs[L.in.buf].ld; d.dtype = dt;
-    void* wstream = stream;
-    if (overlap) {
-      YB_CUDA(cudaEventRecord(net->side_fork, st));
-      YB_CUDA(cudaStreamWaitEvent(net->side_stream, net->side_fork, 0));
-      wstream = net->side_stream;
-      forked = true;
-    }
-    rc = yb_conv2d_wgrad(&d, ten_ptr2(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), wstream);
-    if (rc) return rc;
-    if (L.dgrad_parity) {
-      for (int c = 0; c < 4; ++c) {
-        rc = conv_launch(dt, L.d4_cout_pad[c], L.d4_tmA[c], L.d4_tmB[c], L.d4_params[c], st);
-        if (rc) return rc;
-      }
-    } else {
-      rc = conv_launch(dt, L.d_cout_pad, L.d_tmA, L.d_tmB, L.dparams, st);
+    for (int ph = YB_PHASE_LOCAL; ph <= YB_PHASE_GLOBAL; ++ph) {
+      int rc = train_bwd_layer(net, i, ph, images, 1, false, flags, stream);
       if (rc) return rc;
     }
   }
-  if (forked) {
-    YB_CUDA(cudaEventRecord(net->side_join, net->side_stream));
-    YB_CUDA(cudaStreamWaitEvent(st, net->side_join, 0));
-  }
+  return train_join(net, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int yb_net_train_forward_layer(yb_net* net, const float* images, int layer, int phase, int bn_replicas,
+                                          float bn_decay, float* fm1, float* fm2, float* fm3, int flags, void* stream) {
+  YB_REQUIRE(net && net->training && net->act && net->par && images, "train_forward_layer: not a bound training plan");
+  YB_REQUIRE(layer >= 0 && layer < (int)net->layers.size() && (phase == YB_PHASE_LOCAL || phase == YB_PHASE_GLOBAL),
+             "train_forward_layer: bad layer or phase");
+  YB_REQUIRE(bn_replicas >= 1, "train_forward_layer: bn_replicas must be >= 1");
+  const int s = fwd_slot(layer, phase);
+  int rc = check_slot(net, "train_forward_layer", s, bn_replicas);
+  if (rc) return rc;
+  float* user_fm[3] = {fm1, fm2, fm3};
+  return advance(net, s, bn_replicas, train_fwd_layer(net, layer, phase, images, bn_replicas, bn_decay, user_fm, flags, stream));
+}
+
+extern "C" int yb_net_train_loss(yb_net* net, const float* y_true_1, const float* y_true_2, const float* y_true_3,
+                                 const float* anchors9x2, int use_label_smooth, int use_focal_loss, float loss_scale,
+                                 double* loss4, void* stream) {
+  YB_REQUIRE(net && net->training && net->act && net->par, "train_loss: not a bound training plan");
+  YB_REQUIRE(y_true_1 && y_true_2 && y_true_3 && anchors9x2 && loss4, "train_loss: null pointer");
+  const int s = loss_slot(net);
+  int rc = check_slot(net, "train_loss", s, net->step_replicas);
+  if (rc) return rc;
+  YB_CUDA(cudaMemsetAsync(loss4, 0, 4 * sizeof(double), static_cast<cudaStream_t>(stream)));
+  const float* y_true[3] = {y_true_1, y_true_2, y_true_3};
+  return advance(net, s, net->step_replicas,
+                 train_loss(net, y_true, anchors9x2, use_label_smooth, use_focal_loss, loss_scale, loss4, stream));
+}
+
+extern "C" int yb_net_train_backward_layer(yb_net* net, const float* images, int layer, int phase, int bn_replicas,
+                                           int flags, void* stream) {
+  YB_REQUIRE(net && net->training && net->act && net->par && images, "train_backward_layer: not a bound training plan");
+  YB_REQUIRE(layer >= 0 && layer < (int)net->layers.size() && (phase == YB_PHASE_LOCAL || phase == YB_PHASE_GLOBAL),
+             "train_backward_layer: bad layer or phase");
+  YB_REQUIRE(bn_replicas >= 1, "train_backward_layer: bn_replicas must be >= 1");
+  const int s = bwd_slot(net, layer, phase);
+  int rc = check_slot(net, "train_backward_layer", s, bn_replicas);
+  if (rc) return rc;
+  return advance(net, s, bn_replicas, train_bwd_layer(net, layer, phase, images, bn_replicas, true, flags, stream));
+}
+
+extern "C" int yb_net_train_join(yb_net* net, void* stream) {
+  YB_REQUIRE(net && net->training, "train_join: not a training plan");
+  return train_join(net, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int yb_net_bn_exchange_buffer(yb_net* net, int layer, int backward, float** ptr, size_t* count) {
+  YB_REQUIRE(net && net->training && net->act && ptr && count && layer >= 0 && layer < (int)net->layers.size(),
+             "bn_exchange_buffer: bad argument");
+  const Layer& L = net->layers[layer];
+  YB_REQUIRE(L.info.has_bn, "bn_exchange_buffer: layer %d has no batch norm", layer);
+  *ptr = fact(net, backward ? L.x_bwd : L.st_sum);   // forward: st_sum and st_sqsum are adjacent
+  *count = 2 * (size_t)L.cout_pad;
   return YB_OK;
 }
 

@@ -121,6 +121,15 @@ class _Plan:
         check(lib.yb_net_grad_range(self.handle, int(first_layer), int(last_layer), C.byref(p), C.byref(n)), "yb_net_grad_range")
         return self._view(p.value, (n.value,))
 
+    def bn_exchange_buffer(self, i, backward):
+        """Layer i's sync-BN exchange slab (float32 [2 * cout_pad], activation arena): forward [Σz | Σz²], backward
+        [Σdact·ẑ | Σdact]."""
+        p, n = C.c_void_p(), C.c_size_t()
+        check(lib.yb_net_bn_exchange_buffer(self.handle, int(i), int(bool(backward)), C.byref(p), C.byref(n)),
+              "yb_net_bn_exchange_buffer")
+        off = p.value - self.act.data_ptr()
+        return self.act[off: off + n.value * 4].view(torch.float32)
+
     def grad_flat(self):
         p, n = C.c_void_p(), C.c_size_t()
         check(lib.yb_net_grad_buffer(self.handle, C.byref(p), C.byref(n)), "yb_net_grad_buffer")
@@ -587,27 +596,9 @@ class yolov3(object):
         coff = ctrl.value - self._arena.data_ptr()
         return slots, self._arena[coff: coff + 12].view(torch.int32)
 
-    def train_step(self, images, y_true, learning_rate, momentum=0.9, clip_norm=100.0, process_group=None,
-                   return_feature_maps=False, data_parallel=True, optimizer="momentum", decay=0.9, beta1=0.9,
-                   beta2=0.999, epsilon=None, freeze_bn=False, bucket_mb=32.0):
-        """One training step of the reference (train.py:105-115): forward(is_training=True) -> compute_loss ->
-        gradients of (loss[0] + l2_loss) w.r.t. the trainable tensors (all 222 unless set_trainable() restricted them,
-        train.py:81) -> per-tensor clip_by_norm(clip_norm) -> optimizer update; BN moving statistics updated with
-        self.batch_norm_decay.
-
-        images float32 [N,H,W,3]; y_true = (y_true_13, y_true_26, y_true_52) in process_box format.
-        learning_rate: this step's value (utils.misc_utils.config_learning_rate / learning_rate_at evaluate the
-        reference's schedules on the host).  optimizer: 'momentum' (default), 'sgd', 'rmsprop', 'adam' or the object
-        returned by utils.misc_utils.config_optimizer (utils/misc_utils.py:151-161; TF1 update rules).
-        freeze_bn: BN layers normalise with their moving statistics and keep them (the graph the reference builds with
-        is_training=False, train.py:72): fine-tuning with frozen BN.
-        Data parallel: when torch.distributed is initialised (or process_group is given) the flat gradient is
-        all-reduced (NCCL over NVLink) and averaged over the ranks before the update; every loss term is a
-        mean over the local batch (model.py:276-302), so this equals one big batch of world*N images.  The gradient
-        is reduced in buckets of ~bucket_mb MB, detection heads first, each all-reduce overlapping the backward of
-        the layers below it (bucket_mb <= 0: one blocking all-reduce after the whole backward).
-        Returns [total, xy, wh, conf, class] as 0-dim float32 CUDA tensors of the LOCAL batch."""
-        import torch.distributed as dist
+    def _train_setup(self, images, y_true, learning_rate, momentum, clip_norm, optimizer, decay, beta1, beta2, epsilon,
+                     return_feature_maps):
+        """Checks and state shared by the training-step entry points -> (x, ys, plan, opt without grad_scale, fms)."""
         x = _as_cuda_f32(images, self.device)
         ys = [_as_cuda_f32(y, self.device) for y in y_true]
         n, h, w = int(x.shape[0]), int(x.shape[1]), int(x.shape[2])
@@ -643,9 +634,68 @@ class yolov3(object):
         fms = [None, None, None]
         if return_feature_maps:
             fms = [torch.empty((n, h // s, w // s, 3 * (5 + C_)), dtype=torch.float32, device=self.device) for s in (32, 16, 8)]
-        from .parallel import allreduce_gradients, gradient_buckets, BucketedAllReduce
+        opt = _lib.Optimizer(kind=kind, lr=float(learning_rate), grad_scale=0.0, momentum=float(momentum),
+                             decay=float(decay), beta1=float(beta1), beta2=float(beta2), epsilon=float(epsilon),
+                             weight_decay=float(self.weight_decay), clip_norm=float(clip_norm))
+        return x, ys, plan, opt, fms
+
+    @staticmethod
+    def _grad_buckets(plan, bucket_mb):
+        from .parallel import gradient_buckets
+        if not hasattr(plan, "_buckets") or plan._bucket_mb != bucket_mb:
+            sizes = [plan.grad_range(i, i).numel() for i in range(plan.num_layers)]
+            plan._buckets = gradient_buckets(sizes, int(bucket_mb * (1 << 20) / 4))
+            plan._bucket_mb = bucket_mb
+        return plan._buckets
+
+    def _finish_step(self, plan, opt, grad_scale, fms, return_feature_maps):
+        st = stream_handle()
+        opt.grad_scale = grad_scale
+        check(lib.yb_net_train_update(plan.handle, C.byref(opt), st), "yb_net_train_update")
+        self._fold_dirty = True
+        self._last_plan = plan
+        out = torch.empty(5, dtype=torch.float32, device=self.device)
+        check(lib.yb_loss_finalize(ptr(plan.loss4), ptr(out), st), "yb_loss_finalize")
+        losses = [out[0], out[1], out[2], out[3], out[4]]
+        return (losses, fms) if return_feature_maps else losses
+
+    def train_step(self, images, y_true, learning_rate, momentum=0.9, clip_norm=100.0, process_group=None,
+                   return_feature_maps=False, data_parallel=True, optimizer="momentum", decay=0.9, beta1=0.9,
+                   beta2=0.999, epsilon=None, freeze_bn=False, bucket_mb=32.0, sync_bn=False):
+        """One training step of the reference (train.py:105-115): forward(is_training=True) -> compute_loss ->
+        gradients of (loss[0] + l2_loss) w.r.t. the trainable tensors (all 222 unless set_trainable() restricted them,
+        train.py:81) -> per-tensor clip_by_norm(clip_norm) -> optimizer update; BN moving statistics updated with
+        self.batch_norm_decay.
+
+        images float32 [N,H,W,3]; y_true = (y_true_13, y_true_26, y_true_52) in process_box format.
+        learning_rate: this step's value (utils.misc_utils.config_learning_rate / learning_rate_at evaluate the
+        reference's schedules on the host).  optimizer: 'momentum' (default), 'sgd', 'rmsprop', 'adam' or the object
+        returned by utils.misc_utils.config_optimizer (utils/misc_utils.py:151-161; TF1 update rules).
+        freeze_bn: BN layers normalise with their moving statistics and keep them (the graph the reference builds with
+        is_training=False, train.py:72): fine-tuning with frozen BN.
+        Data parallel: when torch.distributed is initialised (or process_group is given) the flat gradient is
+        all-reduced (NCCL over NVLink) and averaged over the ranks before the update; every loss term is a
+        mean over the local batch (model.py:276-302), so this equals one big batch of world*N images.  The gradient
+        is reduced in buckets of ~bucket_mb MB, detection heads first, each all-reduce overlapping the backward of
+        the layers below it (bucket_mb <= 0: one blocking all-reduce after the whole backward).
+        sync_bn: synchronised batch norm across the ranks.  Training-mode BN then normalises with the statistics of
+        the global batch and back-propagates through them, so the step equals the single-device step on the
+        concatenated batch (up to fp32 summation order) and every rank holds the same moving statistics.  Every rank
+        must run the same N, H and W.  Runs train_step_sync_bn() over NCCL; with one rank it is the ordinary step.
+        Returns [total, xy, wh, conf, class] as 0-dim float32 CUDA tensors of the LOCAL batch."""
+        import torch.distributed as dist
+        if sync_bn and freeze_bn:
+            raise ValueError("sync_bn=True needs training-mode BN: frozen BN (freeze_bn=True) has no batch statistics to synchronise")
+        from .parallel import allreduce_gradients, BucketedAllReduce
         use_dp = data_parallel and (process_group is not None or (dist.is_available() and dist.is_initialized()))
         use_dp = use_dp and dist.get_world_size(process_group) > 1
+        if sync_bn and use_dp:
+            gen = self.train_step_sync_bn(images, y_true, learning_rate, dist.get_world_size(process_group), momentum,
+                                          clip_norm, return_feature_maps, optimizer, decay, beta1, beta2, epsilon, bucket_mb)
+            return _drive_sync_bn(gen, process_group)
+        x, ys, plan, opt, fms = self._train_setup(images, y_true, learning_rate, momentum, clip_norm, optimizer, decay,
+                                                  beta1, beta2, epsilon, return_feature_maps)
+        st = stream_handle()
         flags = _lib.YB_TRAIN_BN_FROZEN if freeze_bn else 0
         bucketed = use_dp and bucket_mb and bucket_mb > 0
         check(lib.yb_net_train_fwd_bwd(plan.handle, ptr(x), ptr(ys[0]), ptr(ys[1]), ptr(ys[2]),
@@ -656,24 +706,80 @@ class yolov3(object):
         grad_scale = 1.0 / float(self.loss_scale)
         if bucketed:
             # backward bucket by bucket (heads first); each bucket's all-reduce overlaps the next bucket's backward
-            if not hasattr(plan, "_buckets") or plan._bucket_mb != bucket_mb:
-                sizes = [plan.grad_range(i, i).numel() for i in range(plan.num_layers)]
-                plan._buckets = gradient_buckets(sizes, int(bucket_mb * (1 << 20) / 4))
-                plan._bucket_mb = bucket_mb
             red = BucketedAllReduce(process_group)
-            for lo, hi in plan._buckets:
+            for lo, hi in self._grad_buckets(plan, bucket_mb):
                 check(lib.yb_net_train_backward(plan.handle, ptr(x), lo, hi, flags, st), "yb_net_train_backward")
                 red.reduce(plan.grad_range(lo, hi))
             grad_scale *= red.wait()
         elif use_dp:
             grad_scale *= allreduce_gradients(plan.grad_flat(), process_group)   # NCCL all-reduce (sum) -> 1/world
-        opt = _lib.Optimizer(kind=kind, lr=float(learning_rate), grad_scale=grad_scale, momentum=float(momentum),
-                             decay=float(decay), beta1=float(beta1), beta2=float(beta2), epsilon=float(epsilon),
-                             weight_decay=float(self.weight_decay), clip_norm=float(clip_norm))
-        check(lib.yb_net_train_update(plan.handle, C.byref(opt), st), "yb_net_train_update")
-        self._fold_dirty = True
-        self._last_plan = plan
-        out = torch.empty(5, dtype=torch.float32, device=self.device)
-        check(lib.yb_loss_finalize(ptr(plan.loss4), ptr(out), st), "yb_loss_finalize")
-        losses = [out[0], out[1], out[2], out[3], out[4]]
-        return (losses, fms) if return_feature_maps else losses
+        return self._finish_step(plan, opt, grad_scale, fms, return_feature_maps)
+
+    def train_step_sync_bn(self, images, y_true, learning_rate, bn_replicas, momentum=0.9, clip_norm=100.0,
+                           return_feature_maps=False, optimizer="momentum", decay=0.9, beta1=0.9, beta2=0.999,
+                           epsilon=None, bucket_mb=32.0):
+        """train_step(sync_bn=True) as a generator that leaves the transport to its caller.
+
+        The step runs layer by layer (include/yolob200.h: yb_net_train_forward_layer).  At every exchange point it
+        yields (kind, tensor), and the caller sums the tensor in place across the bn_replicas ranks:
+          ("bn", slab)        a BN layer's forward [Σz | Σz²] or backward [Σdact·ẑ | Σdact] sums; the next layer
+                              call consumes the sum, so it is on the critical path;
+          ("grad", slice)     a finished gradient bucket (heads first; the whole flat gradient when bucket_mb <= 0);
+          ("grad_scale", None) after the last bucket: send back the factor that turns the summed gradient into the
+                              mean (1/world), which the optimizer folds in.
+        Then the update and the loss finalize run as in train_step, and the generator returns what train_step
+        returns.  Every rank must run the same number of images and the same H x W."""
+        bn_replicas = int(bn_replicas)
+        if bn_replicas < 1:
+            raise ValueError(f"bn_replicas must be >= 1, got {bn_replicas}")
+        x, ys, plan, opt, fms = self._train_setup(images, y_true, learning_rate, momentum, clip_norm, optimizer, decay,
+                                                  beta1, beta2, epsilon, return_feature_maps)
+        st = stream_handle()
+        h, L = plan.handle, plan.num_layers
+        has_bn = [bool(plan.layer_info(i).has_bn) for i in range(L)]
+        decay_bn = float(self.batch_norm_decay)
+        for i in range(L):
+            check(lib.yb_net_train_forward_layer(h, ptr(x), i, _lib.YB_PHASE_LOCAL, bn_replicas, decay_bn, ptr(fms[0]),
+                                                 ptr(fms[1]), ptr(fms[2]), 0, st), "yb_net_train_forward_layer")
+            if has_bn[i]:
+                yield "bn", plan.bn_exchange_buffer(i, backward=False)
+            check(lib.yb_net_train_forward_layer(h, ptr(x), i, _lib.YB_PHASE_GLOBAL, bn_replicas, decay_bn, ptr(fms[0]),
+                                                 ptr(fms[1]), ptr(fms[2]), 0, st), "yb_net_train_forward_layer")
+        check(lib.yb_net_train_loss(h, ptr(ys[0]), ptr(ys[1]), ptr(ys[2]), _lib.fptr(self.anchors.reshape(-1)),
+                                    int(self.use_label_smooth), int(self.use_focal_loss), float(self.loss_scale),
+                                    ptr(plan.loss4), st), "yb_net_train_loss")
+        bucketed = bucket_mb and bucket_mb > 0
+        for lo, hi in (self._grad_buckets(plan, bucket_mb) if bucketed else [(0, L - 1)]):
+            for i in range(hi, lo - 1, -1):
+                check(lib.yb_net_train_backward_layer(h, ptr(x), i, _lib.YB_PHASE_LOCAL, bn_replicas, 0, st),
+                      "yb_net_train_backward_layer")
+                if has_bn[i]:
+                    yield "bn", plan.bn_exchange_buffer(i, backward=True)
+                check(lib.yb_net_train_backward_layer(h, ptr(x), i, _lib.YB_PHASE_GLOBAL, bn_replicas, 0, st),
+                      "yb_net_train_backward_layer")
+            check(lib.yb_net_train_join(h, st), "yb_net_train_join")
+            yield "grad", (plan.grad_range(lo, hi) if bucketed else plan.grad_flat())
+        factor = yield "grad_scale", None
+        return self._finish_step(plan, opt, float(factor) / float(self.loss_scale), fms, return_feature_maps)
+
+
+def _drive_sync_bn(gen, group):
+    """Run a train_step_sync_bn generator over torch.distributed: BN slabs are summed on their own communicator
+    (parallel.sync_bn_group), gradient buckets by BucketedAllReduce on `group`."""
+    import torch.distributed as dist
+    from .parallel import BucketedAllReduce, sync_bn_group
+    bn_group = sync_bn_group(group)
+    red = BucketedAllReduce(group)
+    reply = None
+    try:
+        while True:
+            kind, t = gen.send(reply)
+            reply = None
+            if kind == "bn":
+                dist.all_reduce(t, op=dist.ReduceOp.SUM, group=bn_group)
+            elif kind == "grad":
+                red.reduce(t)
+            else:
+                reply = red.wait()
+    except StopIteration as done:
+        return done.value

@@ -3,8 +3,14 @@ all-reduce of the flat gradient buffer per training step (NCCL over NVLink on GP
 runs over gloo on CPU tensors for the tests).  The reference has no multi-GPU support
 (README.md:140,210) — this is new functionality whose contract is "same math as one big batch":
 every loss term is a mean over the local batch (model.py:276-302), so averaging the per-rank
-gradients equals the single-device gradient of the concatenated batch (BN statistics stay per
-rank, as in standard DP; the reference has no sync-BN either)."""
+gradients equals the single-device gradient of the concatenated batch when BN is frozen.
+
+In BN training mode the statistics stay per rank by default, as in standard DP: each shard is normalised with its
+own batch statistics and each rank keeps its own moving statistics.  train_step(sync_bn=True) synchronises them
+(the reference lists "multi-GPUs with sync batch norm" as a TODO): every BN layer's per-channel sums Σz / Σz² in
+the forward and Σdact·ẑ / Σdact in the backward are all-reduced between the kernel that produces them and the
+kernel that consumes them, on a communicator of their own (sync_bn_group).  The step then equals the single-device
+step on the concatenated batch up to fp32 summation order, and every rank holds the same moving statistics."""
 from __future__ import annotations
 
 import os
@@ -59,6 +65,27 @@ def gradient_buckets(layer_floats, bucket_floats):
             out.append((i, hi))
             hi, acc = i - 1, 0
     return out
+
+
+_SYNC_BN_GROUPS = {}
+
+
+def sync_bn_group(group=None):
+    """A second process group over the ranks of `group` (None: the default group) for the synchronised-BN exchanges,
+    created on first use and cached by its rank list.  Those all-reduces are small (<= 8 KB, 2 x 72 per step) and each
+    one blocks the next layer, so they get their own NCCL communicator and stream instead of queueing behind the 32 MB
+    gradient buckets on `group`.  NCCL requires every rank to issue the collectives of both groups in the same
+    program order: train_step_sync_bn's fixed sequence of yields guarantees it.
+    torch.distributed.new_group is collective over the default group, so only a group spanning every rank is
+    supported: with a proper subgroup the ranks outside it would never make the call."""
+    base = group if group is not None else dist.group.WORLD
+    ranks = tuple(dist.get_process_group_ranks(base))
+    if len(ranks) != dist.get_world_size():
+        raise ValueError(f"sync_bn needs a process group over all {dist.get_world_size()} ranks, got ranks {list(ranks)}")
+    g = _SYNC_BN_GROUPS.get(ranks)
+    if g is None:
+        g = _SYNC_BN_GROUPS[ranks] = dist.new_group(list(ranks))
+    return g
 
 
 class BucketedAllReduce:
