@@ -34,7 +34,8 @@ typedef enum yb_status {
   YB_ERR_WORKSPACE = -4
 } yb_status;
 
-typedef enum yb_dtype { YB_F16 = 0, YB_BF16 = 1, YB_F32 = 2 } yb_dtype;
+/* YB_E4M3: fp8 e4m3 (OCP "fn": finite, max 448) with float32 scales, for the calibrated inference plan only */
+typedef enum yb_dtype { YB_F16 = 0, YB_BF16 = 1, YB_F32 = 2, YB_E4M3 = 3 } yb_dtype;
 
 /* layout of a conv weight tensor handed to the packer */
 typedef enum yb_wlayout {
@@ -89,6 +90,14 @@ int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, co
                   const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,
                   void* stream);
 int yb_conv_cout_pad(int cout);
+/* e4m3 form of yb_conv2d_fwd (d->dtype = YB_E4M3; the fp8 inference plan's convs): x, w_packed and res hold e4m3 codes,
+ * value = code x scale.  scale[co] must already carry (BN scale) x (input scale) x (weight scale of channel co);
+ * out = e4m3 codes of value / out_scale (RN, saturating to +-448), or float32 values when d->out_fp32.  The residual
+ * is added as code x res_scale after the activation.  cin % 64 == 0 and in_ld, out_ld, res_ld multiples of 16; no
+ * statistics.  Runs the ping-pong and cooperative schedules (YB_CONV_PP, YB_CONV_CTAS apply); YB_CONV_EG=1,
+ * YB_CONV_MODE=2cta and YB_CONV_EPI=reg return YB_ERR_INVALID_ARGUMENT. */
+int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
+                       const float* shift, const void* res, float res_scale, void* out, float out_scale, void* stream);
 /* Host-only: the implicit-GEMM kernel and persistent grid yb_conv2d_fwd would launch for `d` with the current options
  * (yb_set_option: YB_CONV_EG, YB_CONV_MODE, YB_CONV_EPI, YB_CONV_PP, YB_CONV_CTAS) on a device with sm_count SMs.
  * kh = kw = 0: the forward ksize x ksize window; kh, kw in {1, 2}: one parity class of yb_conv2d_dgrad_s2 (d = its
@@ -163,6 +172,14 @@ int yb_letterbox_normalize(const uint8_t* bgr, int src_h, int src_w, long src_pi
  * src float32 in `layout` -> dst `dtype` (or float32) OHWI [cout_pad,k,k,cin], rows >= cout zeroed. */
 int yb_pack_conv_weights(const float* src, int layout, int cout, int cin, int ksize, int cout_pad, int dtype,
                          void* dst, void* stream);
+/* Same repack to e4m3 with per-output-channel scales: w_scale[co] (float32 [cout_pad]) = max_k |w[co, k]| / 448 and
+ * dst[co, k] = RN-satfinite e4m3(w[co, k] / w_scale[co]); rows whose max is 0 (and the padding rows >= cout) get
+ * scale 1 and zero codes. */
+int yb_pack_conv_weights_e4m3(const float* src, int layout, int cout, int cin, int ksize, int cout_pad, void* dst,
+                              float* w_scale, void* stream);
+/* out (device float[1], overwritten) = max |x| over the strided [rows, cols] matrix x (row pitch ld elements, dtype
+ * f16 / bf16 / f32): the calibration statistic of the fp8 plan.  Exact, hence bit-reproducible. */
+int yb_amax(const void* x, long ld, long rows, int cols, int dtype, float* out, void* stream);
 /* BN inference fold (model.py:35-41, eps=1e-5): scale = gamma/sqrt(var+eps), shift = beta - mean*scale. */
 int yb_bn_fold(const float* gamma, const float* beta, const float* mean, const float* var, int c, float eps,
                float* scale, float* shift, void* stream);
@@ -454,6 +471,17 @@ int yb_net_layer_grad(yb_net* net, int layer, float** dw, float** dgamma, float*
 int yb_net_train_buffer(yb_net* net, int layer, int which, void** ptr, int* ld, int* h, int* w);
 /* device pointer + geometry of one layer's output activation (tests / debugging). */
 int yb_net_layer_output(const yb_net* net, int layer, void** ptr, int* ld, int* dtype);
+/* ---- calibrated fp8 inference plan: yb_net_create(..., YB_E4M3, training = 0) ----
+ * Layers 0-3 (the stem, Conv_1, Conv_2, Conv_3) compute in fp16; Conv_3's output and every later non-head activation
+ * buffer is e4m3 with one float32 scale per buffer; the heads write float32.  Weights of layers >= 4 are e4m3 with
+ * per-output-channel scales (yb_pack_conv_weights_e4m3, applied by yb_net_set_conv_params), and the folded scale of
+ * each such layer is (BN scale) x (input buffer scale) x (weight scale).  yb_net_set_fp8_amax takes one amax per layer
+ * (host float[num_layers], e.g. yb_amax of the layer outputs of an fp16 plan over calibration images; entries of layers
+ * whose output is not e4m3 are ignored): a buffer's scale is max(amax of the layers writing it) / 448 (1 if that is 0),
+ * and the plan refolds.  Until it is called, forward / detect on the plan fail.  yb_net_fp8_layer_scales: the input,
+ * residual and output buffer scales of one layer (host float[3]) and its device weight scales (NULL for layers 0-3). */
+int yb_net_set_fp8_amax(yb_net* net, const float* amax, int count, void* stream);
+int yb_net_fp8_layer_scales(const yb_net* net, int layer, float* in_res_out, float** w_scale);
 /* number of kernels one yb_net_forward enqueues (for bench.py's gpu_launches). */
 int yb_net_forward_launches(const yb_net* net);
 

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libyolob200.so")
 
-YB_F16, YB_BF16, YB_F32 = 0, 1, 2
+YB_F16, YB_BF16, YB_F32, YB_E4M3 = 0, 1, 2, 3
 YB_W_HWIO, YB_W_OIHW, YB_W_OHWI = 0, 1, 2
 YB_OPT_SGD, YB_OPT_MOMENTUM, YB_OPT_RMSPROP, YB_OPT_ADAM = 0, 1, 2, 3
 YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
@@ -59,6 +59,7 @@ _SIGS = {
     "yb_get_option": ([C.c_char_p], C.c_char_p),
     "yb_device_info": ([C.POINTER(i32)] * 3, i32),
     "yb_conv2d_fwd": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp], i32),
+    "yb_conv2d_fwd_e4m3": ([C.POINTER(ConvDesc), vp, vp, vp, vp, vp, f32, vp, f32, vp], i32),
     "yb_conv_cout_pad": ([i32], i32),
     "yb_conv_schedule": ([C.POINTER(ConvDesc), i32, i32, i32, i32, C.POINTER(ConvSchedule)], i32),
     "yb_stem_conv_fwd": ([vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
@@ -72,6 +73,8 @@ _SIGS = {
     "yb_letterbox_params": ([i32, i32, i32, i32, C.POINTER(C.c_double), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
     "yb_letterbox_normalize": ([vp, i32, i32, C.c_long, i32, i32, vp, vp], i32),
     "yb_pack_conv_weights": ([vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
+    "yb_pack_conv_weights_e4m3": ([vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
+    "yb_amax": ([vp, C.c_long, C.c_long, i32, i32, vp, vp], i32),
     "yb_bn_fold": ([vp, vp, vp, vp, i32, f32, vp, vp, vp], i32),
     "yb_conv2d_wgrad": ([C.POINTER(ConvDesc), vp, vp, i32, i32, vp, vp], i32),
     "yb_stem_conv_wgrad": ([vp, vp, i32, i32, i32, i32, vp, vp], i32),
@@ -129,6 +132,8 @@ _SIGS = {
     "yb_net_layer_grad": ([vp, i32] + [C.POINTER(vp)] * 4, i32),
     "yb_net_train_buffer": ([vp, i32, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
     "yb_net_layer_output": ([vp, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(i32)], i32),
+    "yb_net_set_fp8_amax": ([vp, C.POINTER(f32), i32, vp], i32),
+    "yb_net_fp8_layer_scales": ([vp, i32, C.POINTER(f32), C.POINTER(vp)], i32),
     "yb_net_forward_launches": ([vp], i32),
 }
 for _name, (_args, _ret) in _SIGS.items():

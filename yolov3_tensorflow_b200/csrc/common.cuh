@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -65,6 +66,34 @@ template <> struct Pack2<__nv_bfloat16> {
 };
 
 __device__ __forceinline__ float leaky01(float v) { return v > 0.f ? v : 0.1f * v; }
+
+// e4m3 storage (the fp8 inference plan): cvt.rn.satfinite rounds to nearest even and saturates to +-448.
+// a -> the low byte (the lower address), b -> the high byte.
+__device__ __forceinline__ uint32_t e4m3x2_pack(float a, float b) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
+  return r;
+}
+// 16 values times `mul` -> 16 e4m3 codes in memory order
+__device__ __forceinline__ uint4 e4m3x16_pack(const float (&v)[16], float mul) {
+  uint32_t w[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    w[j] = e4m3x2_pack(v[4 * j] * mul, v[4 * j + 1] * mul) | (e4m3x2_pack(v[4 * j + 2] * mul, v[4 * j + 3] * mul) << 16);
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+// v[j] += code_j * scale for the 16 e4m3 codes of u (the e4m3 -> f16 conversion is exact)
+__device__ __forceinline__ void e4m3x16_unpack_fma(const uint4 u, float scale, float (&v)[16]) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    uint32_t h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"((uint16_t)(w[j >> 1] >> (16 * (j & 1)))));
+    const float2 f = __half22float2(*reinterpret_cast<__half2*>(&h2));
+    v[2 * j] = fmaf(f.x, scale, v[2 * j]);
+    v[2 * j + 1] = fmaf(f.y, scale, v[2 * j + 1]);
+  }
+}
 
 #ifdef __CUDACC__
 // ----------------------------------------------------------------------------------

@@ -29,6 +29,8 @@ struct ConvParams {
   float* stat_sum;        // nullable: BN batch statistics of the raw conv result
   float* stat_sqsum;
   DetParams det;          // det.on: decode + NMS candidate filter instead of the fp32 feature-map store (detection heads)
+  // e4m3 only (1 otherwise): the residual buffer's scale (codes -> values) and 1 / the output buffer's scale
+  float res_scale, out_inv_scale;
 };
 
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
@@ -60,6 +62,9 @@ struct HaloParams {
   const float* stem_scale;     // [32]
   const float* stem_shift;     // [32]
   int in_h, in_w;              // image size (= the stem's output size)
+  // 1: the output is e4m3 codes of value * out_inv_scale (Conv_3 of the fp8 plan: fp16 in, e4m3 out)
+  int out_e4m3;
+  float out_inv_scale;
 };
 bool conv_halo_supported(const yb_conv_desc* d);
 int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,

@@ -19,7 +19,8 @@
 //   * the epilogue is the staging-tile one of conv_igemm.cu, with pixel (not row) addressing.
 // Warp roles: warp 0 TMA producer, warps 4..11 (warpgroups 1, 2) MMA + epilogue, fp32 accumulators in registers; the
 // producer keeps up to NST halo tiles in flight ahead of the MMAs.
-// Inference only (folded BN): scale/shift + leaky + optional residual, 16-bit NHWC in and out.
+// Inference only (folded BN): scale/shift + leaky + optional residual, 16-bit NHWC in and out.  One instantiation
+// (TO = e4m3, fp16 in) writes the first e4m3 buffer of the fp8 plan: Conv_3, whose fp16 residual is read as usual.
 #include <cudaTypedefs.h>
 #include <string.h>
 
@@ -108,7 +109,7 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0>
+template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T>
 __global__ void __launch_bounds__(HALO_THREADS + 32 * STEMW, 1)
 conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ HaloParams p) {
   using C = HaloCfg<CIN, COUT, STRIDE>;
@@ -267,6 +268,10 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
             f = Pack2<T>::unpack(u.w); v[8 * j + 6] += f.x; v[8 * j + 7] += f.y;
           }
         }
+        if constexpr (std::is_same<TO, __nv_fp8_e4m3>::value) {
+          *reinterpret_cast<uint4*>(static_cast<uint8_t*>(p.out) + off * p.out_ld + c0) = e4m3x16_pack(v, p.out_inv_scale);
+          continue;
+        }
         uint4* op = reinterpret_cast<uint4*>(static_cast<T*>(p.out) + off * p.out_ld + c0);
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
@@ -414,11 +419,11 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
   }
 }
 
-template <typename T, int CIN, int COUT, int STRIDE>
+template <typename T, int CIN, int COUT, int STRIDE, typename TO = T>
 static int launch_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
   using C = HaloCfg<CIN, COUT, STRIDE>;
   static DeviceOnce once;
-  auto kern = conv_halo_kernel<T, CIN, COUT, STRIDE>;
+  auto kern = conv_halo_kernel<T, CIN, COUT, STRIDE, 0, TO>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
   kern<<<grid, HALO_THREADS, C::SMEM_BYTES, st>>>(maps, p);
@@ -516,6 +521,13 @@ int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed
 }
 
 int conv_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
+  if (p.out_e4m3) {
+    if (d->dtype == YB_F16 && d->cin == 32 && d->cout == 64 && d->stride == 1 && p.out_ld % 16 == 0)
+      return launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3>(maps, p, st);
+    set_error("conv_halo: e4m3 output only for fp16 3x3/1 32->64 (got dtype %d cin=%d cout=%d stride=%d)", d->dtype, d->cin,
+              d->cout, d->stride);
+    return YB_ERR_UNSUPPORTED;
+  }
 #define YB_HALO(T)                                                                              \
   if (d->cin == 32 && d->cout == 64 && d->stride == 1) return launch_halo<T, 32, 64, 1>(maps, p, st);   \
   if (d->cin == 32 && d->cout == 64 && d->stride == 2) return launch_halo<T, 32, 64, 2>(maps, p, st);   \

@@ -106,9 +106,105 @@ __global__ void bn_fold_kernel(const float* gamma, const float* beta, const floa
   }
 }
 
+// ----------------------------------------------------------------------------------
+// fp8 (e4m3) inference: per-output-channel weight quantisation, calibration amax, scale folding
+// ----------------------------------------------------------------------------------
+// One block per output row co of the packed [cout_pad, k*k*cin] matrix: s_w[co] = amax_co / 448 (1 for an all-zero or
+// padding row), q = RN-satfinite e4m3(w / s_w[co]).
+__global__ void __launch_bounds__(256) pack_weights_e4m3_kernel(const float* __restrict__ src, int layout, int cout, int cin,
+                                                                int ks, uint8_t* __restrict__ dst, float* __restrict__ w_scale) {
+  const int co = blockIdx.x;
+  const int K = ks * ks * cin;
+  auto at = [&](int k) {
+    const int ci = k % cin, s = (k / cin) % ks, r = k / (cin * ks);
+    long si;
+    if (layout == YB_W_HWIO) si = (((long)r * ks + s) * cin + ci) * cout + co;
+    else if (layout == YB_W_OIHW) si = (((long)co * cin + ci) * ks + r) * ks + s;
+    else si = (long)co * K + k;
+    return src[si];
+  };
+  __shared__ float s_red[8];
+  float m = 0.f;
+  if (co < cout)
+    for (int k = threadIdx.x; k < K; k += blockDim.x) m = fmaxf(m, fabsf(at(k)));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = s_red[0];
+  for (int i = 1; i < 8; ++i) m = fmaxf(m, s_red[i]);
+  const float sw = m > 0.f ? m / 448.f : 1.f;
+  uint8_t* row = dst + (long)co * K;
+  for (int k = threadIdx.x; k < K; k += blockDim.x)
+    row[k] = m > 0.f ? (uint8_t)e4m3x2_pack(at(k) / sw, 0.f) : (uint8_t)0;
+  if (threadIdx.x == 0) w_scale[co] = sw;
+}
+
+// out (zeroed by the caller) = max |x| over a strided [rows, cols] matrix; the max of floats is order-independent, so
+// the result is exact and reproducible (the float bits of non-negative values order like unsigned integers)
+template <typename T>
+__global__ void __launch_bounds__(256) amax_kernel(const T* __restrict__ x, long ld, long rows, int cols,
+                                                   unsigned* __restrict__ out) {
+  float m = 0.f;
+  const long total = rows * cols;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x)
+    m = fmaxf(m, fabsf(static_cast<float>(x[(i / cols) * ld + i % cols])));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));
+}
+
+// e4m3 layer: scale = BN scale (1 for the detection heads) x s_in x s_w[c]; BN layers also get shift (the heads' shift
+// is their bias and is left alone)
+__global__ void fp8_fold_kernel(const float* gamma, const float* beta, const float* mean, const float* var, int c, float eps,
+                                float s_in, const float* w_scale, float* scale, float* shift) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c) return;
+  float sc = 1.f;
+  if (gamma) {
+    sc = gamma[i] / sqrtf(var[i] + eps);
+    shift[i] = beta[i] - mean[i] * sc;
+  }
+  scale[i] = sc * s_in * w_scale[i];
+}
+
+int fp8_fold(const float* gamma, const float* beta, const float* mean, const float* var, int c, float eps, float s_in,
+             const float* w_scale, float* scale, float* shift, cudaStream_t st) {
+  fp8_fold_kernel<<<ceil_div(c, 128), 128, 0, st>>>(gamma, beta, mean, var, c, eps, s_in, w_scale, scale, shift);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
 }  // namespace yb
 
 using namespace yb;
+
+extern "C" int yb_pack_conv_weights_e4m3(const float* src, int layout, int cout, int cin, int ksize, int cout_pad,
+                                         void* dst, float* w_scale, void* stream) {
+  YB_REQUIRE(src && dst && w_scale, "pack_e4m3: null pointer");
+  YB_REQUIRE(layout >= 0 && layout <= 2, "pack_e4m3: bad layout %d", layout);
+  YB_REQUIRE(cout_pad >= cout && cout > 0 && cin > 0 && ksize > 0, "pack_e4m3: bad shape");
+  pack_weights_e4m3_kernel<<<cout_pad, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, layout, cout, cin, ksize,
+                                                                                    static_cast<uint8_t*>(dst), w_scale);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_amax(const void* x, long ld, long rows, int cols, int dtype, float* out, void* stream) {
+  YB_REQUIRE(x && out && rows >= 0 && cols > 0 && ld >= cols, "amax: bad argument");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  YB_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
+  const long total = rows * cols;
+  if (total == 0) return YB_OK;
+  const long cap = (long)num_sms() * 8;
+  const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
+  unsigned* o = reinterpret_cast<unsigned*>(out);
+  if (dtype == YB_F16) amax_kernel<__half><<<grid, 256, 0, st>>>(static_cast<const __half*>(x), ld, rows, cols, o);
+  else if (dtype == YB_BF16)
+    amax_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(x), ld, rows, cols, o);
+  else if (dtype == YB_F32) amax_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(x), ld, rows, cols, o);
+  else { set_error("amax: unsupported dtype %d", dtype); return YB_ERR_UNSUPPORTED; }
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
 
 extern "C" int yb_stem_conv_fwd(const float* x, const float* w_ohwi, const float* scale, const float* shift, int n,
                                 int h, int w, int cout, int dtype, int leaky, void* out, void* stream) {

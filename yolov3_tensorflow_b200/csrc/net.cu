@@ -19,11 +19,18 @@ int train_bind(yb_net* net, cudaStream_t st);
 int train_refresh_dgrad_weights(yb_net* net, int layer, void* stream);
 int nms_candidate_buffers(void* workspace, size_t workspace_bytes, int n_images, int num_boxes, int num_classes,
                           int max_boxes, int** cand_count, float** cand_score, int** cand_idx);
+int fp8_fold(const float* gamma, const float* beta, const float* mean, const float* var, int c, float eps, float s_in,
+             const float* w_scale, float* scale, float* shift, cudaStream_t st);
 int nms_select_gather(const float* boxes, int n_images, int num_boxes, int num_classes, int max_boxes, float iou_thresh,
                       void* workspace, size_t workspace_bytes, float* out_boxes, float* out_scores, int32_t* out_labels,
                       int32_t* out_indices, int32_t* out_counts, cudaStream_t st);
 
 static size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
+
+// fp8 plan: the stem, Conv_1, Conv_2 and Conv_3 (layers 0-3) stay fp16 (HBM-bound kernels with no e4m3 variant, ~5 %
+// of the FLOPs); Conv_3 writes the first e4m3 buffer, every later conv reads and writes e4m3 (heads: fp32 out).
+static constexpr int FP8_FIRST_LAYER = 4;
+static bool layer_is_e4m3(const yb_net* net, int i) { return net->dtype == YB_E4M3 && i >= FP8_FIRST_LAYER; }
 
 struct Builder {
   yb_net* net;
@@ -119,19 +126,25 @@ struct Builder {
     net->fm_buf[0] = fm1.buf; net->fm_buf[1] = fm2.buf; net->fm_buf[2] = fm3.buf;
 
     // ---- arenas ----
-    const size_t esz = 2;
+    const bool fp8 = net->dtype == YB_E4M3;
+    for (auto& b : net->bufs) b.esz = b.fp32 ? 4 : (fp8 ? 1 : 2);
+    for (int i = 0; fp8 && i < FP8_FIRST_LAYER - 1; ++i) net->bufs[net->layers[i].out.buf].esz = 2;
+    net->buf_scale.assign(net->bufs.size(), 1.f);
     size_t o = 0;
     for (auto& b : net->bufs) {
-      b.bytes = (size_t)net->n * b.h * b.w * b.ld * (b.fp32 ? 4 : esz);
+      b.bytes = (size_t)net->n * b.h * b.w * b.ld * b.esz;
       b.offset = o;
       o = align256(o + b.bytes);
     }
     net->act_bytes = o;
     o = 0;
     for (auto& L : net->layers) {
+      const bool q = layer_is_e4m3(net, L.info.index);
+      L.dtype = q ? YB_E4M3 : (fp8 ? YB_F16 : net->dtype);
       const size_t kk = (size_t)L.info.ksize * L.info.ksize * L.info.cin;
       L.w_master = o; o = align256(o + (size_t)L.info.cout * kk * 4);
-      L.w_packed = o; o = align256(o + (size_t)L.cout_pad * kk * esz);
+      L.w_packed = o; o = align256(o + (size_t)L.cout_pad * kk * (q ? 1 : 2));
+      if (q) { L.w_scale = o; o = align256(o + (size_t)L.cout_pad * 4); }
       const size_t cb = (size_t)L.cout_pad * 4;
       if (L.info.has_bn) {
         L.gamma = o; o = align256(o + cb);
@@ -151,7 +164,26 @@ struct Builder {
 
 static void* ten_ptr(const yb_net* net, const Ten& t) {
   const Buf& b = net->bufs[t.buf];
-  return net->act + b.offset + (size_t)t.off * (b.fp32 ? 4 : 2);
+  return net->act + b.offset + (size_t)t.off * b.esz;
+}
+
+// e4m3 plan: each layer's residual and output scales come from its buffers (host-side launch parameters)
+static void apply_fp8_scales(yb_net* net) {
+  for (size_t i = FP8_FIRST_LAYER - 1; i < net->layers.size(); ++i) {
+    Layer& L = net->layers[i];
+    const float so = net->buf_scale[L.out.buf];
+    L.params.res_scale = L.res.buf >= 0 ? net->buf_scale[L.res.buf] : 1.f;
+    L.params.out_inv_scale = 1.f / so;
+    L.halo_params.out_inv_scale = 1.f / so;
+  }
+}
+
+// e4m3 layer: scale = (BN scale) x s_in x s_w[c] (the detection heads' shift is their bias)
+static int fold_e4m3_layer(yb_net* net, Layer& L, cudaStream_t st) {
+  const bool bn = L.info.has_bn;
+  auto f = [&](size_t off) { return reinterpret_cast<float*>(net->par + off); };
+  return fp8_fold(bn ? f(L.gamma) : nullptr, bn ? f(L.beta) : nullptr, bn ? f(L.mean) : nullptr, bn ? f(L.var) : nullptr,
+                  L.info.cout, net->bn_eps, net->buf_scale[L.in.buf], f(L.w_scale), f(L.scale), f(L.shift), st);
 }
 
 __global__ void fill_kernel(float* p, int n, float v) {
@@ -167,7 +199,8 @@ extern "C" int yb_net_create(yb_net** out, int class_num, int n, int h, int w, i
   YB_REQUIRE(out, "net_create: null out pointer");
   YB_REQUIRE(class_num > 0 && n > 0, "net_create: bad class_num/batch");
   YB_REQUIRE(h > 0 && w > 0 && h % 32 == 0 && w % 32 == 0, "net_create: H,W must be multiples of 32 (got %dx%d)", h, w);
-  YB_REQUIRE(dtype == YB_F16 || dtype == YB_BF16, "net_create: dtype must be f16 or bf16");
+  YB_REQUIRE(dtype == YB_F16 || dtype == YB_BF16 || dtype == YB_E4M3, "net_create: dtype must be f16, bf16 or e4m3");
+  YB_REQUIRE(!(dtype == YB_E4M3 && training), "net_create: e4m3 is an inference plan (quantize a trained fp16/bf16 model)");
   yb_net* net = new yb_net();
   net->class_num = class_num; net->n = n; net->h = h; net->w = w; net->dtype = dtype; net->training = training;
   Builder b{net};
@@ -211,8 +244,21 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
     d.ksize = L.info.ksize; d.stride = L.info.stride;
     d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = net->bufs[L.out.buf].ld;
     d.res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
-    d.dtype = net->dtype; d.out_fp32 = L.out_fp32; d.leaky = L.info.has_bn; d.upsample2x = L.upsample;
+    d.dtype = L.dtype; d.out_fp32 = L.out_fp32; d.leaky = L.info.has_bn; d.upsample2x = L.upsample;
     int cp = 0;
+    if (net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1) {
+      // Conv_3 of the fp8 plan: fp16 in, e4m3 out, only the halo kernel has that form
+      YB_REQUIRE(conv_halo_supported(&d), "bind: the e4m3 plan needs the halo kernel for layer %d (w %% 16 == 0)", (int)i);
+      L.halo_desc = d;
+      int rc = conv_halo_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, reinterpret_cast<const float*>(net->par + L.scale),
+                                 reinterpret_cast<const float*>(net->par + L.shift), ten_ptr(net, L.res), ten_ptr(net, L.out),
+                                 &L.halo_maps, &L.halo_params);
+      if (rc) return rc;
+      L.halo_params.out_e4m3 = 1;
+      L.halo_ok = true;
+      L.prepared = false;
+      continue;
+    }
     int rc = conv_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed,
                           reinterpret_cast<const float*>(net->par + L.scale),
                           reinterpret_cast<const float*>(net->par + L.shift),
@@ -237,6 +283,7 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
                                   &L.det_cout_pad) == YB_OK;
     }
   }
+  if (net->fp8_ready) apply_fp8_scales(net);
   if (net->training) return train_bind(net, static_cast<cudaStream_t>(stream));
   return YB_OK;
 }
@@ -251,7 +298,10 @@ extern "C" int yb_net_set_conv_params(yb_net* net, int layer, const float* w, in
   const int c = L.info.cout;
   int rc = yb_pack_conv_weights(w, layout, c, L.info.cin, L.info.ksize, c, YB_F32, net->par + L.w_master, stream);
   if (rc) return rc;
-  rc = yb_pack_conv_weights(w, layout, c, L.info.cin, L.info.ksize, L.cout_pad, net->dtype, net->par + L.w_packed, stream);
+  const bool q = L.dtype == YB_E4M3;
+  rc = q ? yb_pack_conv_weights_e4m3(w, layout, c, L.info.cin, L.info.ksize, L.cout_pad, net->par + L.w_packed,
+                                     reinterpret_cast<float*>(net->par + L.w_scale), stream)
+         : yb_pack_conv_weights(w, layout, c, L.info.cin, L.info.ksize, L.cout_pad, L.dtype, net->par + L.w_packed, stream);
   if (rc) return rc;
   float* scale = reinterpret_cast<float*>(net->par + L.scale);
   float* shift = reinterpret_cast<float*>(net->par + L.shift);
@@ -270,6 +320,10 @@ extern "C" int yb_net_set_conv_params(yb_net* net, int layer, const float* w, in
     fill_kernel<<<ceil_div(L.cout_pad, 128), 128, 0, st>>>(scale, L.cout_pad, 1.0f);
     YB_CUDA(cudaGetLastError());
   }
+  if (q) {
+    rc = fold_e4m3_layer(net, L, st);
+    if (rc) return rc;
+  }
   if (net->training) return train_refresh_dgrad_weights(net, layer, stream);
   return YB_OK;
 }
@@ -277,6 +331,11 @@ extern "C" int yb_net_set_conv_params(yb_net* net, int layer, const float* w, in
 extern "C" int yb_net_refold_bn(yb_net* net, void* stream) {
   YB_REQUIRE(net && net->par, "refold_bn: net not bound");
   for (auto& L : net->layers) {
+    if (L.dtype == YB_E4M3) {
+      int rc = fold_e4m3_layer(net, L, static_cast<cudaStream_t>(stream));
+      if (rc) return rc;
+      continue;
+    }
     if (!L.info.has_bn) continue;
     int rc = yb_bn_fold(reinterpret_cast<const float*>(net->par + L.gamma), reinterpret_cast<const float*>(net->par + L.beta),
                         reinterpret_cast<const float*>(net->par + L.mean), reinterpret_cast<const float*>(net->par + L.var),
@@ -305,6 +364,9 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
   YB_REQUIRE(net && net->act && net->par, "forward: net not bound");
   YB_REQUIRE(images, "forward: null images");
   YB_REQUIRE(first >= 0 && first <= last, "forward: bad layer range");
+  YB_REQUIRE(net->dtype != YB_E4M3 || net->fp8_ready,
+             "forward: the e4m3 plan has no activation scales (yb_net_set_fp8_amax after calibration)");
+  const bool fp8 = net->dtype == YB_E4M3;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* user_fm[3] = {fm1, fm2, fm3};
   if (net->fold_dirty) {   // BN parameters / moving statistics changed by a training step: refold for inference
@@ -330,19 +392,19 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
     if (thin)
       rc = yb_stem_conv_fwd_tc(images, reinterpret_cast<const float*>(net->par + L.w_master),
                                reinterpret_cast<const float*>(net->par + L.scale),
-                               reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, net->dtype, 1,
+                               reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.dtype, 1,
                                ten_ptr(net, L.out), stream);
     else
       rc = yb_stem_conv_fwd(images, reinterpret_cast<const float*>(net->par + L.w_master),
                             reinterpret_cast<const float*>(net->par + L.scale),
                             reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.info.cout,
-                            net->dtype, 1, ten_ptr(net, L.out), stream);
+                            L.dtype, 1, ten_ptr(net, L.out), stream);
     if (rc) return rc;
   }
   for (size_t i = first > 1 ? first : 1; i < net->layers.size() && (int)i <= last; ++i) {
     Layer& L = net->layers[i];
     // the mma.sync halo kernel for the Cin = 32 layers is opt-in (YB_THIN=2); by default they take the tensor-core path
-    const bool thin_cin32 = opt("YB_THIN")[0] == '2';
+    const bool thin_cin32 = opt("YB_THIN")[0] == '2' && !fp8;
     if (thin_cin32 && L.info.ksize == 3 && L.info.cin == 32 && L.info.has_bn && !L.upsample) {
       // Cin = 32: 64-byte im2col rows halve the TMA line rate -> direct halo-tile kernel (csrc/conv_thin.cu)
       yb_conv_desc d;
@@ -374,7 +436,7 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
     // halo-tile kernel: default on for Cin = 32, whose 64-byte im2col rows make the implicit GEMM TMA-row bound; the
     // 64->128 layers leave room for only two halo stages beside their weights.  YB_HALO=0: never, YB_HALO=1: wherever supported.
     const char* hopt = opt("YB_HALO");
-    if (L.halo_ok && hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)) {
+    if (L.halo_ok && ((hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)) || !L.prepared)) {
       int rc = conv_halo_launch(&L.halo_desc, L.halo_maps, L.halo_params, st);
       if (rc) return rc;
       continue;
@@ -395,13 +457,13 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
           hs = net->side_stream;
           forked = true;
         }
-        int rc = conv_launch(net->dtype, L.det_cout_pad, L.det_tmA, L.det_tmB, dp, hs);
+        int rc = conv_launch(L.dtype, L.det_cout_pad, L.det_tmA, L.det_tmB, dp, hs);
         if (rc) return rc;
         continue;
       }
       p->out = user_fm[which] ? (void*)user_fm[which] : ten_ptr(net, L.out);
     }
-    int rc = conv_launch(net->dtype, L.cout_pad, L.tmA, L.tmB, *p, st);
+    int rc = conv_launch(L.dtype, L.cout_pad, L.tmA, L.tmB, *p, st);
     if (rc) return rc;
   }
   if (forked) {
@@ -502,8 +564,40 @@ extern "C" int yb_net_layer_output(const yb_net* net, int layer, void** ptr, int
              "layer_output: bad argument");
   const Layer& L = net->layers[layer];
   *ptr = ten_ptr(net, L.out);
-  *ld = net->bufs[L.out.buf].ld;
-  *dtype = L.out_fp32 ? YB_F32 : net->dtype;
+  const Buf& b = net->bufs[L.out.buf];
+  *ld = b.ld;
+  *dtype = b.fp32 ? YB_F32 : (b.esz == 1 ? YB_E4M3 : (net->dtype == YB_E4M3 ? YB_F16 : net->dtype));
+  return YB_OK;
+}
+
+extern "C" int yb_net_set_fp8_amax(yb_net* net, const float* amax, int count, void* stream) {
+  YB_REQUIRE(net && net->par && amax, "set_fp8_amax: net not bound");
+  YB_REQUIRE(net->dtype == YB_E4M3, "set_fp8_amax: not an e4m3 plan");
+  YB_REQUIRE(count == (int)net->layers.size(), "set_fp8_amax: need one amax per layer (%d, got %d)", (int)net->layers.size(),
+             count);
+  // a buffer's scale covers every layer that writes it (the concat buffers: the upsampling conv and the route conv)
+  std::vector<float> bmax(net->bufs.size(), 0.f);
+  for (size_t i = 0; i < net->layers.size(); ++i) {
+    YB_REQUIRE(amax[i] >= 0.f && isfinite(amax[i]), "set_fp8_amax: layer %d amax %g is not finite and >= 0", (int)i, amax[i]);
+    float& m = bmax[net->layers[i].out.buf];
+    m = fmaxf(m, amax[i]);
+  }
+  for (size_t b = 0; b < net->bufs.size(); ++b)
+    net->buf_scale[b] = (net->bufs[b].esz == 1 && bmax[b] > 0.f) ? bmax[b] / 448.f : 1.f;
+  net->fp8_ready = true;
+  apply_fp8_scales(net);
+  return yb_net_refold_bn(net, stream);
+}
+
+extern "C" int yb_net_fp8_layer_scales(const yb_net* net, int layer, float* in_res_out, float** w_scale) {
+  YB_REQUIRE(net && net->par && layer >= 0 && layer < (int)net->layers.size() && in_res_out && w_scale,
+             "fp8_layer_scales: bad argument");
+  YB_REQUIRE(net->dtype == YB_E4M3, "fp8_layer_scales: not an e4m3 plan");
+  const Layer& L = net->layers[layer];
+  in_res_out[0] = L.in.buf >= 0 ? net->buf_scale[L.in.buf] : 1.f;
+  in_res_out[1] = L.res.buf >= 0 ? net->buf_scale[L.res.buf] : 1.f;
+  in_res_out[2] = net->buf_scale[L.out.buf];
+  *w_scale = L.dtype == YB_E4M3 ? reinterpret_cast<float*>(net->par + L.w_scale) : nullptr;
   return YB_OK;
 }
 

@@ -17,6 +17,7 @@ struct Ten {          // a view of an activation: buffer id + channel slice
 struct Buf {
   int h, w, ld;       // [n, h, w, ld]
   int fp32;           // detection outputs are float32
+  int esz = 2;        // bytes per element: 4 (fp32), 2 (fp16 / bf16), 1 (e4m3)
   size_t offset = 0, bytes = 0;
 };
 
@@ -25,8 +26,9 @@ struct Layer {
   Ten in, out, res;   // res.buf == -2: none
   bool upsample = false, out_fp32 = false;
   int cout_pad = 0;
-  // parameter arena offsets (bytes)
-  size_t w_master = 0, w_packed = 0, gamma = 0, beta = 0, mean = 0, var = 0, bias = 0, scale = 0, shift = 0;
+  int dtype = 0;      // yb_dtype of the conv's input and packed weights (e4m3 plan: fp16 for layers 0-3)
+  // parameter arena offsets (bytes); w_scale: e4m3 layers' per-output-channel weight scales, fp32 [cout_pad]
+  size_t w_master = 0, w_packed = 0, gamma = 0, beta = 0, mean = 0, var = 0, bias = 0, scale = 0, shift = 0, w_scale = 0;
   // prepared launch state
   CUtensorMap tmA, tmB;
   ConvParams params;
@@ -66,6 +68,9 @@ struct yb_net {
   std::vector<yb::Buf> bufs;
   int fm_buf[3];
   size_t act_bytes = 0, param_bytes = 0;
+  // e4m3 plan: per-buffer activation scale (value = code x scale; 1 for 16-bit / fp32 buffers), set by calibration
+  std::vector<float> buf_scale;
+  bool fp8_ready = false;
   uint8_t* act = nullptr;
   uint8_t* par = nullptr;
   // ---- training plan ----

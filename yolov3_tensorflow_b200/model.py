@@ -145,14 +145,24 @@ class _Plan:
         p, ld, dt = C.c_void_p(), C.c_int(), C.c_int()
         check(lib.yb_net_layer_output(self.handle, i, C.byref(p), C.byref(ld), C.byref(dt)), "yb_net_layer_output")
         info = self.layer_info(i)
-        tdt = {0: torch.float16, 1: torch.bfloat16, 2: torch.float32}[dt.value]
-        esz = 4 if dt.value == 2 else 2
+        tdt = {0: torch.float16, 1: torch.bfloat16, 2: torch.float32, 3: torch.float8_e4m3fn}[dt.value]
+        esz = {2: 4, 3: 1}.get(dt.value, 2)
         off = p.value - self.act.data_ptr()
         up = 2 if info.upsample2x else 1
         oh, ow = info.out_h * up, info.out_w * up
         nelem = ((self.n * oh * ow - 1) * ld.value + info.cout)
         flat = self.act[off: off + nelem * esz].view(tdt)
         return flat.as_strided((self.n, oh, ow, info.cout), (oh * ow * ld.value, ow * ld.value, ld.value, 1))
+
+    def fp8_scales(self):
+        """e4m3 plan: ([(s_in, s_res, s_out)] per layer, [weight scales float32 [cout_pad] | None] per layer)."""
+        act, wts = [], []
+        for i in range(self.num_layers):
+            v, wp = (C.c_float * 3)(), C.c_void_p()
+            check(lib.yb_net_fp8_layer_scales(self.handle, i, v, C.byref(wp)), "yb_net_fp8_layer_scales")
+            act.append(tuple(float(a) for a in v))
+            wts.append(None if not wp.value else self._view(wp.value, (lib.yb_conv_cout_pad(self.layer_info(i).cout),)).clone())
+        return act, wts
 
     def __del__(self):
         try:
@@ -191,6 +201,7 @@ class yolov3(object):
         self._opt_kind = None        # optimizer whose slots the arena currently holds
         self._frozen = set()         # conv indices excluded from the update (train.py:81 update_part)
         self.loss_scale = 1024.0 if self._torch_dtype == torch.float16 else 1.0   # static loss scale of the 16-bit backward
+        self._fp8_amax = None        # quantize_fp8() models: per-layer calibration amax (their plans are e4m3)
 
     # ------------------------------------------------------------------ parameters
     @staticmethod
@@ -222,9 +233,18 @@ class yolov3(object):
                 conv(f // 2, 1)
         return t
 
+    def _not_fp8(self, what):
+        if self._fp8_amax is not None:
+            raise ValueError(f"{what}: this model is fp8-quantized (inference only, calibrated activation scales); "
+                             "change the fp16/bf16 source model and call quantize_fp8() again")
+
     def set_params(self, params, layout="HWIO"):
         """params: 75 dicts in creation order with 'w' (+ 'gamma','beta','mean','var' | 'b'),
         numpy or torch float32.  layout of 'w': 'HWIO' (TF variables) or 'OIHW' (darknet)."""
+        self._not_fp8("set_params")
+        self._set_params(params, layout)
+
+    def _set_params(self, params, layout):
         table = self.conv_table(self.class_num)
         if len(params) != len(table):
             raise ValueError(f"expected {len(table)} conv parameter sets, got {len(params)}")
@@ -249,6 +269,7 @@ class yolov3(object):
     def init_params(self, seed=0):
         """Random init as the reference graph would (SURVEY.md B.1): Glorot-uniform conv weights,
         gamma=1, beta=0, moving mean 0 / variance 1, zero detection biases (model.py:55-57)."""
+        self._not_fp8("init_params")
         rng = np.random.default_rng(seed)
         ps = []
         for cin, cout, k, s, bn in self.conv_table(self.class_num):
@@ -312,7 +333,61 @@ class yolov3(object):
             self._fold_dirty = False
         if not self._have_params:
             raise _lib.YoloB200Error("no parameters: call load_weights(model, file), set_params() or init_params()")
+        if self._fp8_amax is not None and not getattr(plan, "_fp8_set", False):
+            # every plan of a quantized model (any batch / resolution) uses the one calibrated set of scales
+            a = self._fp8_amax
+            check(lib.yb_net_set_fp8_amax(plan.handle, (C.c_float * len(a))(*a), len(a), stream_handle()), "yb_net_set_fp8_amax")
+            plan._fp8_set = True
         return plan
+
+    # ------------------------------------------------------------------ calibrated fp8 (e4m3) inference
+    def quantize_fp8(self, calib_images):
+        """-> a new inference-only model that runs the convs after Conv_3 with e4m3 activations and weights.
+
+        calib_images: one float32 [N,H,W,3] batch or a list of them.  This model's inference forward runs on each; the
+        max |x| of every layer output over all batches (yb_amax) sets the per-buffer activation scales
+        (amax / 448, buffers with two producers take the larger), and the weights are quantized per output channel
+        from this model's float32 master parameters.  This model is left as it was.  The quantized model supports
+        forward(is_training=False), predict, predict_scores, detect_raw, detect and detect_graphed at any batch size
+        and resolution; training and parameter changes raise ValueError."""
+        self._not_fp8("quantize_fp8")
+        batches = calib_images if isinstance(calib_images, (list, tuple)) else [calib_images]
+        if not batches:
+            raise ValueError("quantize_fp8: no calibration images")
+        amax = None
+        out = torch.empty(1, dtype=torch.float32, device=self.device)
+        for xb in batches:
+            self.forward(xb)
+            plan = self._last_plan
+            vals = torch.zeros(plan.num_layers, dtype=torch.float32, device=self.device)
+            for i in range(1, plan.num_layers):      # layer 0's output is never written (the stem is fused into Conv_1)
+                if not plan.layer_info(i).has_bn:
+                    continue                         # detection heads: float32 outputs, no scale
+                y = plan.layer_output(i)
+                p, ld, dt = C.c_void_p(), C.c_int(), C.c_int()
+                check(lib.yb_net_layer_output(plan.handle, i, C.byref(p), C.byref(ld), C.byref(dt)), "yb_net_layer_output")
+                rows = y.shape[0] * y.shape[1] * y.shape[2]
+                check(lib.yb_amax(p, ld.value, rows, y.shape[3], dt.value, ptr(out), stream_handle()), "yb_amax")
+                vals[i] = out[0]
+            amax = vals if amax is None else torch.maximum(amax, vals)
+        q = yolov3(self.class_num, self.anchors, self.use_label_smooth, self.use_focal_loss, self.batch_norm_decay,
+                   self.weight_decay, self.use_static_shape, dtype="fp16", device=self.device)
+        q._dtype_code = _lib.YB_E4M3
+        q._set_params(self.get_params(), "HWIO")
+        q._fp8_amax = [float(v) for v in amax.cpu().tolist()]
+        return q
+
+    def fp8_scales(self):
+        """quantize_fp8() models: dict(act=[(s_in, s_res, s_out)] per layer: the scales of the layer's input, residual
+        and output buffers (1 for fp16 / float32 buffers), weight=[float32 CPU tensor [cout_pad] | None] per layer:
+        the per-output-channel weight scales (None for the fp16 layers 0-3))."""
+        if self._fp8_amax is None:
+            raise ValueError("fp8_scales: not an fp8-quantized model (see quantize_fp8)")
+        plan = self._last_plan if getattr(self, "_last_plan", None) is not None else next(iter(self._plans.values()), None)
+        if plan is None:
+            raise _lib.YoloB200Error("fp8_scales: run the model once first (its scales are set when a plan is built)")
+        act, wts = plan.fp8_scales()
+        return {"act": act, "weight": [None if w is None else w.cpu() for w in wts]}
 
     def set_trainable(self, conv_indices, trainable=True):
         """train.py:81 `update_part`: conv indices (creation order, 0..74) whose weights / BN affine / bias the
@@ -339,6 +414,8 @@ class yolov3(object):
         if h % 32 or w % 32:
             raise ValueError(f"H and W must be multiples of 32, got {h}x{w}")
         self.img_size = (h, w)
+        if is_training:
+            self._not_fp8("forward(is_training=True)")
         plan = self._plan(n, h, w, training=bool(is_training))
         D = 3 * (5 + self.class_num)
         fms = [torch.empty((n, h // s, w // s, D), dtype=torch.float32, device=self.device) for s in (32, 16, 8)]
@@ -683,6 +760,7 @@ class yolov3(object):
         concatenated batch (up to fp32 summation order) and every rank holds the same moving statistics.  Every rank
         must run the same N, H and W.  Runs train_step_sync_bn() over NCCL; with one rank it is the ordinary step.
         Returns [total, xy, wh, conf, class] as 0-dim float32 CUDA tensors of the LOCAL batch."""
+        self._not_fp8("train_step")
         import torch.distributed as dist
         if sync_bn and freeze_bn:
             raise ValueError("sync_bn=True needs training-mode BN: frozen BN (freeze_bn=True) has no batch statistics to synchronise")
@@ -729,6 +807,7 @@ class yolov3(object):
                               mean (1/world), which the optimizer folds in.
         Then the update and the loss finalize run as in train_step, and the generator returns what train_step
         returns.  Every rank must run the same number of images and the same H x W."""
+        self._not_fp8("train_step_sync_bn")
         bn_replicas = int(bn_replicas)
         if bn_replicas < 1:
             raise ValueError(f"bn_replicas must be >= 1, got {bn_replicas}")

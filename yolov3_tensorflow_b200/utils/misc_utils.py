@@ -33,7 +33,9 @@ def load_weights(model, weights_file):
     conv [beta, gamma, mean, var] (or [bias]) followed by the weights as (Cout, Cin, kh, kw) float32.
     The (Cout,Cin,kh,kw) -> engine-layout transposition the reference does on the host (:117-120)
     happens on the GPU (yb_pack_conv_weights).  Raises ValueError on a size mismatch
-    (tf.assign(validate_shape=True))."""
+    (tf.assign(validate_shape=True)), and on an fp8-quantized model (yolov3.quantize_fp8), whose weights are fixed."""
+    if getattr(model, "_fp8_amax", None) is not None:
+        model._not_fp8("load_weights")
     with open(weights_file, "rb") as fp:
         np.fromfile(fp, dtype=np.int32, count=5)
         weights = np.fromfile(fp, dtype=np.float32)
