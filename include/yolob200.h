@@ -282,6 +282,37 @@ int yb_nms(const float* boxes, const float* scores, int n_images, int num_boxes,
            float* out_scores, int32_t* out_labels, int32_t* out_indices, int32_t* out_counts, void* stream);
 
 /* ---------------------------------------------------------------------------------
+ * PASCAL-VOC evaluation  (replaces utils/eval_utils.py:311-423 voc_ap / voc_eval, called per class by
+ * eval.py:114-137 and train.py's validation): detections of a whole validation set are matched batch by batch
+ * into a caller-owned pool of 64-bit records, then sorted and reduced to per-class (npos, nd, rec, prec, ap).
+ * --------------------------------------------------------------------------------- */
+/* ground-truth boxes per image that yb_voc_match accepts (vmax) */
+enum { YB_VOC_MAX_GT = 1024 };
+/* Match one batch of NMS output to its ground truth and append one record per detection at pool[pool_offset + ...].
+ *   out_boxes [n, cap, 4] float32 xyxy, out_scores / out_labels [n, cap], counts [n] int32: yb_nms / yb_net_detect
+ *   output (classes ascending, score descending inside a class; entries past counts[i], clamped to [0, cap], ignored)
+ *   gt_boxes [n, vmax, 4] float64 xyxy, gt_labels [n, vmax] int32, gt_counts [n] int32 (clamped to [0, vmax]);
+ *   labels outside [0, num_classes) belong to no class.  vmax <= YB_VOC_MAX_GT.
+ *   Image i's records go to pool_offset + counts[0] + ... + counts[i-1] onward (same order as out_*); the caller keeps
+ *   pool_offset + sum(counts) <= pool_capacity (records past the capacity are dropped).
+ *   class_counts [num_classes][2] uint64 (npos, nd) is ACCUMULATED into: zero it when a new evaluation starts.
+ * The rule is voc_eval's: a detection is a TP iff the first gt box of its class with the highest '+1 pixel' IoU
+ * (float64; the detection's own area in float32) has IoU > iou_thresh and no higher-scored detection of the same
+ * (image, class) took it. */
+int yb_voc_match(const float* out_boxes, const float* out_scores, const int32_t* out_labels, const int32_t* counts,
+                 int n, int cap, const double* gt_boxes, const int32_t* gt_labels, const int32_t* gt_counts, int vmax,
+                 int num_classes, double iou_thresh, uint64_t* pool, long pool_offset, long pool_capacity,
+                 uint64_t* class_counts, void* stream);
+/* out [num_classes][5] float64 = voc_eval(...) of every class over the first pool_size records: (npos, nd, rec, prec,
+ * ap), (1e-6, 1e-6, 0, 0, 0) for a class without detections.  Detections are ranked by descending score, ties in pool
+ * order (a stable sort).  use_07_metric: 11-point AP (bit-exact), else the area under the precision envelope (summed in
+ * a different order than numpy: equal within 1e-12).  The pool is not modified.  num_classes <= 65535,
+ * pool_size < 2^31. */
+int yb_voc_ap_workspace_bytes(long pool_size, int num_classes, size_t* bytes);
+int yb_voc_ap(const uint64_t* pool, long pool_size, const uint64_t* class_counts, int num_classes, int use_07_metric,
+              void* workspace, size_t workspace_bytes, double* out, void* stream);
+
+/* ---------------------------------------------------------------------------------
  * Loss  (replaces model.py:192-304 loss_layer, :307-345 box_iou, :348-365 compute_loss and
  * the part of TF autodiff (train.py:112) that differentiates them)
  * --------------------------------------------------------------------------------- */

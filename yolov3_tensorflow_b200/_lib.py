@@ -16,6 +16,7 @@ YB_W_HWIO, YB_W_OIHW, YB_W_OHWI = 0, 1, 2
 YB_OPT_SGD, YB_OPT_MOMENTUM, YB_OPT_RMSPROP, YB_OPT_ADAM = 0, 1, 2, 3
 YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
 YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
+YB_VOC_MAX_GT = 1024
 
 
 class YoloB200Error(RuntimeError):
@@ -96,6 +97,9 @@ _SIGS = {
     "yb_predict": ([vp, vp, vp, i32, i32, i32, i32, C.POINTER(f32), vp, vp, vp, vp, vp], i32),
     "yb_nms_workspace_bytes": ([i32, i32, i32, i32, C.POINTER(sz)], i32),
     "yb_nms": ([vp, vp, i32, i32, i32, i32, f32, f32, vp, sz, vp, vp, vp, vp, vp, vp], i32),
+    "yb_voc_match": ([vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, C.c_double, vp, C.c_long, C.c_long, vp, vp], i32),
+    "yb_voc_ap_workspace_bytes": ([C.c_long, i32, C.POINTER(sz)], i32),
+    "yb_voc_ap": ([vp, C.c_long, vp, i32, i32, vp, sz, vp, vp], i32),
     "yb_loss_workspace_bytes": ([i32, i32, i32, C.POINTER(sz)], i32),
     "yb_loss_layer": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32, i32, f32, f32, vp, sz, vp, vp, i32, i32, vp], i32),
     "yb_loss_finalize": ([vp, vp, vp], i32),

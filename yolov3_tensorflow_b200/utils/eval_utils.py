@@ -5,9 +5,13 @@ through ONE batched NMS call on the device (utils.nms_utils.batched_nms_raw) and
 to the host, where the bookkeeping (a few hundred boxes) stays numpy like the reference's."""
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 import torch
 
+from .. import _lib
+from .._lib import lib, check, ptr, stream_handle
 from .nms_utils import batched_nms_raw
 
 
@@ -171,3 +175,129 @@ def parse_gt_rec_lines(lines, target_img_size, letterbox_resize=True):
                 objs.append([x0 * new_w / ow, y0 * new_h / oh, x1 * new_w / ow, y1 * new_h / oh, lab])
         gt[img_id] = objs
     return gt
+
+
+def pack_gt_rec(gt_dict, image_ids, vmax=None):
+    """Ground truth of a batch in parse_gt_rec_lines' format ({img_id: [[x0, y0, x1, y1, label], ...]}) -> padded host
+    arrays for VOCEvaluator.add_batch, pinned when CUDA is available: boxes [n, vmax, 4] float64 (the coordinates voc_eval compares
+    with), labels [n, vmax] int32, counts [n] int32.  Padding is zero boxes with label -1."""
+    objs = [gt_dict.get(i, []) for i in image_ids]
+    n = len(objs)
+    if n == 0:
+        raise ValueError("pack_gt_rec: no images")
+    counts = np.asarray([len(o) for o in objs], np.int32)
+    vmax = int(vmax or max(1, int(counts.max())))
+    if int(counts.max()) > vmax:
+        raise ValueError(f"pack_gt_rec: {int(counts.max())} boxes > vmax {vmax}")
+    hb = torch.zeros((n, vmax, 4), dtype=torch.float64)
+    hl = torch.full((n, vmax), -1, dtype=torch.int32)
+    for i, o in enumerate(objs):
+        if o:
+            hb[i, :len(o)] = torch.from_numpy(np.asarray([r[:4] for r in o], np.float64))
+            hl[i, :len(o)] = torch.from_numpy(np.asarray([int(r[-1]) for r in o], np.int32))
+    out = (hb, hl, torch.from_numpy(counts))
+    return tuple(t.pin_memory() for t in out) if torch.cuda.is_available() else out
+
+
+class VOCEvaluator:
+    """voc_eval for every class of a validation set on the device (libyolob200.so: yb_voc_match, yb_voc_ap).
+
+    add_batch() takes one batch's NMS output as detect_raw / batched_nms_raw return it ([n, C*max_boxes] layout) and
+    its ground truth (pack_gt_rec), matches detections to ground truth on the device and appends one 8-byte record
+    per detection to a device pool; no detection is copied to the host.  result() sorts the pool and returns, per
+    class, what voc_eval(gt_dict, rows, c, iou_thresh, use_07_metric) returns for the get_preds_gpu rows of the same
+    batches in the same order, with ties in score ranked in that order (a stable sort; numpy's default sort may order
+    ties either way).  Both metrics can be read from one pool."""
+
+    def __init__(self, num_classes, iou_thresh=0.5, device=None):
+        self.num_classes = int(num_classes)
+        if not 1 <= self.num_classes <= 65535:
+            raise ValueError(f"VOCEvaluator: num_classes {num_classes} outside [1, 65535]")
+        self.iou_thresh = float(iou_thresh)
+        self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+        self._pool = torch.empty((1 << 16,), dtype=torch.int64, device=self.device)
+        self._class_counts = torch.zeros((self.num_classes, 2), dtype=torch.int64, device=self.device)
+        self._size = 0
+        self._ws = None
+
+    def reset(self):
+        self._size = 0
+        self._class_counts.zero_()
+
+    def __len__(self):
+        """Detections added so far."""
+        return self._size
+
+    def add_batch(self, out_boxes, out_scores, out_labels, counts, gt_boxes, gt_labels, gt_counts):
+        """out_boxes [n, cap, 4] float32, out_scores [n, cap] float32, out_labels [n, cap] int32, counts [n] int32 on
+        the device (detect_raw / batched_nms_raw output); gt_boxes [n, vmax, 4] float64, gt_labels [n, vmax] int32,
+        gt_counts [n] int32, host (copied asynchronously) or device.  One host synchronisation: the batch's detection
+        count, read to grow the pool."""
+        dev = self.device
+        for t in (out_boxes, out_scores, out_labels, counts):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == dev):
+                raise TypeError(f"VOCEvaluator.add_batch: detections must be CUDA tensors on {dev}")
+        if (out_boxes.dtype, out_scores.dtype, out_labels.dtype, counts.dtype) != (torch.float32, torch.float32,
+                                                                                    torch.int32, torch.int32):
+            raise TypeError("VOCEvaluator.add_batch: expects float32 boxes / scores and int32 labels / counts")
+        n, cap = int(out_scores.shape[0]), int(out_scores.shape[1])
+        if tuple(out_boxes.shape) != (n, cap, 4) or tuple(out_labels.shape) != (n, cap) or tuple(counts.shape) != (n,):
+            raise ValueError(f"VOCEvaluator.add_batch: detection shapes {tuple(out_boxes.shape)} / {tuple(out_scores.shape)}"
+                             f" / {tuple(out_labels.shape)} / {tuple(counts.shape)}")
+        gb = gt_boxes.to(dev, non_blocking=True).contiguous()
+        gl = gt_labels.to(dev, non_blocking=True).contiguous()
+        gc = gt_counts.to(dev, non_blocking=True).contiguous()
+        if gb.dtype != torch.float64 or gl.dtype != torch.int32 or gc.dtype != torch.int32:
+            raise TypeError("VOCEvaluator.add_batch: expects float64 gt boxes and int32 gt labels / counts")
+        vmax = int(gb.shape[1]) if gb.dim() == 3 else -1
+        if tuple(gb.shape) != (n, vmax, 4) or tuple(gl.shape) != (n, vmax) or tuple(gc.shape) != (n,):
+            raise ValueError(f"VOCEvaluator.add_batch: gt shapes {tuple(gb.shape)} / {tuple(gl.shape)} / {tuple(gc.shape)}"
+                             f" do not match {n} images")
+        if vmax > _lib.YB_VOC_MAX_GT:
+            raise ValueError(f"VOCEvaluator.add_batch: {vmax} gt boxes per image > {_lib.YB_VOC_MAX_GT}")
+        if n == 0:
+            return
+        ob, os_, ol, oc = out_boxes.contiguous(), out_scores.contiguous(), out_labels.contiguous(), counts.contiguous()
+        with torch.cuda.device(dev):
+            total = int(oc.clamp(0, cap).sum())               # the one host synchronisation
+            need = self._size + total
+            if need > self._pool.numel():
+                pool = torch.empty((max(need, 2 * self._pool.numel()),), dtype=torch.int64, device=dev)
+                pool[:self._size].copy_(self._pool[:self._size])
+                self._pool = pool
+            check(lib.yb_voc_match(ptr(ob), ptr(os_), ptr(ol), ptr(oc), n, cap, ptr(gb), ptr(gl), ptr(gc), vmax,
+                                   self.num_classes, self.iou_thresh, ptr(self._pool), self._size, self._pool.numel(),
+                                   ptr(self._class_counts), stream_handle()), "yb_voc_match")
+        self._size = need
+
+    def result(self, use_07_metric=False):
+        """[(npos, nd, rec, prec, ap)] for classes 0..C-1, as voc_eval returns them ((1e-6, 1e-6, 0, 0, 0) for a class
+        without detections)."""
+        dev = self.device
+        need = C.c_size_t()
+        check(lib.yb_voc_ap_workspace_bytes(self._size, self.num_classes, C.byref(need)), "yb_voc_ap_workspace_bytes")
+        if self._ws is None or self._ws.numel() < need.value:
+            self._ws = torch.empty((max(need.value, 256),), dtype=torch.uint8, device=dev)
+        out = torch.empty((self.num_classes, 5), dtype=torch.float64, device=dev)
+        with torch.cuda.device(dev):
+            check(lib.yb_voc_ap(ptr(self._pool), self._size, ptr(self._class_counts), self.num_classes,
+                                int(bool(use_07_metric)), ptr(self._ws), self._ws.numel(), ptr(out), stream_handle()),
+                  "yb_voc_ap")
+            res = out.cpu().numpy()
+        rows = []
+        for npos, nd, rec, prec, ap in res.tolist():
+            if nd == 1e-6:
+                rows.append((1e-6, 1e-6, 0, 0, 0))
+            else:
+                rows.append((int(npos), int(nd), np.float64(rec), np.float64(prec), np.float64(ap)))
+        return rows
+
+    def summary(self, use_07_metric=False):
+        """(mAP, recall, precision) as eval.py:125-137 reports them: AP averaged over the classes, recall weighted by
+        npos, precision weighted by nd (AverageMeter.update(val, n) in class order)."""
+        sums, cnts = [0., 0., 0.], [0., 0., 0.]
+        for npos, nd, rec, prec, ap in self.result(use_07_metric):
+            for k, (v, w) in enumerate(((ap, 1), (rec, npos), (prec, nd))):
+                sums[k] += v * w
+                cnts[k] += w
+        return tuple(s / float(c) for s, c in zip(sums, cnts))
