@@ -212,11 +212,22 @@ int yb_pack_dgrad_weights_s2(const float* w_ohwi, int cout, int cin, int k_cout,
                              void* stream);
 int yb_conv2d_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
                        const void* res, int res_ld, void* dx, int dx_ld, void* stream);
-/* Host-only: the split-K plan yb_conv2d_wgrad picks for a layer with `tiles` output tiles (tap groups x ci chunks x
- * co tiles) over `num_pixel_blocks` 64-pixel blocks on `sms` SMs — the count that minimises
- * waves x (blocks per CTA + epi_blocks); every block is covered exactly once. */
-int yb_wgrad_split_plan(long num_pixel_blocks, long tiles, int sms, int epi_blocks, long* splits,
-                        long* blocks_per_split);
+/* Host-only: the kernel and grid yb_conv2d_wgrad would launch for `d` with the current options (yb_set_option:
+ * YB_WGRAD_TP, YB_WGRAD_EPI, YB_WGRAD_SPLITS) on a device with sm_count SMs.  The output pixels form num_kb 64-pixel
+ * blocks; split-K cuts them into `splits` ranges of kb_per_split blocks (the last range may be shorter, none is empty),
+ * by default the count that minimises waves x (blocks per CTA + YB_WGRAD_EPI).  Grid = (splits, tap groups x input-
+ * channel chunks of bnw, 128-row output-channel tiles); tiles = grid_y x grid_z. */
+typedef struct yb_wgrad_schedule_info {
+  int bnw;           /* input channels per tap and tile                 */
+  int tp;            /* filter taps per CTA (1, or 3: one kernel row)   */
+  int stages;        /* operand-ring depth of that kernel               */
+  int num_kb;        /* 64-pixel blocks                                 */
+  int kb_per_split;  /* blocks per CTA                                  */
+  int splits;
+  int tiles;
+  int grid_x, grid_y, grid_z;
+} yb_wgrad_schedule_info;
+int yb_wgrad_schedule(const yb_conv_desc* d, int sm_count, yb_wgrad_schedule_info* info);
 /* BN batch statistics -> scale/shift for bn_act_apply, saved mean/invstd for the backward, moving-stat update
  * (biased variance normalises, unbiased variance feeds the moving average; moving_* nullable). */
 int yb_bn_finalize(const float* sum, const float* sqsum, long count, int c, const float* gamma, const float* beta,

@@ -105,28 +105,98 @@ def test_config_optimizer_and_tf_variable_names():
     assert names[5][2] == "yolov3/darknet53_body/Conv_1/weights:0" and names[1][2] == "yolov3/darknet53_body/Conv/BatchNorm/gamma:0"
 
 
-def test_wgrad_split_plan_one_wave_and_every_block_once():
-    """Host logic of yb_conv2d_wgrad (csrc/conv_wgrad.cu: wgrad_pick_splits): the split-K count minimises
-    waves x (pixel blocks per CTA + epilogue); every 64-pixel block is covered exactly once, no split is empty."""
+def _wgrad_desc(n, h, w, cin, cout, k, s):
+    from yolov3_tensorflow_b200 import _lib as L
+    return L.ConvDesc(n=n, h=h, w=w, cin=cin, cout=cout, ksize=k, stride=s, in_ld=cin, out_ld=cout, res_ld=0,
+                      dtype=L.YB_F16, out_fp32=0, leaky=0, upsample2x=0)
+
+
+def _wgrad_schedule(desc, sms=148, **opts):
+    """yb_wgrad_schedule under the given YB_WGRAD_* options (restored afterwards)."""
     import ctypes as C
     from yolov3_tensorflow_b200 import _lib as L
+    keys = ("YB_WGRAD_TP", "YB_WGRAD_EPI", "YB_WGRAD_SPLITS")
+    info = L.WgradSchedule()
+    try:
+        for k in keys:
+            L.set_option(k, opts.get(k))
+        L.check(L.lib.yb_wgrad_schedule(C.byref(desc), sms, C.byref(info)), "yb_wgrad_schedule")
+    finally:
+        for k in keys:
+            L.set_option(k, None)
+    return info
 
-    def plan(num_kb, tiles, sms=148, epi=40):
-        s, k = C.c_long(), C.c_long()
-        L.check(L.lib.yb_wgrad_split_plan(num_kb, tiles, sms, epi, C.byref(s), C.byref(k)), "yb_wgrad_split_plan")
-        return s.value, k.value
 
-    # the training step's layers at batch 32 @416 (pixel blocks, tiles) -> (splits, blocks per split)
-    cases = {(21632, 1): (148, 147), (5408, 3): (49, 111), (1352, 6): (24, 57), (338, 24): (6, 57), (85, 96): (1, 85),
-             (85, 32): (4, 22), (1352, 2): (72, 19)}
-    for (num_kb, tiles), want in cases.items():
-        assert plan(num_kb, tiles) == want, (num_kb, tiles, plan(num_kb, tiles))
-    for num_kb, tiles in list(cases) + [(1, 1), (7, 400), (1000, 149), (64, 1)]:
-        s, k = plan(num_kb, tiles)
+# (n, h, w, cin, cout, k, s) -> (64-pixel blocks, tiles): the training step's layers at batch 32 @416 and a few more
+WGRAD_PLAN_DESCS = {
+    (32, 208, 208, 64, 32, 1, 1): (21632, 1),
+    (32, 104, 104, 64, 128, 3, 1): (5408, 3),
+    (32, 52, 52, 128, 128, 3, 1): (1352, 6),
+    (32, 26, 26, 256, 256, 3, 1): (338, 24),
+    (32, 13, 13, 512, 512, 3, 1): (85, 96),
+    (32, 13, 13, 1024, 512, 1, 1): (85, 32),
+    (32, 52, 52, 256, 128, 1, 1): (1352, 2),
+    (1, 8, 8, 64, 64, 1, 1): (1, 1),
+    (1, 20, 21, 3200, 2048, 1, 1): (7, 400),
+    (1, 250, 256, 4768, 128, 1, 1): (1000, 149),
+    (1, 64, 64, 64, 64, 1, 1): (64, 1),
+}
+
+
+def test_wgrad_schedule_one_wave_and_every_block_once():
+    """Host logic of yb_conv2d_wgrad (csrc/conv_wgrad.cu: yb_wgrad_schedule): the split-K count minimises
+    waves x (pixel blocks per CTA + epilogue); every 64-pixel block is covered exactly once, no split is empty."""
+    want = {(21632, 1): (148, 147), (5408, 3): (49, 111), (1352, 6): (24, 57), (338, 24): (6, 57), (85, 96): (1, 85),
+            (85, 32): (4, 22), (1352, 2): (72, 19)}
+    for shape, (num_kb, tiles) in WGRAD_PLAN_DESCS.items():
+        i = _wgrad_schedule(_wgrad_desc(*shape))
+        assert (i.num_kb, i.tiles) == (num_kb, tiles), shape
+        assert (i.grid_x, i.grid_y * i.grid_z) == (i.splits, i.tiles)
+        if (num_kb, tiles) in want:
+            assert (i.splits, i.kb_per_split) == want[(num_kb, tiles)], (shape, i.splits, i.kb_per_split)
+        s, k = i.splits, i.kb_per_split
         assert s >= 1 and (s - 1) * k < num_kb <= s * k
         if tiles <= 148 and num_kb >= 148 // tiles:
             assert tiles * s <= 148                 # one wave of one-CTA-per-SM blocks whenever the work allows it
     # ignoring the epilogue cost (the first version's behaviour) splits further
-    assert plan(338, 24, epi=0)[0] > plan(338, 24)[0]
+    d = _wgrad_desc(32, 26, 26, 256, 256, 3, 1)
+    assert _wgrad_schedule(d, YB_WGRAD_EPI="0").splits > _wgrad_schedule(d).splits
     with pytest.raises(Exception):
-        plan(0, 1)
+        _wgrad_schedule(_wgrad_desc(1, 8, 8, 48, 64, 1, 1))      # cin not a multiple of 32
+    with pytest.raises(Exception):
+        _wgrad_schedule(_wgrad_desc(1, 8, 8, 64, 64, 1, 1), sms=0)
+
+
+def test_wgrad_schedule_kernel_choice_and_ring_depth():
+    """bnw / tp / stages of the five kernel instantiations: (128, 1) for 1x1 with cin % 128 == 0, one kernel row of
+    taps for 3x3 unless YB_WGRAD_TP=1, and the ring depth that 192 KB of stages allows (at most 8)."""
+    cases = [((1, 16, 16, 256, 64, 1, 1), {}, (128, 1, 6)),
+             ((1, 16, 16, 64, 64, 1, 1), {}, (64, 1, 8)),
+             ((1, 16, 16, 96, 64, 1, 1), {}, (32, 1, 8)),
+             ((1, 16, 16, 128, 64, 3, 1), {}, (64, 3, 4)),
+             ((1, 16, 16, 32, 64, 3, 2), {}, (32, 3, 6)),
+             ((1, 16, 16, 128, 64, 3, 1), {"YB_WGRAD_TP": "1"}, (64, 1, 8)),
+             ((1, 16, 16, 32, 64, 3, 1), {"YB_WGRAD_TP": "1"}, (32, 1, 8))]
+    for shape, opts, want in cases:
+        i = _wgrad_schedule(_wgrad_desc(*shape), **opts)
+        assert (i.bnw, i.tp, i.stages) == want, (shape, opts)
+        n, h, w, cin, cout, k, s = shape
+        assert i.grid_y == k * k // i.tp * (cin // i.bnw) and i.grid_z == -(-cout // 128)
+
+
+def test_wgrad_schedule_forced_splits_clamp():
+    """YB_WGRAD_SPLITS=N forces the split count, clamped to [1, num_kb]: kb_per_split = ceil(num_kb / N) and the
+    effective count is ceil(num_kb / kb_per_split)."""
+    d = _wgrad_desc(2, 20, 16, 64, 128, 3, 1)           # 640 pixels = 10 blocks
+    assert _wgrad_schedule(d).num_kb == 10
+    for forced, (kbs, splits) in {"1": (10, 1), "3": (4, 3), "4": (3, 4), "6": (2, 5), "7": (2, 5), "9": (2, 5),
+                                  "10": (1, 10), "11": (1, 10), "100000": (1, 10), "0": (10, 1),
+                                  "-3": (10, 1)}.items():
+        i = _wgrad_schedule(d, YB_WGRAD_SPLITS=forced)
+        assert (i.kb_per_split, i.splits, i.grid_x) == (kbs, splits, splits), (forced, i.kb_per_split, i.splits)
+        assert (i.splits - 1) * i.kb_per_split < i.num_kb <= i.splits * i.kb_per_split
+    # the forced count overrides the cost model (and the SM count) but not the tile decomposition
+    big = _wgrad_desc(32, 208, 208, 64, 32, 1, 1)
+    i = _wgrad_schedule(big, sms=4, YB_WGRAD_SPLITS="1000")
+    assert (i.splits, i.kb_per_split, i.tiles) == (984, 22, 1)       # 21632 blocks: ceil(21632 / 1000) = 22 per split
+    assert _wgrad_schedule(big, YB_WGRAD_SPLITS="1000", YB_WGRAD_TP="1").tiles == 1

@@ -43,6 +43,11 @@ class ConvSchedule(C.Structure):   # yb_conv_schedule_info
                                    "num_m_tiles", "num_n_tiles", "grid")]
 
 
+class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info
+    _fields_ = [(n, i32) for n in ("bnw", "tp", "stages", "num_kb", "kb_per_split", "splits", "tiles", "grid_x",
+                                   "grid_y", "grid_z")]
+
+
 class LayerInfo(C.Structure):
     _fields_ = [(n, i32) for n in ("index", "cin", "cout", "ksize", "stride", "has_bn", "in_h", "in_w", "out_h",
                                    "out_w", "is_head", "scope_index", "upsample2x")]
@@ -85,7 +90,7 @@ _SIGS = {
     "yb_conv2d_dgrad_s2": ([vp, vp, i32, i32, vp, vp, i32, vp, i32, vp], i32),
     "yb_bn_finalize": ([vp, vp, C.c_long, i32, vp, vp, f32, f32, vp, vp, vp, vp, vp, vp, vp], i32),
     "yb_bn_act_apply": ([vp, C.c_long, vp, vp, vp, C.c_long, vp, C.c_long, i32, i32, i32, i32, i32, i32, i32, vp], i32),
-    "yb_wgrad_split_plan": ([C.c_long, C.c_long, i32, i32, C.POINTER(C.c_long), C.POINTER(C.c_long)], i32),
+    "yb_wgrad_schedule": ([C.POINTER(ConvDesc), i32, C.POINTER(WgradSchedule)], i32),
     "yb_bn_stats_act_apply": ([vp, C.c_long, vp, vp, vp, vp, f32, f32, vp, vp, vp, vp, vp, vp, vp, C.c_long, vp, C.c_long,
                                i32, i32, i32, i32, i32, i32, i32, vp], i32),
     "yb_bn_bwd_reduce_workspace_bytes": ([C.POINTER(sz)], i32),

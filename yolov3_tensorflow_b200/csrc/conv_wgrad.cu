@@ -242,48 +242,76 @@ long wgrad_pick_splits(long num_kb, long tiles, long sms, long epi_blocks) {
   return splits;
 }
 
+// Operand-ring depth of the kernel instantiation a (BNW, TP) pair runs.
+static int wgrad_stages(int bnw, int tp) {
+  if (bnw == 128) return WCfg<128, 1>::STAGES;
+  if (bnw == 64) return tp == 3 ? WCfg<64, 3>::STAGES : WCfg<64, 1>::STAGES;
+  return tp == 3 ? WCfg<32, 3>::STAGES : WCfg<32, 1>::STAGES;
+}
+
 }  // namespace yb
 
 using namespace yb;
 
-// host-only view of the split selection (tests): tiles = tap groups x ci chunks x co tiles of the layer
-extern "C" int yb_wgrad_split_plan(long num_pixel_blocks, long tiles, int sms, int epi_blocks, long* splits,
-                                   long* blocks_per_split) {
-  YB_REQUIRE(num_pixel_blocks > 0 && tiles > 0 && sms > 0 && epi_blocks >= 0 && splits && blocks_per_split,
-             "wgrad_split_plan: bad argument");
-  const long s = wgrad_pick_splits(num_pixel_blocks, tiles, sms, epi_blocks);
-  *blocks_per_split = (num_pixel_blocks + s - 1) / s;
-  *splits = (num_pixel_blocks + *blocks_per_split - 1) / *blocks_per_split;
+// Host-only: the kernel and grid yb_conv2d_wgrad launches for `d` on a device with sm_count SMs, with the current options
+// (YB_WGRAD_TP, YB_WGRAD_EPI, YB_WGRAD_SPLITS).  yb_conv2d_wgrad calls it with the device's SM count.
+extern "C" int yb_wgrad_schedule(const yb_conv_desc* d, int sm_count, yb_wgrad_schedule_info* info) {
+  YB_REQUIRE(d && info && sm_count > 0, "wgrad_schedule: bad argument");
+  YB_REQUIRE(d->ksize == 1 || d->ksize == 3, "wgrad: ksize must be 1 or 3");
+  YB_REQUIRE(d->stride == 1 || d->stride == 2, "wgrad: stride must be 1 or 2");
+  YB_REQUIRE(d->cin > 0 && d->cin % 32 == 0, "wgrad: cin must be a positive multiple of 32 (got %d)", d->cin);
+  YB_REQUIRE(d->cout > 0 && d->n > 0 && d->h >= d->stride && d->w >= d->stride, "wgrad: empty problem");
+  YB_REQUIRE(d->dtype == YB_F16 || d->dtype == YB_BF16, "wgrad: dtype must be f16 or bf16");
+  const long P = (long)d->n * (d->h / d->stride) * (d->w / d->stride);
+  const long num_kb = ceil_div(P, WG_BKP);
+  YB_REQUIRE(num_kb <= 0x7fffffff, "wgrad: too many output pixels");
+  const int taps = d->ksize * d->ksize;
+  // 3x3 convs accumulate one kernel row (3 taps) per CTA, at most 64 input channels per tap: 3 x 64 accumulator columns
+  // are 96 registers per thread.  1x1 convs have one tap and take up to 128 channels.
+  const int bnw = taps == 1 && d->cin % 128 == 0 ? 128 : (d->cin % 64 == 0 ? 64 : 32);
+  const char* tpf = opt("YB_WGRAD_TP");     // "1": one tap per CTA (A/B testing)
+  const int tp = (taps == 1 || (tpf && tpf[0] == '1')) ? 1 : 3;
+  const int tap_groups = taps / tp;
+  const int n_chunks = d->cin / bnw;
+  const int co_tiles = ceil_div(d->cout, WG_BM);
+  const long tiles = (long)tap_groups * n_chunks * co_tiles;
+  long splits;
+  if (opt("YB_WGRAD_SPLITS")[0]) {          // forced split count (tests: deep rings, short last splits)
+    splits = opt_int("YB_WGRAD_SPLITS", 1);
+    splits = splits < 1 ? 1 : (splits > num_kb ? num_kb : splits);
+  } else {
+    splits = wgrad_pick_splits(num_kb, tiles, sm_count, opt_int("YB_WGRAD_EPI", 40));
+  }
+  const long kb_per_split = ceil_div(num_kb, splits);
+  splits = ceil_div(num_kb, kb_per_split);
+  info->bnw = bnw;
+  info->tp = tp;
+  info->stages = wgrad_stages(bnw, tp);
+  info->num_kb = (int)num_kb;
+  info->kb_per_split = (int)kb_per_split;
+  info->splits = (int)splits;
+  info->tiles = (int)tiles;
+  info->grid_x = (int)splits;
+  info->grid_y = tap_groups * n_chunks;
+  info->grid_z = co_tiles;
   return YB_OK;
 }
 
 extern "C" int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void* dz, int dz_ld, int dz_dilated,
                                float* dw, void* stream) {
   YB_REQUIRE(d && x && dz && dw, "wgrad: null pointer");
-  YB_REQUIRE(d->ksize == 1 || d->ksize == 3, "wgrad: ksize must be 1 or 3");
-  YB_REQUIRE(d->stride == 1 || d->stride == 2, "wgrad: stride must be 1 or 2");
-  YB_REQUIRE(d->cin % 32 == 0, "wgrad: cin must be a multiple of 32 (got %d)", d->cin);
-  YB_REQUIRE(d->dtype == YB_F16 || d->dtype == YB_BF16, "wgrad: dtype must be f16 or bf16");
+  yb_wgrad_schedule_info s;
+  { const int rc = yb_wgrad_schedule(d, num_sms(), &s); if (rc) return rc; }
   YB_REQUIRE(dz_ld >= d->cout && dz_ld % 8 == 0 && d->in_ld % 8 == 0, "wgrad: bad leading dimensions");
   const int ho = d->h / d->stride, wo = d->w / d->stride;
   WgradParams p;
   p.P = (long)d->n * ho * wo; p.ho = ho; p.wo = wo;
   p.cin = d->cin; p.cout = d->cout; p.ksize = d->ksize; p.stride = d->stride; p.pad = d->ksize / 2;
-  p.num_kb = ceil_div(p.P, WG_BKP);
-  const int taps = d->ksize * d->ksize;
-  // 3x3 convs accumulate one kernel row (3 taps) per CTA, at most 64 input channels per tap: 3 x 64 accumulator columns
-  // are 96 registers per thread.  1x1 convs have one tap and take up to 128 channels.
-  const int bnw = taps == 1 && d->cin % 128 == 0 ? 128 : (d->cin % 64 == 0 ? 64 : 32);
-  p.n_chunks = d->cin / bnw;
+  p.num_kb = s.num_kb;
+  p.kb_per_split = s.kb_per_split;
+  p.n_chunks = d->cin / s.bnw;
   p.dw = dw;
-  const char* tpf = opt("YB_WGRAD_TP");     // "1": one tap per CTA (A/B testing)
-  const int tp = (taps == 1 || (tpf && tpf[0] == '1')) ? 1 : 3;
-  const int tap_groups = taps / tp;
-  const int co_tiles = ceil_div(d->cout, WG_BM);
-  const long tiles = (long)tap_groups * p.n_chunks * co_tiles;
-  long splits = wgrad_pick_splits(p.num_kb, tiles, num_sms(), opt_int("YB_WGRAD_EPI", 40));
-  p.kb_per_split = ceil_div(p.num_kb, splits);
-  splits = ceil_div(p.num_kb, p.kb_per_split);
+  const int bnw = s.bnw, tp = s.tp;
   CUtensorMap tmA, tmB;
   p.a_dilated = dz_dilated ? 1 : 0;
   int rc;
@@ -297,7 +325,7 @@ extern "C" int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void*
   rc = make_tmap_im2col_px(&tmB, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->ksize, d->stride, p.pad,
                            bnw < 64 ? bnw : 64, WG_BKP);
   if (rc) return rc;
-  dim3 grid((unsigned)splits, (unsigned)(tap_groups * p.n_chunks), (unsigned)co_tiles);
+  dim3 grid((unsigned)s.grid_x, (unsigned)s.grid_y, (unsigned)s.grid_z);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define YB_WG(T)                                                                       \
   if (bnw == 128) return launch_wgrad<T, 128, 1>(tmA, tmB, p, grid, st);              \
