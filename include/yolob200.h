@@ -167,6 +167,27 @@ int yb_letterbox_params(int src_h, int src_w, int new_h, int new_w, double* resi
                         int* dh, int* dw);
 int yb_letterbox_normalize(const uint8_t* bgr, int src_h, int src_w, long src_pitch_bytes, int new_h, int new_w,
                            float* out_rgb, void* stream);
+/* The evaluation input path for a batch of images of different sizes, in one launch: letterbox_resize or a plain
+ * stretch (cv2.resize to the target), nearest (interp 0) or OpenCV's bilinear (interp 1), then BGR->RGB + float32 / 255
+ * (parse_data(mode='val') at utils/data_utils.py:166-176, eval.py, test_single_image.py:39-46).
+ *   images     device, n uint8 BGR images packed in images_bytes bytes
+ *   desc_host  host int64 [n, 4]: (byte offset, h, w, row pitch in bytes) per image, validated here;
+ *   desc_dev   the same table on the device (8-byte aligned), read by the kernel: the two must hold the same values
+ *   out_rgb    float32 [n, new_h, new_w, 3]; letterbox borders are 128 / 255
+ *   params     optional float64 [n, 4]: letterbox (resize_ratio, dw, dh, 1), stretch (w / new_w, h / new_h, 0, 0)
+ * Bit-exact vs cv2.resize of OpenCV 4.13 (INTER_LINEAR is not bit-stable across OpenCV builds).  n <= 65535, image
+ * sides in 1..2^20, and a letterbox whose int() truncation leaves an empty resize is rejected. */
+int yb_resize_batch(const uint8_t* images, long images_bytes, const int64_t* desc_host, const int64_t* desc_dev, int n,
+                    int new_h, int new_w, int letterbox, int interp, float* out_rgb, double* params, void* stream);
+/* resize_with_bbox's box transform (utils/data_aug.py:301-318), in place, float32 in the reference's order:
+ * boxes float32 [n, vmax, box_ld] (columns 0-3 x_min, y_min, x_max, y_max; the rest untouched), counts int32 [n],
+ * desc_dev the yb_resize_batch descriptor table of the same images. */
+int yb_resize_boxes(float* boxes, const int32_t* counts, int n, int vmax, int box_ld, const int64_t* desc_dev, int new_h,
+                    int new_w, int letterbox, void* stream);
+/* Detections back to source-image coordinates (test_single_image.py:64-70), in place: boxes float32 [n, slots, box_ld]
+ * (yb_net_detect's per-image output slots), the first counts[i] of image i mapped with params row i of yb_resize_batch. */
+int yb_restore_boxes(float* boxes, const int32_t* counts, int n, int slots, int box_ld, const double* params,
+                     void* stream);
 
 /* Weight repack (utils/misc_utils.py:114-123 does (Cout,Cin,kh,kw) -> HWIO on the host):
  * src float32 in `layout` -> dst `dtype` (or float32) OHWI [cout_pad,k,k,cin], rows >= cout zeroed. */

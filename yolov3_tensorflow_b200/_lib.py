@@ -78,6 +78,9 @@ _SIGS = {
     "yb_process_box": ([vp, vp, vp, i32, i32, i32, i32, i32, C.POINTER(f32), vp, vp, vp, vp], i32),
     "yb_letterbox_params": ([i32, i32, i32, i32, C.POINTER(C.c_double), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
     "yb_letterbox_normalize": ([vp, i32, i32, C.c_long, i32, i32, vp, vp], i32),
+    "yb_resize_batch": ([vp, C.c_long, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
+    "yb_resize_boxes": ([vp, vp, i32, i32, i32, vp, i32, i32, i32, vp], i32),
+    "yb_restore_boxes": ([vp, vp, i32, i32, i32, vp, vp], i32),
     "yb_pack_conv_weights": ([vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
     "yb_pack_conv_weights_e4m3": ([vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
     "yb_amax": ([vp, C.c_long, C.c_long, i32, i32, vp, vp], i32),

@@ -125,6 +125,158 @@ letterbox_kernel(const uint8_t* __restrict__ src, int sh, int sw, long src_pitch
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The evaluation input path for a batch of images of different sizes: parse_data(mode='val') (utils/data_utils.py:166-
+// 176: resize_with_bbox(interp=1) + BGR->RGB + / 255), eval.py / eval_voc.py (stretch), test_single_image.py (stretch
+// or letterbox, then the detections mapped back to the source image).
+// ---------------------------------------------------------------------------------------------------------------------
+
+static constexpr int RESIZE_MAX_SIDE = 1 << 20;      // source image sides; keeps every index product in int32
+
+// letterbox_resize's scalars (utils/data_aug.py:279-289); stretch is the whole target with no border.  Host and device
+// share this so the box kernels see exactly the geometry the host validated.
+struct ResizeGeom {
+  double ratio;        // letterbox resize_ratio
+  int rh, rw, dh, dw;  // resized size and border offsets
+};
+__host__ __device__ inline ResizeGeom resize_geom(int sh, int sw, int nh, int nw, int letterbox) {
+  ResizeGeom g;
+  if (letterbox) {
+    const double a = (double)nw / (double)sw, b = (double)nh / (double)sh;
+    g.ratio = a < b ? a : b;
+    g.rw = (int)(g.ratio * sw);
+    g.rh = (int)(g.ratio * sh);
+    g.dw = (int)((nw - g.rw) / 2.0);
+    g.dh = (int)((nh - g.rh) / 2.0);
+  } else {
+    g.ratio = 0.0; g.rh = nh; g.rw = nw; g.dh = 0; g.dw = 0;
+  }
+  return g;
+}
+
+// OpenCV's linear source coordinate: f = (float)((d + 0.5) * scale - 0.5), s = floor(f), f -= s (resize.cpp,
+// resizeGeneric setup).  Double ops spelled _rn so no FMA is contracted.
+struct LinTap { int s; float f; };
+__device__ __forceinline__ LinTap linear_tap(int d, double scale) {
+  float f = __double2float_rn(__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5));
+  const int s = (int)floorf(f);
+  f = __fsub_rn(f, (float)s);
+  return {s, f};
+}
+// saturate_cast<short>(w * INTER_RESIZE_COEF_SCALE): round half to even
+__device__ __forceinline__ int coef11(float w) { return __float2int_rn(__fmul_rn(w, 2048.f)); }
+
+struct ImgDesc { long off; int h, w; long pitch; };   // one row of the int64 [n, 4] descriptor table
+
+// grid (blocks per image, n): block (bx, img) covers pixels bx, bx + gridDim.x, ... (x 256) of output image img.
+// letterbox_resize / cv2.resize(interp) -> cvtColor(BGR2RGB) -> float32 / 255.
+__global__ void __launch_bounds__(256)
+resize_batch_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ desc, int nh, int nw, int letterbox,
+                    int interp, float* __restrict__ dst, double* __restrict__ params) {
+  __shared__ ImgDesc s_d;
+  __shared__ ResizeGeom s_g;
+  const int img = blockIdx.y;
+  if (threadIdx.x == 0) {
+    const int64_t* d = desc + 4L * img;
+    s_d = {(long)d[0], (int)d[1], (int)d[2], (long)d[3]};
+    s_g = resize_geom(s_d.h, s_d.w, nh, nw, letterbox);
+    if (params && blockIdx.x == 0) {
+      double* p = params + 4L * img;
+      if (letterbox) { p[0] = s_g.ratio; p[1] = s_g.dw; p[2] = s_g.dh; p[3] = 1.0; }
+      else { p[0] = (double)s_d.w / (double)nw; p[1] = (double)s_d.h / (double)nh; p[2] = 0.0; p[3] = 0.0; }
+    }
+  }
+  __syncthreads();
+  const ImgDesc d = s_d;
+  const ResizeGeom g = s_g;
+  const uint8_t* im = src + d.off;
+  // OpenCV: inv_scale = dsize / ssize; scale = 1. / inv_scale (resizeNN's ifx / resizeGeneric's scale_x alike)
+  const double scx = 1.0 / ((double)g.rw / (double)d.w), scy = 1.0 / ((double)g.rh / (double)d.h);
+  const long total = (long)nh * nw;
+  float* out = dst + (long)img * total * 3;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int y = (int)(i / nw), x = (int)(i - (long)y * nw);
+    int r = 128, gr = 128, b = 128;                 // np.full(..., 128, np.uint8)
+    const int ry = y - g.dh, rx = x - g.dw;
+    if (ry >= 0 && ry < g.rh && rx >= 0 && rx < g.rw) {
+      if (interp == 0) {                            // resizeNN, as letterbox_kernel
+        const int sy = min((int)floor(ry * scy), d.h - 1);
+        const int sx = min((int)floor(rx * scx), d.w - 1);
+        const uint8_t* px = im + (long)sy * d.pitch + sx * 3;
+        b = px[0]; gr = px[1]; r = px[2];
+      } else {
+        // x: a source column outside [0, w - 1) takes that border pixel with weight 1 (fraction zeroed)
+        LinTap tx = linear_tap(rx, scx);
+        if (tx.s < 0) { tx.s = 0; tx.f = 0.f; }
+        if (tx.s >= d.w - 1) { tx.s = d.w - 1; tx.f = 0.f; }
+        const int cx0 = coef11(__fsub_rn(1.f, tx.f)), cx1 = coef11(tx.f);
+        const int x0 = tx.s * 3, x1 = min(tx.s + 1, d.w - 1) * 3;
+        // y: the fraction is kept, only the two row indices are clamped
+        const LinTap ty = linear_tap(ry, scy);
+        const int cy0 = coef11(__fsub_rn(1.f, ty.f)), cy1 = coef11(ty.f);
+        const uint8_t* r0 = im + (long)min(max(ty.s, 0), d.h - 1) * d.pitch;
+        const uint8_t* r1 = im + (long)min(max(ty.s + 1, 0), d.h - 1) * d.pitch;
+        int v[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const int h0 = r0[x0 + c] * cx0 + r0[x1 + c] * cx1;          // horizontal pass, int32
+          const int h1 = r1[x0 + c] * cx0 + r1[x1 + c] * cx1;
+          // vertical pass as OpenCV's SIMD VResizeLinearVec_32s8u: (h >> 4) * c as int16 mul_hi, +2 >> 2, saturate
+          const int t = (((h0 >> 4) * cy0) >> 16) + (((h1 >> 4) * cy1) >> 16);
+          v[c] = min(max((t + 2) >> 2, 0), 255);
+        }
+        b = v[0]; gr = v[1]; r = v[2];
+      }
+    }
+    float* o = out + i * 3;
+    o[0] = __fdiv_rn((float)r, 255.f); o[1] = __fdiv_rn((float)gr, 255.f); o[2] = __fdiv_rn((float)b, 255.f);
+  }
+}
+
+// resize_with_bbox's box lines (utils/data_aug.py:301-318) in place, float32 in the reference's order; the Python
+// float / int scalars act as float32 under numpy 2 (NEP 50).  One thread per box slot.
+__global__ void __launch_bounds__(256)
+resize_boxes_kernel(float* __restrict__ boxes, const int32_t* __restrict__ counts, int n, int vmax, int ld,
+                    const int64_t* __restrict__ desc, int nh, int nw, int letterbox) {
+  const long t = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (t >= (long)n * vmax) return;
+  const int img = (int)(t / vmax), j = (int)(t - (long)img * vmax);
+  if (j >= min(counts[img], vmax)) return;
+  const int sh = (int)desc[4L * img + 1], sw = (int)desc[4L * img + 2];
+  float* b = boxes + t * ld;
+  if (letterbox) {                                  // bbox * resize_ratio + dw / dh
+    const ResizeGeom g = resize_geom(sh, sw, nh, nw, 1);
+    const float r = __double2float_rn(g.ratio), dw = (float)g.dw, dh = (float)g.dh;
+    b[0] = __fadd_rn(__fmul_rn(b[0], r), dw); b[2] = __fadd_rn(__fmul_rn(b[2], r), dw);
+    b[1] = __fadd_rn(__fmul_rn(b[1], r), dh); b[3] = __fadd_rn(__fmul_rn(b[3], r), dh);
+  } else {                                          // bbox / ori_width * new_width
+    const float fw = (float)sw, fh = (float)sh, fnw = (float)nw, fnh = (float)nh;
+    b[0] = __fmul_rn(__fdiv_rn(b[0], fw), fnw); b[2] = __fmul_rn(__fdiv_rn(b[2], fw), fnw);
+    b[1] = __fmul_rn(__fdiv_rn(b[1], fh), fnh); b[3] = __fmul_rn(__fdiv_rn(b[3], fh), fnh);
+  }
+}
+
+// test_single_image.py:64-70 in place: letterbox (b - dw) / resize_ratio, stretch b * (ori / new), float32.
+__global__ void __launch_bounds__(256)
+restore_boxes_kernel(float* __restrict__ boxes, const int32_t* __restrict__ counts, int n, int slots, int ld,
+                     const double* __restrict__ params) {
+  const long t = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (t >= (long)n * slots) return;
+  const int img = (int)(t / slots), j = (int)(t - (long)img * slots);
+  if (j >= min(counts[img], slots)) return;
+  const double* p = params + 4L * img;
+  float* b = boxes + t * ld;
+  if (p[3] != 0.0) {
+    const float r = __double2float_rn(p[0]), dw = __double2float_rn(p[1]), dh = __double2float_rn(p[2]);
+    b[0] = __fdiv_rn(__fsub_rn(b[0], dw), r); b[2] = __fdiv_rn(__fsub_rn(b[2], dw), r);
+    b[1] = __fdiv_rn(__fsub_rn(b[1], dh), r); b[3] = __fdiv_rn(__fsub_rn(b[3], dh), r);
+  } else {
+    const float fx = __double2float_rn(p[0]), fy = __double2float_rn(p[1]);
+    b[0] = __fmul_rn(b[0], fx); b[2] = __fmul_rn(b[2], fx);
+    b[1] = __fmul_rn(b[1], fy); b[3] = __fmul_rn(b[3], fy);
+  }
+}
+
 }  // namespace yb
 
 using namespace yb;
@@ -190,6 +342,62 @@ extern "C" int yb_letterbox_normalize(const uint8_t* bgr, int src_h, int src_w, 
   if (blocks > cap) blocks = cap;
   letterbox_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(bgr, src_h, src_w, src_pitch_bytes, rh, rw, dh,
                                                                              dw, new_h, new_w, ify, ifx, out_rgb);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_resize_batch(const uint8_t* images, long images_bytes, const int64_t* desc_host,
+                               const int64_t* desc_dev, int n, int new_h, int new_w, int letterbox, int interp,
+                               float* out_rgb, double* params, void* stream) {
+  YB_REQUIRE(images && desc_host && desc_dev && out_rgb, "resize_batch: null pointer");
+  YB_REQUIRE(((uintptr_t)desc_dev & 7) == 0 && ((uintptr_t)params & 7) == 0,
+             "resize_batch: the descriptor table and params must be 8-byte aligned");
+  YB_REQUIRE(n > 0 && n <= 65535, "resize_batch: n must be in 1..65535 (got %d)", n);
+  YB_REQUIRE(new_h > 0 && new_w > 0, "resize_batch: target size must be positive (got %dx%d)", new_w, new_h);
+  YB_REQUIRE(letterbox == 0 || letterbox == 1, "resize_batch: letterbox must be 0 or 1 (got %d)", letterbox);
+  YB_REQUIRE(interp == 0 || interp == 1, "resize_batch: interp must be 0 (nearest) or 1 (linear), got %d", interp);
+  for (int i = 0; i < n; ++i) {
+    const int64_t off = desc_host[4L * i], h = desc_host[4L * i + 1], w = desc_host[4L * i + 2], pitch = desc_host[4L * i + 3];
+    YB_REQUIRE(h > 0 && w > 0 && h <= RESIZE_MAX_SIDE && w <= RESIZE_MAX_SIDE,
+               "resize_batch: image %d has size %lldx%lld", i, (long long)w, (long long)h);
+    YB_REQUIRE(off >= 0 && pitch >= 3 * w && off + (h - 1) * pitch + 3 * w <= images_bytes,
+               "resize_batch: image %d (offset %lld, pitch %lld) lies outside the %ld-byte buffer", i, (long long)off,
+               (long long)pitch, images_bytes);
+    const ResizeGeom g = resize_geom((int)h, (int)w, new_h, new_w, letterbox);
+    YB_REQUIRE(g.rh > 0 && g.rw > 0, "resize_batch: image %d (%lldx%lld) letterboxes to an empty resize", i,
+               (long long)w, (long long)h);
+  }
+  const long total = (long)new_h * new_w;
+  long bx = (total + 255) / 256;
+  const long cap = ((long)num_sms() * 16 + n - 1) / n;  // about 16 CTAs per SM over the batch, then grid-stride
+  if (bx > cap) bx = cap;
+  resize_batch_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      images, desc_dev, new_h, new_w, letterbox, interp, out_rgb, params);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_resize_boxes(float* boxes, const int32_t* counts, int n, int vmax, int box_ld, const int64_t* desc_dev,
+                               int new_h, int new_w, int letterbox, void* stream) {
+  YB_REQUIRE(boxes && counts && desc_dev, "resize_boxes: null pointer");
+  YB_REQUIRE(((uintptr_t)desc_dev & 7) == 0, "resize_boxes: the descriptor table must be 8-byte aligned");
+  YB_REQUIRE(n > 0 && vmax > 0 && box_ld >= 4, "resize_boxes: bad shape (n %d, vmax %d, box_ld %d)", n, vmax, box_ld);
+  YB_REQUIRE(new_h > 0 && new_w > 0 && (letterbox == 0 || letterbox == 1), "resize_boxes: bad target or mode");
+  const long total = (long)n * vmax;
+  resize_boxes_kernel<<<ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      boxes, counts, n, vmax, box_ld, desc_dev, new_h, new_w, letterbox);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_restore_boxes(float* boxes, const int32_t* counts, int n, int slots, int box_ld, const double* params,
+                                void* stream) {
+  YB_REQUIRE(boxes && counts && params, "restore_boxes: null pointer");
+  YB_REQUIRE(((uintptr_t)params & 7) == 0, "restore_boxes: params must be 8-byte aligned");
+  YB_REQUIRE(n > 0 && slots > 0 && box_ld >= 4, "restore_boxes: bad shape (n %d, slots %d, box_ld %d)", n, slots, box_ld);
+  const long total = (long)n * slots;
+  restore_boxes_kernel<<<ceil_div(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(boxes, counts, n, slots,
+                                                                                            box_ld, params);
   YB_CUDA(cudaGetLastError());
   return YB_OK;
 }

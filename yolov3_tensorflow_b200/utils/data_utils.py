@@ -1,7 +1,9 @@
 """utils/data_utils.py of the reference, the part on the hot path's input side: `process_box` (ground-truth lists ->
 y_true_13 / _26 / _52, utils/data_utils.py:51-115) as ONE device call for a whole batch (libyolob200.so: yb_process_box).
 The box lists (24 B per box) are what crosses PCIe; the 3.66 MB-per-image tensors are built in HBM, bit-identical to
-the reference's numpy loop (list order decides collisions: the last box of a slot wins, class bits accumulate)."""
+the reference's numpy loop (list order decides collisions: the last box of a slot wins, class bits accumulate).
+`val_batch` is parse_data(mode='val') for a whole batch: images resized from uint8 on the device, boxes transformed
+the same way, then process_box_batch."""
 from __future__ import annotations
 
 import numpy as np
@@ -54,6 +56,41 @@ def process_box_batch(boxes, labels, counts, img_size, class_num, anchors, devic
         check(lib.yb_process_box(ptr(b), ptr(l), ptr(c), n, vmax, W, H, int(class_num), _lib.fptr(anchors.reshape(-1)),
                                  ptr(out[0]), ptr(out[1]), ptr(out[2]), stream_handle()), "yb_process_box")
     return out[0], out[1], out[2]
+
+
+def val_batch(images, boxes_list, labels_list, img_size, class_num, anchors, letterbox_resize=True, device=None):
+    """parse_data(mode='val') (utils/data_utils.py:166-182) for a batch, on the device: resize_with_bbox(interp=1,
+    letterbox=letterbox_resize) + cvtColor(BGR2RGB) + float32 / 255 for the images (one H2D copy of the uint8 pixels,
+    one launch), the same box transform, then process_box_batch.
+      images: uint8 [H, W, 3] BGR images of any sizes; boxes_list: per image float32 [V, 4] (x_min, y_min, x_max,
+      y_max in source pixels) or [V, 5] with a mix-up weight (1 when absent, as parse_data adds); labels_list: per
+      image [V] ints; img_size: [W, H], multiples of 32.
+    -> (x [n, H, W, 3], y_true_13, y_true_26, y_true_52), float32 on the device, no host synchronisation."""
+    from .data_aug import PackedImages, _resize_packed
+    n = len(images)
+    if n != len(boxes_list):
+        raise ValueError(f"val_batch: {n} images but {len(boxes_list)} box arrays")
+    bl = []
+    for i, b in enumerate(boxes_list):
+        b = np.asarray(b, np.float32)
+        b = b.reshape(-1, b.shape[-1] if b.size else 4)
+        if b.shape[1] == 4:
+            b = np.concatenate([b, np.ones((len(b), 1), np.float32)], 1)
+        if b.shape[1] != 5:
+            raise ValueError(f"val_batch: image {i}: boxes must be [V, 4] or [V, 5], got {b.shape}")
+        bl.append(b)
+    W, H = int(img_size[0]), int(img_size[1])
+    packed = PackedImages(images, device)
+    dev = packed.device
+    x, _ = _resize_packed(packed, W, H, letterbox_resize, 1)
+    hb, hl, hc = pack_gt(bl, labels_list)
+    b = hb.to(dev, non_blocking=True)
+    c = hc.to(dev, non_blocking=True)
+    with torch.cuda.device(dev):
+        check(lib.yb_resize_boxes(ptr(b), ptr(c), n, int(b.shape[1]), 5, ptr(packed.desc_dev), H, W,
+                                  int(bool(letterbox_resize)), stream_handle()), "yb_resize_boxes")
+    y13, y26, y52 = process_box_batch(b, hl, c, [W, H], class_num, anchors, device=dev)
+    return x, y13, y26, y52
 
 
 def process_box(boxes, labels, img_size, class_num, anchors):
