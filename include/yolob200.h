@@ -265,6 +265,22 @@ int yb_bn_stats_act_apply(const void* z, long z_ld, const float* sum, const floa
                           float* scale, float* shift, float* save_mean, float* save_invstd, const void* res,
                           long res_ld, void* out, long out_ld, int n, int h, int w, int c, int dtype, int leaky,
                           int upsample2x, void* stream);
+/* Host-only: the launch shape of the BN streaming kernels (yb_bn_act_apply, yb_bn_stats_act_apply, yb_bn_bwd_reduce,
+ * yb_bn_bwd_apply) for `rows` = n*h*w rows of c channels on a device with sm_count SMs, with the current options
+ * (YB_BN_CPT).  A thread owns cpt consecutive channels (cv = c / cpt channel vectors per row) of one of `lanes` =
+ * 256 / cv row lanes and walks its rows r unrolled (rows lane, lane + lanes, ...); block b owns rows
+ * [b * rows_per_block, min((b + 1) * rows_per_block, rows)), rows_per_block a multiple of lanes chosen so that
+ * grid <= sm_count * blocks_per_sm (one wave of co-resident blocks). */
+typedef struct yb_bn_schedule_info {
+  int cpt;             /* channels per thread: 8, or 4 (YB_BN_CPT=4, 32 <= c <= 1024) */
+  int r;               /* rows in flight per thread (unroll)                           */
+  int blocks_per_sm;
+  int cv;              /* channel vectors per row                                      */
+  int lanes;           /* row lanes per 256-thread block                               */
+  long rows_per_block;
+  int grid;
+} yb_bn_schedule_info;
+int yb_bn_schedule(long rows, int c, int sm_count, yb_bn_schedule_info* info);
 /* dgamma/dbeta (fp32 [c], overwritten) from dA (gradient w.r.t. the layer output; upsample2x: summed over the
  * 4 copies) and the saved z.  workspace: NULL (atomic accumulation) or yb_bn_bwd_reduce_workspace_bytes() bytes,
  * zero-initialised once (two-stage deterministic reduction, no same-address atomics). */

@@ -48,6 +48,11 @@ class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info
                                    "grid_y", "grid_z")]
 
 
+class BnSchedule(C.Structure):     # yb_bn_schedule_info
+    _fields_ = [(n, i32) for n in ("cpt", "r", "blocks_per_sm", "cv", "lanes")] + [("rows_per_block", C.c_long),
+                                                                                    ("grid", i32)]
+
+
 class LayerInfo(C.Structure):
     _fields_ = [(n, i32) for n in ("index", "cin", "cout", "ksize", "stride", "has_bn", "in_h", "in_w", "out_h",
                                    "out_w", "is_head", "scope_index", "upsample2x")]
@@ -96,6 +101,7 @@ _SIGS = {
     "yb_wgrad_schedule": ([C.POINTER(ConvDesc), i32, C.POINTER(WgradSchedule)], i32),
     "yb_bn_stats_act_apply": ([vp, C.c_long, vp, vp, vp, vp, f32, f32, vp, vp, vp, vp, vp, vp, vp, C.c_long, vp, C.c_long,
                                i32, i32, i32, i32, i32, i32, i32, vp], i32),
+    "yb_bn_schedule": ([C.c_long, i32, i32, C.POINTER(BnSchedule)], i32),
     "yb_bn_bwd_reduce_workspace_bytes": ([C.POINTER(sz)], i32),
     "yb_bn_bwd_reduce": ([vp, C.c_long, vp, C.c_long, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp], i32),
     "yb_bn_bwd_apply": ([vp, C.c_long, vp, C.c_long, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, C.c_long, vp], i32),

@@ -407,29 +407,28 @@ bn_bwd_apply_kernel(const T* __restrict__ dA, long dA_ld, const T* __restrict__ 
   }
 }
 
-// one balanced wave: at most (SM count) x bps co-resident blocks, every row lane of a block gets >= 1 row
-static StreamGeom stream_geom(long rows, int c, int cpt, int bps, int* grid) {
-  StreamGeom sg;
-  sg.cv = c / cpt;
-  sg.lanes = 256 / sg.cv;
-  if (sg.lanes < 1) sg.lanes = 1;
-  const long blocks = (long)num_sms() * bps;
-  long rpb = (rows + blocks - 1) / blocks;
-  rpb = (rpb + sg.lanes - 1) / sg.lanes * sg.lanes;
-  sg.rows_per_block = rpb;
-  *grid = (int)((rows + rpb - 1) / rpb);
-  return sg;
-}
-static int aligned16(std::initializer_list<const void*> ps) {
-  for (const void* q : ps) if (q && (reinterpret_cast<uintptr_t>(q) & 15)) return 0;
-  return 1;
-}
 // kernel shape: 8 channels per thread (16-byte accesses) unless YB_BN_CPT=4, whose 8-byte accesses double the
 // load/store instructions per byte.
 static int bn_cpt(int c) {
   const char* o = opt("YB_BN_CPT");
   if (c > 1024 || c < 32) return 8;
   return (o && o[0] == '4') ? 4 : 8;
+}
+// the launch shape yb_bn_schedule reports for this device (the callers have validated rows and c)
+static StreamGeom stream_geom(long rows, int c, int* cpt, int* grid) {
+  yb_bn_schedule_info s;
+  yb_bn_schedule(rows, c, num_sms(), &s);
+  StreamGeom sg;
+  sg.cv = s.cv;
+  sg.lanes = s.lanes;
+  sg.rows_per_block = s.rows_per_block;
+  *cpt = s.cpt;
+  *grid = s.grid;
+  return sg;
+}
+static int aligned16(std::initializer_list<const void*> ps) {
+  for (const void* q : ps) if (q && (reinterpret_cast<uintptr_t>(q) & 15)) return 0;
+  return 1;
 }
 
 template <typename T>
@@ -463,6 +462,25 @@ using namespace yb;
   YB_REQUIRE(n > 0 && h > 0 && w > 0 && c >= 8 && c <= 2048 && (c & (c - 1)) == 0, name ": channels must be a power of two in [8, 2048]"); \
   YB_REQUIRE(dtype == YB_F16 || dtype == YB_BF16, name ": dtype must be f16 or bf16");
 
+// one balanced wave: at most (SM count) x bps co-resident blocks, every row lane of a block gets >= 1 row
+extern "C" int yb_bn_schedule(long rows, int c, int sm_count, yb_bn_schedule_info* info) {
+  YB_REQUIRE(info && sm_count > 0 && rows > 0, "bn_schedule: bad argument");
+  YB_REQUIRE(c >= 8 && c <= 2048 && (c & (c - 1)) == 0, "bn_schedule: channels must be a power of two in [8, 2048]");
+  const int cpt = bn_cpt(c);
+  info->cpt = cpt;
+  info->r = cpt == 4 ? 8 : 4;                 // the YB_BN_SHAPES instantiations below
+  info->blocks_per_sm = cpt == 4 ? 3 : 2;
+  info->cv = c / cpt;
+  info->lanes = 256 / info->cv;
+  if (info->lanes < 1) info->lanes = 1;
+  const long blocks = (long)sm_count * info->blocks_per_sm;
+  long rpb = (rows + blocks - 1) / blocks;
+  rpb = (rpb + info->lanes - 1) / info->lanes * info->lanes;
+  info->rows_per_block = rpb;
+  info->grid = (int)((rows + rpb - 1) / rpb);
+  return YB_OK;
+}
+
 extern "C" int yb_bn_finalize(const float* sum, const float* sqsum, long count, int c, const float* gamma,
                               const float* beta, float eps, float decay, float* moving_mean, float* moving_var,
                               float* scale, float* shift, float* save_mean, float* save_invstd, void* stream) {
@@ -488,9 +506,8 @@ static int launch_act_apply(const void* z, long z_ld, const float* scale, const 
                             long res_ld, void* out, long out_ld, int n, int h, int w, int c, int dtype, int leaky,
                             int upsample2x, const BnFin* fin, cudaStream_t st) {
   RowGeom g{(long)n * h * w, h, w, c};
-  int grid;
-  const int cpt = bn_cpt(c);
-  const StreamGeom sg = stream_geom(g.rows, c, cpt, cpt == 4 ? 3 : 2, &grid);
+  int grid, cpt;
+  const StreamGeom sg = stream_geom(g.rows, c, &cpt, &grid);
   BnFin f; memset(&f, 0, sizeof(f));
   int vec = aligned16({scale, shift});
   if (fin) {
@@ -563,9 +580,8 @@ int bn_bwd_reduce_x(const void* dA, long dA_ld, const void* z, long z_ld, const 
   YB_REQUIRE((xg == nullptr) == (xb == nullptr) && (xg == nullptr || workspace), "bn_bwd_reduce: bad exchange slab");
   RowGeom g{(long)n * h * w, h, w, c};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int grid;
-  const int cpt = bn_cpt(c);
-  const StreamGeom sg = stream_geom(g.rows, c, cpt, cpt == 4 ? 3 : 2, &grid);
+  int grid, cpt;
+  const StreamGeom sg = stream_geom(g.rows, c, &cpt, &grid);
   // workspace (zero-initialised once by the caller): [0,256) ticket counter, then per-block partials
   unsigned int* ticket = static_cast<unsigned int*>(workspace);
   float* partial = workspace ? reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + 256) : nullptr;
@@ -605,9 +621,8 @@ int bn_bwd_apply_n(const void* dA, long dA_ld, const void* z, long z_ld, const f
   YB_REQUIRE(count >= (long)n * h * w, "bn_bwd_apply: count must cover the local rows");
   RowGeom g{(long)n * h * w, h, w, c};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int grid;
-  const int cpt = bn_cpt(c);
-  const StreamGeom sg = stream_geom(g.rows, c, cpt, cpt == 4 ? 3 : 2, &grid);
+  int grid, cpt;
+  const StreamGeom sg = stream_geom(g.rows, c, &cpt, &grid);
   const int vec = aligned16({gamma, scale, shift, save_mean, save_invstd, dgamma, dbeta});
 #define YB_APP_LAUNCH(T, CPT, R, BPS)                                                                                  \
   bn_bwd_apply_kernel<T, CPT, R, BPS><<<grid, 256, 0, st>>>((const T*)dA, dA_ld, (const T*)z, z_ld, gamma, scale,      \
