@@ -405,6 +405,23 @@ int yb_net_create(yb_net** net, int class_num, int n, int h, int w, int dtype, i
 int yb_net_destroy(yb_net* net);
 int yb_net_num_layers(const yb_net* net);
 int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* info);
+/* Host-only unless sm_count == 0: the kernel, multicast-cluster shape and persistent grid the forward of a plan
+ * (yb_net_forward / yb_net_detect, current options) launches for `layer`.  sm_count > 0: a device with that many SMs,
+ * max_clusters = sm_count / (cluster_m * cluster_n); sm_count == 0: the current device, max_clusters from
+ * cudaOccupancyMaxActiveClusters for the kernel.  igemm = 0 (all other fields 0): the layer runs the stem or the halo
+ * kernel.  The detection heads are reported as yb_net_forward runs them (unfused). */
+typedef struct yb_layer_schedule_info {
+  int igemm;         /* 1: the implicit-GEMM conv                                                  */
+  int pingpong;      /* 1: ping-pong schedule, 0: cooperative                                       */
+  int cluster_m;     /* CTAs of a cluster along M (each a different m-tile)                         */
+  int cluster_n;     /* CTAs of a cluster along N (ping-pong multicast clusters only)               */
+  int block_m, block_n;
+  int num_m_tiles, num_n_tiles;
+  int units;         /* work units: ceil(num_m_tiles / cluster_m) x num_n_tiles / cluster_n         */
+  int max_clusters;  /* most clusters resident at once                                              */
+  int grid;          /* CTAs launched: a multiple of cluster_m x cluster_n, <= max_clusters of them */
+} yb_layer_schedule_info;
+int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info);
 int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes);
 /* Bind caller-owned arenas (256-byte aligned).  Must be called before set_params/forward.  The PARAMETER arena layout
  * depends only on (class_num, dtype, training): plans of different batch / image sizes may share one parameter arena

@@ -74,7 +74,7 @@ def main():
 
     import torch
     import yolov3_tensorflow_b200 as pkg
-    from yolov3_tensorflow_b200._lib import lib, check, ptr, stream_handle
+    from yolov3_tensorflow_b200._lib import LayerSchedule, lib, check, ptr, stream_handle
     from bench import make_bench_params
 
     for key in ("YB_HALO", "YB_THIN", "YB_STEM_FUSE", "YB_HEAD_STREAM"):
@@ -102,7 +102,11 @@ def main():
         if i == 1:
             flop += 2.0 * B * S * S * 27 * plan.layer_info(0).cout          # the stem's FLOPs run in this launch
         row = dict(layer=i, cin=info.cin, cout=info.cout, k=info.ksize, s=info.stride, hw=info.out_h,
-                   up=info.upsample2x, kernel=kern, gflop=flop / 1e9, ms=0.0)
+                   up=info.upsample2x, kernel=kern, gflop=flop / 1e9, ms=0.0, sched="")
+        if kern == "conv_igemm":               # the plan's schedule: ping-pong / cooperative, multicast cluster shape
+            sc = LayerSchedule()
+            check(lib.yb_net_layer_schedule(plan.handle, i, 0, C.byref(sc)), "yb_net_layer_schedule")
+            row["sched"] = ("pp " if sc.pingpong else "co ") + f"{sc.cluster_m}x{sc.cluster_n}"
         if i > 0:
             for _ in range(3):
                 run(i)
@@ -118,14 +122,14 @@ def main():
         rows.append(row)
 
     print(f"# card: {card()}   SMs: {sms}   batch {B}, {S}x{S}, fp16, {args.reps} reps per layer")
-    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'tiles':>6} {'kb':>4} {'waves':>5}"
-          f" {'ms':>8} {'TFLOP/s':>8}")
+    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'sched':<6} {'tiles':>6} {'kb':>4}"
+          f" {'waves':>5} {'ms':>8} {'TFLOP/s':>8}")
     for r in rows:
         if r["layer"] == 0:
             continue
         tf = r["gflop"] / r["ms"] if r["ms"] > 0 else 0.0
         print(f"{r['layer']:>3} {r['cin']:>5} {r['cout']:>5} {r['k']:>2} {r['s']:>2} {r['hw']:>4} {r['kernel']:<10}"
-              f" {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
+              f" {r['sched']:<6} {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
     conv_ms = sum(r["ms"] for r in rows)
     igemm = [r for r in rows if r["kernel"] == "conv_igemm"]
     igemm_ms = sum(r["ms"] for r in igemm)

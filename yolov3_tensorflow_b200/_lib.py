@@ -43,6 +43,11 @@ class ConvSchedule(C.Structure):   # yb_conv_schedule_info
                                    "num_m_tiles", "num_n_tiles", "grid")]
 
 
+class LayerSchedule(C.Structure):  # yb_layer_schedule_info
+    _fields_ = [(n, i32) for n in ("igemm", "pingpong", "cluster_m", "cluster_n", "block_m", "block_n", "num_m_tiles",
+                                   "num_n_tiles", "units", "max_clusters", "grid")]
+
+
 class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info
     _fields_ = [(n, i32) for n in ("bnw", "tp", "stages", "num_kb", "kb_per_split", "splits", "tiles", "grid_x",
                                    "grid_y", "grid_z")]
@@ -122,6 +127,7 @@ _SIGS = {
     "yb_net_destroy": ([vp], i32),
     "yb_net_num_layers": ([vp], i32),
     "yb_net_layer_info": ([vp, i32, C.POINTER(LayerInfo)], i32),
+    "yb_net_layer_schedule": ([vp, i32, i32, C.POINTER(LayerSchedule)], i32),
     "yb_net_arena_bytes": ([vp, C.POINTER(sz), C.POINTER(sz)], i32),
     "yb_net_bind": ([vp, vp, sz, vp, sz, vp], i32),
     "yb_net_refold_bn": ([vp, vp], i32),

@@ -217,6 +217,19 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta)
       "r"(cta)
       : "memory");
 }
+// The same arrive with the default .release.cta semantics.  The consumers' stage release only has to follow their own
+// wgmma reads (already retired by wgmma.wait_group); a .cluster-scope release compiles to MEMBAR.ALL.GPU + ERRBAR per
+// arrive, which in the conv main loop stalls every k-block (DESIGN.md §5).
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
+}
 // the box lands at the same shared-memory offset in every CTA of `mask`; each destination's bytes are credited to the
 // barrier at the same offset in that CTA
 __device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
@@ -225,6 +238,16 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorM
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%4, %5}], [%2], %3;"
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
+      : "memory");
+}
+// im2col-mode load (tma_load_im2col_4d) multicast like tma_load_2d_multicast
+__device__ __forceinline__ void tma_load_im2col_4d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c, int w,
+                                                             int h, int n, uint16_t ow, uint16_t oh, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6, %7}], [%2], {%8, %9}, %3;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(mask), "r"(c), "r"(w), "r"(h),
+      "r"(n), "h"(ow), "h"(oh)
       : "memory");
 }
 

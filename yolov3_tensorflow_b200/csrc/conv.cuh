@@ -14,7 +14,9 @@ struct ConvParams {
   int scatter;            // 0, or 1 + 2a + b: output pixel (p, q) is stored at (2p + a, 2q + b) of a [n, 2P, 2Q] grid
   int im2col;             // 1: A via im2col TMA, 0: A via 2D tiled TMA
   int consumers;          // consumer warpgroups per CTA: 64 output rows each (1 | 2)
-  int cluster;            // CTAs per cluster sharing one multicast weight tile (1 | 2 | 4)
+  int cluster;            // CTAs per cluster (1 | 2 | 4): cooperative, along M sharing one multicast weight tile;
+                          // ping-pong, (cluster / cluster_n) x cluster_n m x n tiles multicasting A and B
+  int cluster_n;          // CTAs of a cluster along N (1 | 2; 1 for the cooperative clusters)
   int epi_reg;            // 1: accumulator fragments stored straight from registers (no staging tile)
   int pingpong;           // 1: the two consumer warpgroups take whole tiles in turn (csrc/conv_igemm.cu)
   int ctas;               // > 0: the persistent grid is capped at this many CTAs (YB_CONV_CTAS; launch_cfg)
@@ -36,6 +38,12 @@ struct ConvParams {
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
                  const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
                  ConvParams* p, int* cout_pad_out);
+// conv_prepare of a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
+// YB_CONV_MCAST is unset (csrc/conv_igemm.cu)
+int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
+                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out);
+// the kernel choice of conv_prepare without pointers (no device work)
+int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, ConvParams* p);
 // Window variant used by the stride-2 dgrad: a kh x kw window whose taps sit at offsets (0..kh-1, 0..kw-1) from the
 // output pixel (zero-filled past the border), stride 1, output scattered to parity class `scatter`.
 // w_packed is [cout_pad][kh*kw*cin].
@@ -78,5 +86,11 @@ int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const floa
 int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);
 int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
                 cudaStream_t st);
+// what conv_launch would launch on the current device, without launching: grid (CTAs) and the most clusters of
+// p.cluster CTAs that can be resident at once (cudaOccupancyMaxActiveClusters; the SM count when p.cluster == 1)
+int conv_launch_grid(int dtype, int cout_pad, const ConvParams& p, int* grid, int* max_clusters);
+// the persistent grid for sms SMs of which at most max_clusters clusters are resident (<= 0: sms / cluster)
+int conv_grid(const ConvParams& p, int sms, int max_clusters);
+int conv_block_n(int cout_pad);   // 128 or 64 output channels per tile
 
 }  // namespace yb

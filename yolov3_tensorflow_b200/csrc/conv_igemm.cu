@@ -89,6 +89,22 @@ __device__ __forceinline__ void unit_coords(const ConvParams& p, int unit, int r
   else { sm = unit / p.num_n_tiles; n_idx = unit - sm * p.num_n_tiles; }
   m_idx = sm * p.cluster + rank;
 }
+// Ping-pong multicast clusters of CM x CN CTAs: a unit is CM consecutive m-tiles x CN consecutive n-tiles (n-groups
+// fastest for inference, as above), and rank r = rm * CN + rn takes m-tile rm and n-tile rn of it.  The host takes
+// CN = 2 only where the n-tile count is even; ranks past the last m-tile take part in the multicasts, rows masked.
+template <int CM, int CN>
+__device__ __forceinline__ int num_units_mn(const ConvParams& p) {
+  return (p.num_m_tiles + CM - 1) / CM * (p.num_n_tiles / CN);
+}
+template <int CM, int CN>
+__device__ __forceinline__ void unit_coords_mn(const ConvParams& p, int unit, uint32_t rank, int& m_idx, int& n_idx) {
+  const int m_groups = (p.num_m_tiles + CM - 1) / CM, n_groups = p.num_n_tiles / CN;
+  int mg, ng;
+  if (p.stat_sum != nullptr) { ng = unit / m_groups; mg = unit - ng * m_groups; }
+  else { mg = unit / n_groups; ng = unit - mg * n_groups; }
+  m_idx = mg * CM + (int)rank / CN;
+  n_idx = ng * CN + (int)rank % CN;
+}
 
 // executed by the 128 threads of one consumer warpgroup: add the per-CTA column sums into the global statistics
 template <int BN>
@@ -323,13 +339,19 @@ __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float
 // start its next main loop" (ping-pong)
 static constexpr int MMA_TURN_BAR = 3;
 
-// DET_E = 5 + classes: detection head with the decode fused in.  PP: ping-pong schedule (NC = 2, no cluster, staged
-// epilogue, no fused decode; see the top of the file).  BKB: bytes per k-block row (Cfg).
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false>
+// DET_E = 5 + classes: detection head with the decode fused in.  PP: ping-pong schedule (NC = 2, staged epilogue, no
+// fused decode; see the top of the file).  BKB: bytes per k-block row (Cfg).
+// CM x CN (ping-pong only): a cluster of CM m-tiles x CN n-tiles.  Each CTA loads 1/CN of its A tile, multicast to the
+// CN CTAs of its m-tile, and 1/CM of its B tile, multicast to the CM CTAs of its n-tile: every CTA still receives the
+// full STAGE_BYTES per k-block but reads only A_BYTES / CN + B_BYTES / CM of them from L2.  Each warpgroup computes
+// the same tiles with the same wgmma sequence as without the cluster, so the outputs are the same bit for bit.
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
   static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
+  static_assert(PP || (CM == 1 && CN == 1), "multicast cluster shapes are a ping-pong variant");
+  constexpr int MCS = CM * CN;                           // CTAs per ping-pong cluster
   constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
   using C = Cfg<BN, BKB, NC>;
   constexpr int BK = BKB / (int)sizeof(T);               // channels per k-block
@@ -353,17 +375,21 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], PP ? 4 : 4 * NC * p.cluster);
+      // every consumer warp that reads a stage arrives on that stage's empty barrier in every CTA of the cluster (any of
+      // them may multicast into it next): ping-pong, the 4 warps of the one warpgroup that read it, in each of MCS CTAs
+      mbar_init(&empty_bar[i], PP ? 4 * MCS : 4 * NC * p.cluster);
     }
     fence_barrier_init();
   }
   __syncthreads();
   if (p.cluster > 1) cluster_sync_all();                 // every peer's barriers exist before the first multicast
 
-  const int cs = PP ? 1 : p.cluster;                     // CTAs per cluster (1: no cluster, no multicast)
+  const int cs = PP ? MCS : p.cluster;                   // CTAs per cluster (1: no cluster, no multicast)
   const uint32_t rank = cs > 1 ? cluster_ctarank() : 0u;
   const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
-  const int nunits = num_units(p);
+  int nunits;
+  if constexpr (MCS > 1) nunits = num_units_mn<CM, CN>(p);
+  else nunits = num_units(p);
   const int kb_per_tap = p.cin / BK;
   const int num_kb = p.kh * p.kw * kb_per_tap;
 
@@ -371,8 +397,58 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================== TMA producer =====================
     // One thread runs the whole loop: a k-block costs one barrier wait, one expect_tx and two TMA issues.  The filter
     // tap / channel-chunk coordinates are carried as counters instead of being divided out of the k-block index.
-    // In a cluster every CTA loads its own A tile and 1/cs of the shared weight tile, multicast to all cs CTAs.
-    if (threadIdx.x == 0) {
+    // In a cooperative cluster every CTA loads its own A tile and 1/cs of the shared weight tile, multicast to all cs
+    // CTAs.  In a CM x CN ping-pong cluster CTA (rm, rn) loads A rows [rn BLOCK_M / CN, +BLOCK_M / CN) — for a 3x3 conv
+    // an im2col box of BLOCK_M / CN pixels from output pixel m0 + rn BLOCK_M / CN — multicast to the CTAs (rm, *), and
+    // B rows [rm BN / CM, +BN / CM), multicast to the CTAs (*, rn).  The halves start on whole 8-row swizzle groups,
+    // so they land exactly where the whole-tile loads put them.
+    if constexpr (MCS > 1) {
+      if (threadIdx.x == 0) {
+        constexpr int A_ROWS = C::BLOCK_M / CN, B_ROWS = BN / CM;
+        const int rm = (int)rank / CN, rn = (int)rank % CN;
+        const uint16_t a_mask = (uint16_t)(((1u << CN) - 1u) << (rm * CN));
+        uint16_t b_mask = 0;
+#pragma unroll
+        for (int i = 0; i < CM; ++i) b_mask |= (uint16_t)(1u << (i * CN + rn));
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
+          int m_idx, n_idx;
+          unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
+          const int ma = m_idx * C::BLOCK_M + rn * A_ROWS;     // first row of this CTA's A slice
+          const int nb = n_idx * BN + rm * B_ROWS;             // first row of this CTA's B slice
+          const int q = ma % p.Q;
+          const int pp = (ma / p.Q) % p.P;
+          const int img = ma / (p.Q * p.P);
+          const int w_base = q * p.stride - p.pad;
+          const int h_base = pp * p.stride - p.pad;
+          int c0 = 0, tw = 0, th = 0, kcol = 0;
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+            uint8_t* a_dst = sA + stage * C::A_BYTES + rn * A_ROWS * BKB;
+            uint8_t* b_dst = sB + stage * C::B_BYTES + rm * B_ROWS * BKB;
+            if constexpr (CN > 1) {
+              if (p.im2col)
+                tma_load_im2col_4d_multicast(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
+                                             (uint16_t)th, a_mask);
+              else
+                tma_load_2d_multicast(a_dst, &tmA, &full_bar[stage], c0, ma, a_mask);
+            } else {
+              if (p.im2col)
+                tma_load_im2col_4d(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw, (uint16_t)th);
+              else
+                tma_load_2d(a_dst, &tmA, &full_bar[stage], c0, ma);
+            }
+            if constexpr (CM > 1) tma_load_2d_multicast(b_dst, &tmB, &full_bar[stage], kcol, nb, b_mask);
+            else tma_load_2d(b_dst, &tmB, &full_bar[stage], kcol, nb);
+            c0 += BK; kcol += BK;
+            if (c0 == p.cin) { c0 = 0; if (++tw == p.kw) { tw = 0; ++th; } }
+            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    } else if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int b_rows = BN / cs;
@@ -429,8 +505,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     auto release = [&](int st) {
       __syncwarp();
       if (lane == 0) {
-        if (cs == 1) mbar_arrive(&empty_bar[st]);
-        else for (int r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
+        if constexpr (MCS > 1) {
+#pragma unroll
+          for (int r = 0; r < MCS; ++r) mbar_arrive_remote(&empty_bar[st], (uint32_t)r);
+        } else if (cs == 1) {
+          mbar_arrive(&empty_bar[st]);
+        } else {
+          for (int r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
+        }
       }
     };
     float acc[NH][BN / 2];
@@ -448,7 +530,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int unit_step = PP ? 2 * num_clusters : num_clusters;
     for (int unit = cluster_id + (PP ? cw * num_clusters : 0); unit < nunits; unit += unit_step) {
       int m_idx, n_idx;
-      unit_coords(p, unit, rank, m_idx, n_idx);
+      if constexpr (MCS > 1) unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
+      else unit_coords(p, unit, rank, m_idx, n_idx);
       const int m0 = m_idx * C::BLOCK_M;
       const int n0 = n_idx * BN;
       // Ping-pong: wait until the other warpgroup has issued the previous unit's main loop.  Besides keeping the two
@@ -669,12 +752,14 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
   return YB_OK;
 }
 
-// Persistent grid in CTAs: one cluster per work unit, at most one CTA per SM, and at most p.ctas CTAs (rounded down to
-// whole clusters, at least one cluster) when YB_CONV_CTAS caps it.
-static int conv_grid(const ConvParams& p, int sms) {
-  const int cs = p.cluster;
-  const int units = ceil_div(p.num_m_tiles, cs) * p.num_n_tiles;
+// Persistent grid in CTAs: one cluster per work unit, at most one CTA per SM and at most max_clusters resident clusters
+// (cudaOccupancyMaxActiveClusters: an H100's GPCs hold 30, not 33, clusters of 4 of these CTAs), and at most p.ctas
+// CTAs (rounded down to whole clusters, at least one cluster) when YB_CONV_CTAS caps it.
+int conv_grid(const ConvParams& p, int sms, int max_active) {
+  const int cs = p.cluster, cn = p.cluster_n;
+  const int units = ceil_div(p.num_m_tiles, cs / cn) * (p.num_n_tiles / cn);
   int max_clusters = sms / cs;
+  if (max_active > 0 && max_active < max_clusters) max_clusters = max_active;
   if (p.ctas > 0) {
     const int cap = p.ctas / cs > 1 ? p.ctas / cs : 1;
     if (cap < max_clusters) max_clusters = cap;
@@ -683,16 +768,55 @@ static int conv_grid(const ConvParams& p, int sms) {
   return clusters * cs;
 }
 
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false>
-static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
+// Most clusters of cs CTAs of `kern` resident at once on the current device, queried once per device and cluster size.
+struct ClusterCapacity { int v[64][5] = {}; };
+static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads, int smem, int cs, int* out) {
+  int dev = 0;
+  YB_CUDA(cudaGetDevice(&dev));
+  int& v = cap.v[dev & 63][cs];
+  if (v == 0) {
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(cs);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    YB_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+    if (n <= 0) { set_error("conv: no cluster of %d CTAs (%d bytes of shared memory each) fits the device", cs, smem); return YB_ERR_CUDA; }
+    v = n;
+  }
+  *out = v;
+  return YB_OK;
+}
+
+// grid != nullptr: report the grid and the resident-cluster bound (grid[1]) instead of launching
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1>
+static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st,
+                      int* grid = nullptr) {
   using C = Cfg<BN, BKB, NC>;
   static DeviceOnce once;
-  auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP>;
+  static ClusterCapacity capacity;
+  auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int cs = p.cluster;
+  if (PP && (p.cluster != CM * CN || p.cluster_n != CN)) {
+    set_error("conv: ping-pong cluster %d (%d along N) launched as %d x %d", p.cluster, p.cluster_n, CM, CN);
+    return YB_ERR_INVALID_ARGUMENT;
+  }
+  int max_clusters = num_sms();
+  if (cs > 1) {
+    const int rc = cluster_capacity(capacity, reinterpret_cast<const void*>(kern), C::THREADS, C::SMEM_BYTES, cs, &max_clusters);
+    if (rc) return rc;
+  }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(conv_grid(p, num_sms()));
+  cfg.gridDim = dim3(conv_grid(p, num_sms(), max_clusters));
+  if (grid) { grid[0] = (int)cfg.gridDim.x; grid[1] = max_clusters; return YB_OK; }
   cfg.blockDim = dim3(C::THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = st;
@@ -703,6 +827,18 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv
   cfg.numAttrs = 1;
   YB_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
   return YB_OK;
+}
+
+// ping-pong: the kernel of the cluster shape (cluster / cluster_n) x cluster_n
+template <typename T, int BN, int BKB>
+static int launch_pp(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
+  const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
+  if (cm == 1 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true>(tmA, tmB, p, st, grid);
+  if (cm == 2 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 1>(tmA, tmB, p, st, grid);
+  if (cm == 1 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 2>(tmA, tmB, p, st, grid);
+  if (cm == 2 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 2>(tmA, tmB, p, st, grid);
+  set_error("conv: no ping-pong kernel for a %d x %d cluster", cm, cn);
+  return YB_ERR_UNSUPPORTED;
 }
 
 int conv_block_k(int cin) { return (cin % 64 == 0) ? 64 : 32; }
@@ -721,15 +857,15 @@ static int conv_stages(int bn, int kb, int nc) {
   return 0;
 }
 
-// Launch with prebuilt tensor maps (used by the network plan).
-int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
-                cudaStream_t st) {
+// Launch with prebuilt tensor maps (used by the network plan); grid != nullptr: report instead of launching.
+static int conv_launch_impl(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
+                            cudaStream_t st, int* grid) {
   const int kb = conv_block_kb(p.cin, dtype);
   if (p.det.on) {
     // detection head with the decode fused in: one n-tile holding all 3 * E columns
 #define YB_DISPATCH_DET(T)                                                                             \
-  if (cout_pad == 256 && kb == 128 && p.det.E == 85) return launch_cfg<T, 256, 128, 2, 85>(tmA, tmB, p, st); \
-  if (cout_pad == 128 && kb == 128 && p.det.E == 25) return launch_cfg<T, 128, 128, 2, 25>(tmA, tmB, p, st);
+  if (cout_pad == 256 && kb == 128 && p.det.E == 85) return launch_cfg<T, 256, 128, 2, 85>(tmA, tmB, p, st, grid); \
+  if (cout_pad == 128 && kb == 128 && p.det.E == 25) return launch_cfg<T, 128, 128, 2, 25>(tmA, tmB, p, st, grid);
     if (dtype == YB_F16) { YB_DISPATCH_DET(__half) }
     else if (dtype == YB_BF16) { YB_DISPATCH_DET(__nv_bfloat16) }
     else if (dtype == YB_E4M3) { YB_DISPATCH_DET(__nv_fp8_e4m3) }
@@ -741,8 +877,8 @@ int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorM
   const int nc = p.consumers;
 #define YB_DISPATCH_BN_KB(T, BN, KB)                                                          \
   if (bn == BN && kb == KB) {                                                                 \
-    if (p.pingpong) return launch_cfg<T, BN, KB, 2, 0, true>(tmA, tmB, p, st);               \
-    return nc == 2 ? launch_cfg<T, BN, KB, 2>(tmA, tmB, p, st) : launch_cfg<T, BN, KB, 1>(tmA, tmB, p, st); \
+    if (p.pingpong) return launch_pp<T, BN, KB>(tmA, tmB, p, st, grid);                        \
+    return nc == 2 ? launch_cfg<T, BN, KB, 2>(tmA, tmB, p, st, grid) : launch_cfg<T, BN, KB, 1>(tmA, tmB, p, st, grid); \
   }
 #define YB_DISPATCH(T)                                                       \
   YB_DISPATCH_BN_KB(T, 128, 128) YB_DISPATCH_BN_KB(T, 128, 64) YB_DISPATCH_BN_KB(T, 64, 128) YB_DISPATCH_BN_KB(T, 64, 64)
@@ -752,8 +888,8 @@ int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorM
   // e4m3: two consumer warpgroups, no cluster (conv_select), so only the ping-pong and cooperative NC = 2 kernels exist
 #define YB_DISPATCH_E4M3(BN, KB)                                                                       \
   if (bn == BN && kb == KB) {                                                                          \
-    if (p.pingpong) return launch_cfg<__nv_fp8_e4m3, BN, KB, 2, 0, true>(tmA, tmB, p, st);            \
-    return launch_cfg<__nv_fp8_e4m3, BN, KB, 2>(tmA, tmB, p, st);                                      \
+    if (p.pingpong) return launch_cfg<__nv_fp8_e4m3, BN, KB, 2, 0, true>(tmA, tmB, p, st, grid);            \
+    return launch_cfg<__nv_fp8_e4m3, BN, KB, 2>(tmA, tmB, p, st, grid);                                      \
   }
   if (dtype == YB_E4M3 && nc == 2 && p.cluster == 1) {
     YB_DISPATCH_E4M3(128, 128) YB_DISPATCH_E4M3(128, 64) YB_DISPATCH_E4M3(64, 128) YB_DISPATCH_E4M3(64, 64)
@@ -764,11 +900,27 @@ int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorM
   return YB_ERR_UNSUPPORTED;
 }
 
+int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
+                cudaStream_t st) {
+  return conv_launch_impl(dtype, cout_pad, tmA, tmB, p, st, nullptr);
+}
+
+int conv_launch_grid(int dtype, int cout_pad, const ConvParams& p, int* grid, int* max_clusters) {
+  CUtensorMap none;
+  memset(&none, 0, sizeof(none));
+  int g[2] = {0, 0};
+  const int rc = conv_launch_impl(dtype, cout_pad, none, none, p, nullptr, g);
+  *grid = g[0];
+  *max_clusters = g[1];
+  return rc;
+}
+
 // Shape checks, tiling and kernel variant of one conv: everything conv_prepare_core decides before it looks at the
 // data pointers.  yb_conv_schedule reports what this picks.
 // win = 0: the forward rule (ksize x ksize, symmetric padding ksize/2); win = 1: kh x kw window at offsets >= 0.
 // det = 1: one n-tile spans the whole padded cout (the fused-decode detection heads).
-static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, int det, ConvParams* p) {
+static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, int det, bool plan_rule,
+                       ConvParams* p) {
   YB_REQUIRE(win || d->ksize == 1 || d->ksize == 3, "conv: ksize must be 1 or 3 (got %d)", d->ksize);
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2 (got %d)", d->stride);
   YB_REQUIRE(!(d->ksize == 1 && d->stride != 1), "conv: 1x1 stride-2 is not on the YOLOv3 path");
@@ -809,6 +961,8 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   //                       128-column tiles included; unset: the shape rule below
   //   YB_CONV_CTAS=N      persistent grid capped at N CTAs (rounded down to whole clusters, at least one), so that
   //                       small tests give every CTA and warpgroup many work units; the kernel is unchanged
+  //   YB_CONV_MCAST=0|2x1|1x2|2x2   ping-pong multicast clusters (below): 0 off everywhere, AxB that shape on every
+  //                       16-bit ping-pong launch; unset: the plan rule in inference plans, off elsewhere
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
   p->epi_reg = (!det && !stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
@@ -822,12 +976,32 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   const bool pp_shape = pp[0] == '1' || (pp[0] != '0' && (kh * kw > 1 || bn != 128));
   p->pingpong = (!det && p->consumers == 2 && p->cluster == 1 && !p->epi_reg && pp_shape) ? 1 : 0;
   const int block_m = 64 * p->consumers;
+  p->num_m_tiles = ceil_div(p->M, block_m);
+  p->num_n_tiles = cout_pad / bn;
+  // Ping-pong multicast clusters, CM m-tiles x CN n-tiles (csrc/conv_igemm.cu, DESIGN.md §4): each CTA reads 1/CN of
+  // its im2col / activation tile and 1/CM of its weight tile from L2.  The plan rule (16-bit inference plans, forward
+  // layers without statistics): 2 x 2 for the windowed convs with an even n-tile count, 2 x 1 for the other windowed
+  // convs; the 1x1 convs, whose activation tile comes from HBM once anyway, stay unclustered.  CN = 2 only where the
+  // n-tile count is even (a forced 1x2 / 2x2 falls back to 1x1 / 2x1 elsewhere).
+  p->cluster_n = 1;
+  if (p->pingpong && !e4m3) {
+    const char* mc = opt("YB_CONV_MCAST");
+    int cm = 1, cn = 1;
+    if (mc[0] != '\0' && mc[0] != '0') {
+      YB_REQUIRE((mc[0] == '1' || mc[0] == '2') && mc[1] == 'x' && (mc[2] == '1' || mc[2] == '2') && mc[3] == '\0',
+                 "conv: YB_CONV_MCAST must be 0, 2x1, 1x2 or 2x2 (got '%s')", mc);
+      cm = mc[0] - '0'; cn = mc[2] - '0';
+    } else if (mc[0] == '\0' && plan_rule && kh * kw > 1) {
+      cm = 2; cn = 2;
+    }
+    if (p->num_n_tiles % 2 != 0) cn = 1;
+    p->cluster = cm * cn;
+    p->cluster_n = cn;
+  }
   memset(&p->det, 0, sizeof(p->det));
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
   p->kh = kh; p->kw = kw; p->scatter = scatter;
   p->im2col = kh * kw > 1;
-  p->num_m_tiles = ceil_div(p->M, block_m);
-  p->num_n_tiles = cout_pad / bn;
   p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
   p->res_scale = 1.f; p->out_inv_scale = 1.f;
   return YB_OK;
@@ -837,8 +1011,8 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
 static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
                              const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
                              float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
-                             int* cout_pad_out, int det = 0) {
-  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, det, p);
+                             int* cout_pad_out, int det = 0, bool plan_rule = false) {
+  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, det, plan_rule, p);
   if (rc) return rc;
   YB_REQUIRE(x && w_packed && out && (scale == nullptr) == (shift == nullptr), "conv: null pointer");   // scale = shift = NULL: identity
   YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 &&
@@ -850,19 +1024,20 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   const int bk = conv_block_kb(d->cin, d->dtype) / tm_esize(d->dtype);   // channels per k-block
   const int pad = p->pad;
   kh = p->kh; kw = p->kw;
-  const int block_m = 64 * p->consumers;
-  const int bn = det ? cout_pad : conv_block_n(cout_pad);
+  // TMA boxes: this CTA's share of the A tile (1 / cluster_n of its rows) and of the B tile (1 / (cluster / cluster_n))
+  const int a_rows = 64 * p->consumers / p->cluster_n;
+  const int b_rows = (det ? cout_pad : conv_block_n(cout_pad)) / (p->cluster / p->cluster_n);
   p->scale = scale; p->shift = shift;
   p->out = out; p->out_ld = d->out_ld; p->res = res; p->res_ld = d->res_ld;
   p->stat_sum = stat_sum; p->stat_sqsum = stat_sqsum;
   if (p->im2col) {
     rc = make_tmap_im2col_px(tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride, pad, bk,
-                             block_m);
+                             a_rows);
   } else {
-    rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, block_m, bk, 0);
+    rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, a_rows, bk, 0);
   }
   if (rc) return rc;
-  rc = make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, bn / p->cluster, bk, 1);
+  rc = make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, b_rows, bk, 1);
   if (rc) return rc;
   *cout_pad_out = cout_pad;
   return YB_OK;
@@ -873,6 +1048,17 @@ int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, con
                  ConvParams* p, int* cout_pad_out) {
   return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, tmA, tmB, p,
                            cout_pad_out);
+}
+
+int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
+                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out) {
+  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p,
+                           cout_pad_out, 0, true);
+}
+
+int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, ConvParams* p) {
+  memset(p, 0, sizeof(*p));
+  return conv_select(d, 0, 0, 0, 0, false, 0, plan_rule, p);
 }
 
 // Detection head with the decode fused into the epilogue (yb_net_detect): ONE n-tile that holds all 3 * (5 + C)
@@ -914,7 +1100,7 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
   }
   yb::ConvParams p;
   memset(&p, 0, sizeof(p));
-  const int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, 0, &p);
+  const int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, 0, false, &p);
   if (rc) return rc;
   info->pingpong = p.pingpong;
   info->consumers = p.consumers;
@@ -927,7 +1113,7 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
   info->num_kb = p.kh * p.kw * d->cin / info->block_k;
   info->num_m_tiles = p.num_m_tiles;
   info->num_n_tiles = p.num_n_tiles;
-  info->grid = yb::conv_grid(p, sm_count);
+  info->grid = yb::conv_grid(p, sm_count, 0);
   return YB_OK;
 }
 

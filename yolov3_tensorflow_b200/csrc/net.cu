@@ -186,6 +186,20 @@ static int fold_e4m3_layer(yb_net* net, Layer& L, cudaStream_t st) {
                   L.info.cout, net->bn_eps, net->buf_scale[L.in.buf], f(L.w_scale), f(L.scale), f(L.shift), st);
 }
 
+// conv descriptor of a tensor-core layer of the plan
+static yb_conv_desc layer_desc(const yb_net* net, const Layer& L) {
+  yb_conv_desc d;
+  memset(&d, 0, sizeof(d));
+  d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
+  d.ksize = L.info.ksize; d.stride = L.info.stride;
+  d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = net->bufs[L.out.buf].ld;
+  d.res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
+  d.dtype = L.dtype; d.out_fp32 = L.out_fp32; d.leaky = L.info.has_bn; d.upsample2x = L.upsample;
+  return d;
+}
+// the multicast-cluster rule of conv_select applies to the 16-bit inference plans (not training, not e4m3)
+static bool plan_mcast_rule(const yb_net* net) { return !net->training && net->dtype != YB_E4M3; }
+
 __global__ void fill_kernel(float* p, int n, float v) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -220,6 +234,38 @@ extern "C" int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* in
   return YB_OK;
 }
 
+extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info) {
+  YB_REQUIRE(net && info && layer >= 0 && layer < (int)net->layers.size() && sm_count >= 0, "layer_schedule: bad argument");
+  memset(info, 0, sizeof(*info));
+  const Layer& L = net->layers[layer];
+  if (layer == 0) return YB_OK;                        // the stem (fused into layer 1's halo kernel by default)
+  const yb_conv_desc d = layer_desc(net, L);
+  // the default dispatch of forward_layers_impl: the halo kernel for the Cin = 32 BN layers it supports (always for
+  // the e4m3 plan's Conv_3), the implicit-GEMM conv for every other layer
+  const char* hopt = opt("YB_HALO");
+  if (L.info.has_bn && conv_halo_supported(&d) &&
+      ((net->dtype == YB_E4M3 && layer == FP8_FIRST_LAYER - 1) || (hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32))))
+    return YB_OK;
+  ConvParams p;
+  int rc = conv_schedule_params(&d, plan_mcast_rule(net), &p);
+  if (rc) return rc;
+  info->igemm = 1;
+  info->pingpong = p.pingpong;
+  info->cluster_m = p.cluster / p.cluster_n;
+  info->cluster_n = p.cluster_n;
+  info->block_m = 64 * p.consumers;
+  info->block_n = conv_block_n(L.cout_pad);
+  info->num_m_tiles = p.num_m_tiles;
+  info->num_n_tiles = p.num_n_tiles;
+  info->units = ceil_div(p.num_m_tiles, info->cluster_m) * (p.num_n_tiles / p.cluster_n);
+  if (sm_count > 0) {
+    info->max_clusters = sm_count / p.cluster;
+    info->grid = conv_grid(p, sm_count, 0);
+    return YB_OK;
+  }
+  return conv_launch_grid(L.dtype, L.cout_pad, p, &info->grid, &info->max_clusters);
+}
+
 extern "C" int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes) {
   YB_REQUIRE(net && activation_bytes && param_bytes, "arena_bytes: bad argument");
   *activation_bytes = net->act_bytes;
@@ -238,13 +284,7 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
   // prepare every tensor-core conv (layer 0 is the CUDA-core stem)
   for (size_t i = 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
-    yb_conv_desc d;
-    memset(&d, 0, sizeof(d));
-    d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
-    d.ksize = L.info.ksize; d.stride = L.info.stride;
-    d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = net->bufs[L.out.buf].ld;
-    d.res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
-    d.dtype = L.dtype; d.out_fp32 = L.out_fp32; d.leaky = L.info.has_bn; d.upsample2x = L.upsample;
+    yb_conv_desc d = layer_desc(net, L);
     int cp = 0;
     if (net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1) {
       // Conv_3 of the fp8 plan: fp16 in, e4m3 out, only the halo kernel has that form
@@ -259,11 +299,14 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
       L.prepared = false;
       continue;
     }
-    int rc = conv_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed,
-                          reinterpret_cast<const float*>(net->par + L.scale),
-                          reinterpret_cast<const float*>(net->par + L.shift),
-                          L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), nullptr, nullptr, &L.tmA,
-                          &L.tmB, &L.params, &cp);
+    const void* res = L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr;
+    const float* scale = reinterpret_cast<const float*>(net->par + L.scale);
+    const float* shift = reinterpret_cast<const float*>(net->par + L.shift);
+    int rc = plan_mcast_rule(net)
+                 ? conv_prepare_plan(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
+                                     &L.tmA, &L.tmB, &L.params, &cp)
+                 : conv_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
+                                nullptr, nullptr, &L.tmA, &L.tmB, &L.params, &cp);
     if (rc) return rc;
     L.prepared = true;
     L.halo_ok = false;
