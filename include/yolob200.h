@@ -113,6 +113,8 @@ typedef struct yb_conv_schedule_info {
   int num_kb;        /* k-blocks per tile                                                       */
   int num_m_tiles, num_n_tiles;
   int grid;          /* CTAs launched                                                           */
+  int res_smem;      /* 1: a launch with a residual prefetches it into shared memory (YB_CONV_RES) */
+  int res_stages;    /* operand-ring depth of a launch with a residual                          */
 } yb_conv_schedule_info;
 int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count, yb_conv_schedule_info* info);
 
@@ -420,6 +422,9 @@ typedef struct yb_layer_schedule_info {
   int units;         /* work units: ceil(num_m_tiles / cluster_m) x num_n_tiles / cluster_n         */
   int max_clusters;  /* most clusters resident at once                                              */
   int grid;          /* CTAs launched: a multiple of cluster_m x cluster_n, <= max_clusters of them */
+  int residual;      /* 1: the layer adds a shortcut (also reported for the halo-kernel layers)     */
+  int res_smem;      /* 1: the shortcut tile is TMA-prefetched into shared memory during the main   */
+                     /*    loop (YB_CONV_RES); 0: the epilogue reads it from global memory          */
 } yb_layer_schedule_info;
 int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info);
 int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes);

@@ -7,6 +7,11 @@ Every layer is launched alone through yb_net_forward_layers(first = last = i) --
 two events.  The detection heads run unfused here (fp32 feature map out), not with the decode of yb_net_detect.
 Layer 0 (the stem) runs inside layer 1's launch.  Per layer: shape, kernel, ms, algorithmic TFLOP/s.
 
+The `res` column marks the layers that add a shortcut.  Each shortcut layer is then paired with its no-shortcut
+twins, the layers of the same GEMM (cin, cout, k, output size; stride free) and kernel: Conv_6/8 with Conv_4 at 104^2,
+and at 52^2, 26^2 and 13^2 the darknet 3x3s with the yolo-block 3x3s.  The summary prints the time each class loses to
+its shortcut (sum over its shortcut layers of ms - mean twin ms).
+
 Then the conv_igemm time of a layer is split into a per-k-block and a per-tile fixed cost from pairs of layers
 with the same tile count and different K (52^2: layer 68 vs 70/72; 26^2: layer 60 vs 62/64):
     t = waves * (kblocks * c_kb + c_fix),   waves = ceil(tiles / SMs)
@@ -102,11 +107,14 @@ def main():
         if i == 1:
             flop += 2.0 * B * S * S * 27 * plan.layer_info(0).cout          # the stem's FLOPs run in this launch
         row = dict(layer=i, cin=info.cin, cout=info.cout, k=info.ksize, s=info.stride, hw=info.out_h,
-                   up=info.upsample2x, kernel=kern, gflop=flop / 1e9, ms=0.0, sched="")
-        if kern == "conv_igemm":               # the plan's schedule: ping-pong / cooperative, multicast cluster shape
+                   up=info.upsample2x, kernel=kern, gflop=flop / 1e9, ms=0.0, sched="", res="")
+        if i > 0:
             sc = LayerSchedule()
             check(lib.yb_net_layer_schedule(plan.handle, i, 0, C.byref(sc)), "yb_net_layer_schedule")
-            row["sched"] = ("pp " if sc.pingpong else "co ") + f"{sc.cluster_m}x{sc.cluster_n}"
+            # shortcut: "ldg" read by the epilogue from global memory, "smem" prefetched into shared memory
+            row["res"] = ("smem" if sc.res_smem else "ldg") if sc.residual else ""
+            if kern == "conv_igemm":           # the plan's schedule: ping-pong / cooperative, multicast cluster shape
+                row["sched"] = ("pp " if sc.pingpong else "co ") + f"{sc.cluster_m}x{sc.cluster_n}"
         if i > 0:
             for _ in range(3):
                 run(i)
@@ -122,20 +130,41 @@ def main():
         rows.append(row)
 
     print(f"# card: {card()}   SMs: {sms}   batch {B}, {S}x{S}, fp16, {args.reps} reps per layer")
-    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'sched':<6} {'tiles':>6} {'kb':>4}"
+    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'sched':<6} {'res':<4} {'tiles':>6} {'kb':>4}"
           f" {'waves':>5} {'ms':>8} {'TFLOP/s':>8}")
     for r in rows:
         if r["layer"] == 0:
             continue
         tf = r["gflop"] / r["ms"] if r["ms"] > 0 else 0.0
         print(f"{r['layer']:>3} {r['cin']:>5} {r['cout']:>5} {r['k']:>2} {r['s']:>2} {r['hw']:>4} {r['kernel']:<10}"
-              f" {r['sched']:<6} {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
+              f" {r['sched']:<6} {r['res']:<4} {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
     conv_ms = sum(r["ms"] for r in rows)
     igemm = [r for r in rows if r["kernel"] == "conv_igemm"]
     igemm_ms = sum(r["ms"] for r in igemm)
     gflop = sum(r["gflop"] for r in rows)
     print(f"# sum of layers: {conv_ms:.3f} ms ({gflop / conv_ms:.1f} TFLOP/s); conv_igemm: {igemm_ms:.3f} ms over "
           f"{len(igemm)} layers; conv_halo: {conv_ms - igemm_ms:.3f} ms")
+
+    # shortcut penalty per class: each shortcut layer against the mean of its no-shortcut twins
+    def gemm(r):
+        return (r["cin"], r["cout"], r["k"], r["hw"], r["kernel"])
+    res_rows = [r for r in rows if r["res"]]
+    penalty = {}
+    for key in sorted({gemm(r) for r in res_rows}, key=lambda g: -g[3]):
+        sr = [r for r in res_rows if gemm(r) == key]
+        tw = [r for r in rows if not r["res"] and r["layer"] > 1 and gemm(r) == key]   # layer 1 runs the stem too
+        s_ms = sum(r["ms"] for r in sr)
+        if not tw:
+            print(f"# shortcut {key[3]}^2 {key[0]}->{key[1]} k{key[2]} ({key[4]}): layers "
+                  f"{[r['layer'] for r in sr]} {s_ms:.3f} ms, no twin")
+            continue
+        t_ms = sum(r["ms"] for r in tw) / len(tw)
+        pen = s_ms - len(sr) * t_ms
+        penalty[f"{key[3]}^2 {key[0]}->{key[1]} k{key[2]}"] = pen
+        print(f"# shortcut {key[3]}^2 {key[0]}->{key[1]} k{key[2]} ({key[4]}): layers {[r['layer'] for r in sr]} "
+              f"mean {s_ms / len(sr):.4f} ms vs twins {[r['layer'] for r in tw]} mean {t_ms:.4f} ms -> "
+              f"penalty {pen:.3f} ms")
+    print(f"# shortcut penalty summed over the classes with a twin: {sum(penalty.values()):.3f} ms")
 
     # per-k-block / per-tile split from the two same-tile-count pairs
     fits = {}
@@ -161,7 +190,8 @@ def main():
     if args.json:
         with open(args.json, "w") as f:
             json.dump(dict(card=card(), sms=sms, batch=B, size=S, reps=args.reps, rows=rows,
-                           fits={str(k): v for k, v in fits.items()}, fixed_ms=fixed), f, indent=1)
+                           fits={str(k): v for k, v in fits.items()}, fixed_ms=fixed, shortcut_penalty_ms=penalty),
+                      f, indent=1)
 
 
 if __name__ == "__main__":

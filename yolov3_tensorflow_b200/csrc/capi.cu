@@ -52,7 +52,7 @@ int ensure_smem_attr(DeviceOnce& once, const void* kernel, int bytes) {
 // ---- runtime switches (A/B experiments and tests only; DESIGN.md 5b).  Seeded ONCE from the YB_* environment
 // ---- variables, changed afterwards only through yb_set_option(): no getenv() on any call path.
 struct Opt { const char* key; char val[32]; };
-static Opt g_opts[] = {{"YB_CONV_MODE", ""}, {"YB_CONV_MC", ""}, {"YB_CONV_MCAST", ""}, {"YB_CONV_EPI", ""}, {"YB_CONV_EG", ""}, {"YB_CONV_PP", ""}, {"YB_CONV_CTAS", ""}, {"YB_THIN", ""}, {"YB_STEM_DBG", ""},
+static Opt g_opts[] = {{"YB_CONV_MODE", ""}, {"YB_CONV_MC", ""}, {"YB_CONV_MCAST", ""}, {"YB_CONV_RES", ""}, {"YB_CONV_EPI", ""}, {"YB_CONV_EG", ""}, {"YB_CONV_PP", ""}, {"YB_CONV_CTAS", ""}, {"YB_THIN", ""}, {"YB_STEM_DBG", ""},
                        {"YB_STEM_WGRAD", ""}, {"YB_WGRAD_TP", ""}, {"YB_DGRAD_S2", ""},
                        {"YB_HALO", ""}, {"YB_STEM_FUSE", ""},
                        {"YB_BN_CPT", ""}, {"YB_BN_FIN", ""}, {"YB_PACK_MT", ""}, {"YB_WGRAD_EPI", ""}, {"YB_WGRAD_SPLITS", ""}, {"YB_STEM_TRAIN", ""}, {"YB_WGRAD_STREAM", ""}, {"YB_STEM_SPLIT", ""}, {"YB_HEAD_STREAM", ""}};

@@ -33,6 +33,8 @@ struct ConvParams {
   DetParams det;          // det.on: decode + NMS candidate filter instead of the fp32 feature-map store (detection heads)
   // e4m3 only (1 otherwise): the residual buffer's scale (codes -> values) and 1 / the output buffer's scale
   float res_scale, out_inv_scale;
+  int res_smem;           // 1: the ping-pong kernel TMA-prefetches the residual tile into shared memory (YB_CONV_RES)
+  CUtensorMap tmR;        // res_smem: the residual as a [M, cout] matrix, 128-row x 64-channel 128B-swizzled boxes
 };
 
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
@@ -53,7 +55,7 @@ int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const v
 int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
                      const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out);
 // halo-tile conv for the Cin <= 64 3x3 layers (csrc/conv_halo.cu)
-struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; };
+struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; CUtensorMap res; };
 struct HaloParams {
   int n, ho, wo;               // output geometry
   int tiles_x, tiles_y, num_tiles;
@@ -73,8 +75,10 @@ struct HaloParams {
   // 1: the output is e4m3 codes of value * out_inv_scale (Conv_3 of the fp8 plan: fp16 in, e4m3 out)
   int out_e4m3;
   float out_inv_scale;
+  int res_smem;                // 1: the residual is TMA-loaded with each tile's halo (YB_CONV_RES; conv_halo_res_smem)
 };
 bool conv_halo_supported(const yb_conv_desc* d);
+bool conv_halo_res_smem(const yb_conv_desc* d);
 int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
                       const void* res, void* out, HaloMaps* maps, HaloParams* p);
 int conv_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);

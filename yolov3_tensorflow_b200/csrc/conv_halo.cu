@@ -42,7 +42,9 @@ static constexpr int HT_H = 16, HT_W = 8;       // output tile
 static constexpr int HALO_THREADS = 384;         // warp 0: TMA, warpgroups 1, 2: MMA + epilogue
 static constexpr int HALO_EPI_LD = 33;          // staging row pitch in floats
 
-template <int CIN, int COUT, int STRIDE>
+// RES (Conv_3: 32 -> 64, stride 1, with a shortcut): every stage also holds the tile's residual, a [16][8] x 64-channel
+// box of 128B-swizzled pixel rows loaded by TMA with the halo, so the epilogue adds it from shared memory.
+template <int CIN, int COUT, int STRIDE, bool RES = false>
 struct HaloCfg {
   static constexpr int ROWB = CIN * 2;                                   // bytes per pixel row of a plane (one swizzle span)
   static constexpr int NPLANE = STRIDE == 1 ? 1 : 4;
@@ -51,9 +53,12 @@ struct HaloCfg {
   static constexpr int pw(int p) { return STRIDE == 1 ? HT_W + 2 : ((p & 1) == 0 ? HT_W + 1 : HT_W); }
   static constexpr int pbytes(int p) { return (ph(p) * pw(p) * ROWB + 1023) / 1024 * 1024; }
   static constexpr int poff(int p) { return p == 0 ? 0 : poff(p - 1) + pbytes(p - 1); }
-  static constexpr int STAGE_BYTES = poff(NPLANE - 1) + pbytes(NPLANE - 1);
-  static constexpr int STAGE_TX = STRIDE == 1 ? ph(0) * pw(0) * ROWB
-                                              : (ph(0) * pw(0) + ph(1) * pw(1) + ph(2) * pw(2) + ph(3) * pw(3)) * ROWB;
+  static constexpr int RES_OFF = poff(NPLANE - 1) + pbytes(NPLANE - 1);  // 1024-byte aligned
+  static constexpr int RES_BYTES = RES ? HT_H * HT_W * COUT * 2 : 0;
+  static constexpr int STAGE_BYTES = RES_OFF + RES_BYTES;
+  static constexpr int STAGE_TX = (STRIDE == 1 ? ph(0) * pw(0) * ROWB
+                                               : (ph(0) * pw(0) + ph(1) * pw(1) + ph(2) * pw(2) + ph(3) * pw(3)) * ROWB) +
+                                  RES_BYTES;
   static constexpr int B_TAP_BYTES = COUT * ROWB;                        // one tap's [COUT][CIN] weight tile
   static constexpr int B_BYTES = 9 * B_TAP_BYTES;
   static constexpr int EPI_BYTES = 2 * 64 * HALO_EPI_LD * 4;              // a [64][33] fp32 staging tile per consumer warpgroup
@@ -109,10 +114,11 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T>
+template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T, bool RES = false>
 __global__ void __launch_bounds__(HALO_THREADS + 32 * STEMW, 1)
 conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ HaloParams p) {
-  using C = HaloCfg<CIN, COUT, STRIDE>;
+  using C = HaloCfg<CIN, COUT, STRIDE, RES>;
+  static_assert(!RES || (CIN == 32 && COUT == 64 && STRIDE == 1 && STEMW == 0), "the residual box is Conv_3's");
   constexpr int PROD_WARP0 = HALO_THREADS / 32;  // first stem-producer warp
   static_assert(STEMW == 0 || (CIN == 32 && STRIDE == 2), "the fused stem feeds Conv_1 (32 -> 64, stride 2)");
   extern __shared__ uint8_t smem_raw[];
@@ -137,6 +143,7 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       for (int i = 0; i < C::NPLANE; ++i) tma_prefetch_desc(&maps.plane[i]);
     }
     tma_prefetch_desc(&maps.w);
+    if (RES) tma_prefetch_desc(&maps.res);
     for (int i = 0; i < C::NST; ++i) { mbar_init(&full_bar[i], STEMW > 0 ? STEMW : 1); mbar_init(&empty_bar[i], 8); }
     if (STEMW > 0) {
       tma_prefetch_desc(&maps.in3d);
@@ -184,6 +191,7 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         uint8_t* dst = sA + stage * C::STAGE_BYTES;
         if (STRIDE == 1) {
           tma_load_4d(dst, &maps.plane[0], &full_bar[stage], 0, w0 - 1, h0 - 1, img);
+          if (RES) tma_load_4d(dst + C::RES_OFF, &maps.res, &full_bar[stage], 0, w0, h0, img);   // rows past ho: zeros
         } else {
 #pragma unroll
           for (int pl = 0; pl < 4; ++pl) {
@@ -231,8 +239,13 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       wgmma_fence_operand(acc);
       wgmma_wait<0>();
       wgmma_fence_operand(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      // RES: the stage also holds the residual the epilogue reads, so it is released after the epilogue
+      const uint8_t* sres = sA + stage * C::STAGE_BYTES + C::RES_OFF;
+      const int rel_stage = stage;
+      if (!RES) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      }
       if (++stage == C::NST) { stage = 0; phase ^= 1; }
 
       const int tx = tile % p.tiles_x;
@@ -258,9 +271,12 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         }
         if (has_res) {
           const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + off * p.res_ld + c0);
+          // RES: pixel 64 cw + er of the [16][8] box, 16-byte chunks c0 / 8 and c0 / 8 + 1 stored at chunk ^ (pixel & 7)
+          const int px = 64 * cw + er;
+          const uint8_t* rrow = sres + px * 128;
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
-            const uint4 u = __ldg(rp + j);
+            const uint4 u = RES ? *reinterpret_cast<const uint4*>(rrow + ((((c0 >> 3) + j) ^ (px & 7)) << 4)) : __ldg(rp + j);
             float2 f;
             f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
             f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
@@ -282,6 +298,10 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
           pk.w = Pack2<T>::pack(v[8 * j + 6], v[8 * j + 7]);
           op[j] = pk;
         }
+      }
+      if (RES) {                                 // this warp's last read of the stage is done
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[rel_stage]);
       }
     }
   } else if (STEMW > 0 && warp >= PROD_WARP0) {
@@ -419,11 +439,11 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
   }
 }
 
-template <typename T, int CIN, int COUT, int STRIDE, typename TO = T>
+template <typename T, int CIN, int COUT, int STRIDE, typename TO = T, bool RES = false>
 static int launch_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-  using C = HaloCfg<CIN, COUT, STRIDE>;
+  using C = HaloCfg<CIN, COUT, STRIDE, RES>;
   static DeviceOnce once;
-  auto kern = conv_halo_kernel<T, CIN, COUT, STRIDE, 0, TO>;
+  auto kern = conv_halo_kernel<T, CIN, COUT, STRIDE, 0, TO, RES>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
   kern<<<grid, HALO_THREADS, C::SMEM_BYTES, st>>>(maps, p);
@@ -478,6 +498,11 @@ int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const Hal
   return YB_ERR_UNSUPPORTED;
 }
 
+// the residual of a launch with one is TMA-loaded with the halo (Conv_3's shape only) unless YB_CONV_RES=ldg
+bool conv_halo_res_smem(const yb_conv_desc* d) {
+  return d->cin == 32 && d->cout == 64 && d->stride == 1 && strcmp(opt("YB_CONV_RES"), "ldg") != 0;
+}
+
 bool conv_halo_supported(const yb_conv_desc* d) {
   if (d->ksize != 3 || (d->stride != 1 && d->stride != 2)) return false;
   if (!(d->cin == 32 || d->cin == 64) || !(d->cout == 64 || d->cout == 128)) return false;
@@ -504,6 +529,12 @@ int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed
   p->cout = d->cout; p->leaky = d->leaky; p->scale = scale; p->shift = shift;
   p->res = res; p->res_ld = d->res_ld; p->out = out; p->out_ld = d->out_ld;
   int rc;
+  p->res_smem = res != nullptr && conv_halo_res_smem(d);
+  if (p->res_smem) {
+    // the residual as {C, W, H, N} = [n, ho, wo, res_ld]: one 64-channel x 8 x 16-pixel box per tile
+    rc = make_tmap_tiled4d(&maps->res, res, d->dtype, d->n, p->ho, p->wo, d->cout, d->res_ld, 64, HT_W, HT_H, 1);
+    if (rc) return rc;
+  }
   if (d->stride == 1) {
     rc = make_tmap_tiled4d(&maps->plane[0], x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->cin, HT_W + 2, HT_H + 2, 1);
     if (rc) return rc;
@@ -523,13 +554,15 @@ int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed
 int conv_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
   if (p.out_e4m3) {
     if (d->dtype == YB_F16 && d->cin == 32 && d->cout == 64 && d->stride == 1 && p.out_ld % 16 == 0)
-      return launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3>(maps, p, st);
+      return p.res_smem ? launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3, true>(maps, p, st)
+                        : launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3>(maps, p, st);
     set_error("conv_halo: e4m3 output only for fp16 3x3/1 32->64 (got dtype %d cin=%d cout=%d stride=%d)", d->dtype, d->cin,
               d->cout, d->stride);
     return YB_ERR_UNSUPPORTED;
   }
 #define YB_HALO(T)                                                                              \
-  if (d->cin == 32 && d->cout == 64 && d->stride == 1) return launch_halo<T, 32, 64, 1>(maps, p, st);   \
+  if (d->cin == 32 && d->cout == 64 && d->stride == 1)                                          \
+    return p.res_smem ? launch_halo<T, 32, 64, 1, T, true>(maps, p, st) : launch_halo<T, 32, 64, 1>(maps, p, st); \
   if (d->cin == 32 && d->cout == 64 && d->stride == 2) return launch_halo<T, 32, 64, 2>(maps, p, st);   \
   if (d->cin == 32 && d->cout == 128 && d->stride == 1) return launch_halo<T, 32, 128, 1>(maps, p, st); \
   if (d->cin == 32 && d->cout == 128 && d->stride == 2) return launch_halo<T, 32, 128, 2>(maps, p, st); \

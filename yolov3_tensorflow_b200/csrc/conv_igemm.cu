@@ -25,7 +25,9 @@
 //     epilogue; conv_prepare_core chooses): the NC consumer warpgroups split
 //     every tile by rows (64 each), run the k-loop in lockstep and then the epilogue together.
 // The epilogue stages 32-column chunks of one 64-row accumulator block through shared memory so that each thread then
-// owns 16 consecutive channels of one pixel (two 16-byte stores per output row).
+// owns 16 consecutive channels of one pixel (two 16-byte stores per output row).  Ping-pong launches with a residual
+// (RES) find it already in shared memory: a second producer thread TMA-loads each unit's shortcut tile while the unit's
+// main loop runs.
 //
 // Replaces: slim.conv2d/batch_norm/leaky_relu (utils/layer_utils.py:20, model.py:43-49),
 // tf.add (utils/layer_utils.py:30), tf.pad (:15-16), resize_nearest_neighbor (:86),
@@ -51,22 +53,33 @@ static constexpr int EPI_FLOATS = WG_ROWS * EPI_LD;
 // NC consumer warpgroups per CTA (tile = 64 NC rows x BN); warpgroup 0 is the TMA producer.  Both schedules use the
 // same 128-row tile for NC = 2, so they share the ring and the tensor maps.
 // BKB = bytes of one k-block row (128 or 64): 64 / 32 channels of fp16 / bf16, 128 / 64 channels of e4m3.
-template <int BN, int BKB, int NC>
+// RES (ping-pong, 16-bit): every consumer warpgroup owns a BLOCK_M x BN shortcut tile in shared memory, TMA-loaded in
+// 64-column boxes of 128-byte swizzled rows; the operand ring takes what is left of the 227 KB.
+template <int BN, int BKB, int NC, bool RES = false>
 struct Cfg {
   static constexpr int BLOCK_M = WG_ROWS * NC;
   static constexpr int THREADS = 128 * (NC + 1);
   static constexpr int A_BYTES = BLOCK_M * BKB;
   static constexpr int B_BYTES = BN * BKB;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (RING_BYTES / STAGE_BYTES) > 8 ? 8 : (RING_BYTES / STAGE_BYTES);
-  // ring | NC x staging tile | NC x [2][BN] statistics | NC x [2][BN] scale / shift | barriers.  A ping-pong warpgroup
-  // stages its 128-row tile one 64-row half after the other through its own 64-row staging tile, so the budget is the
-  // same for both schedules (BN = 128, BKB = 128: 6 x 32 KB ring + 2 x 8.4 KB staging + 4 KB = 214 KB).
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + NC * EPI_FLOATS * 4 + NC * 4 * BN * 4 + 256;
+  static constexpr int RES_BOX_COLS = 64;                      // 16-bit channels per 128-byte swizzled row
+  static constexpr int RES_BOX_BYTES = BLOCK_M * 128;          // one 64-column box of the tile
+  static constexpr int RES_TILE_BYTES = BLOCK_M * BN * 2;      // one warpgroup's shortcut tile
+  static constexpr int RES_BYTES = RES ? NC * RES_TILE_BYTES : 0;
+  static constexpr int FIXED_BYTES = 1024 + NC * EPI_FLOATS * 4 + NC * 4 * BN * 4 + 256;
+  static constexpr int RING = RES ? 227 * 1024 - FIXED_BYTES - RES_BYTES : RING_BYTES;
+  static constexpr int STAGES = (RING / STAGE_BYTES) > 8 ? 8 : (RING / STAGE_BYTES);
+  // ring | [RES: NC x shortcut tile] | NC x staging tile | NC x [2][BN] statistics | NC x [2][BN] scale / shift |
+  // barriers.  A ping-pong warpgroup stages its 128-row tile one 64-row half after the other through its own 64-row
+  // staging tile, so the budget is the same for both schedules (BN = 128, BKB = 128: 6 x 32 KB ring + 2 x 8.4 KB
+  // staging + 4 KB = 214 KB; with RES, 4 x 32 KB ring + 2 x 32 KB shortcut tiles + the same 21 KB = 213 KB).
+  static constexpr int SMEM_BYTES = FIXED_BYTES + STAGES * STAGE_BYTES + RES_BYTES;
   static constexpr uint32_t SWIZZLE = BKB;        // a k-block row is exactly one swizzle span (128B / 64B)
   static constexpr uint32_t SBO = 8 * BKB;        // bytes between 8-row groups
 };
 static_assert(Cfg<256, 128, 2>::SMEM_BYTES <= 227 * 1024, "conv: the widest tile does not fit shared memory");
+static_assert(Cfg<128, 128, 2, true>::SMEM_BYTES <= 227 * 1024 && Cfg<128, 128, 2, true>::STAGES >= 4,
+              "conv: the shortcut tiles leave too short an operand ring");
 
 // the wgmma of an operand type: m64nBNk16 for fp16 / bf16, m64nBNk32 for e4m3 (both 32 bytes of K per instruction)
 template <typename T, int BN>
@@ -122,10 +135,12 @@ __device__ __forceinline__ void stat_flush(const ConvParams& p, float* s_stat, i
 }
 
 // 16 consecutive channels of one accumulator row: scale/shift (+leaky) (+residual) -> 16-bit / fp32 global stores
-// (channel-slice, 2x-upsample and parity-scatter aware).
-template <typename T>
+// (channel-slice, 2x-upsample and parity-scatter aware).  SRES: the residual's two 16-byte halves are read from the
+// shared-memory shortcut tile at sr0 / sr1 instead of from global memory (same arithmetic, same result).
+template <typename T, bool SRES = false>
 __device__ __forceinline__ void epi_store16(const ConvParams& p, const float* src, const int row, const int col0,
-                                            const float* sc, const float* sh) {
+                                            const float* sc, const float* sh, const uint4* sr0 = nullptr,
+                                            const uint4* sr1 = nullptr) {
   float v[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) v[j] = fmaf(src[j], sc[j], sh[j]);
@@ -169,11 +184,11 @@ __device__ __forceinline__ void epi_store16(const ConvParams& p, const float* sr
     for (int rep = 0; rep < nrep; ++rep)
       *reinterpret_cast<uint4*>(static_cast<uint8_t*>(p.out) + (orow0 + (rep >> 1) * W2 + (rep & 1)) * p.out_ld + col0) = pk;
   } else {
-    if (p.res != nullptr) {
+    if (SRES || p.res != nullptr) {
       const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const T*>(p.res) + orow0 * p.res_ld + col0);
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
-        const uint4 u = __ldg(rp + j);
+        const uint4 u = SRES ? (j == 0 ? *sr0 : *sr1) : __ldg(rp + j);
         float2 f;
         f = Pack2<T>::unpack(u.x); v[8 * j + 0] += f.x; v[8 * j + 1] += f.y;
         f = Pack2<T>::unpack(u.y); v[8 * j + 2] += f.x; v[8 * j + 3] += f.y;
@@ -345,15 +360,19 @@ static constexpr int MMA_TURN_BAR = 3;
 // CN CTAs of its m-tile, and 1/CM of its B tile, multicast to the CM CTAs of its n-tile: every CTA still receives the
 // full STAGE_BYTES per k-block but reads only A_BYTES / CN + B_BYTES / CM of them from L2.  Each warpgroup computes
 // the same tiles with the same wgmma sequence as without the cluster, so the outputs are the same bit for bit.
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1>
+// RES (ping-pong, 16-bit, p.res != nullptr, YB_CONV_RES): the shortcut tile of every work unit is prefetched by TMA
+// (p.tmR) into its warpgroup's shared-memory tile while the unit's main loop runs, and the epilogue adds it from there
+// instead of waiting on a global load per 32-column chunk.  Each CTA loads its own tile (never multicast).
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1, bool RES = false>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
   static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
   static_assert(PP || (CM == 1 && CN == 1), "multicast cluster shapes are a ping-pong variant");
+  static_assert(!RES || (PP && sizeof(T) == 2), "the shared-memory shortcut tile is a 16-bit ping-pong variant");
   constexpr int MCS = CM * CN;                           // CTAs per ping-pong cluster
   constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
-  using C = Cfg<BN, BKB, NC>;
+  using C = Cfg<BN, BKB, NC, RES>;
   constexpr int BK = BKB / (int)sizeof(T);               // channels per k-block
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by POINTER ARITHMETIC on the __shared__ array: an integer round trip makes the pointer generic,
@@ -361,12 +380,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + C::STAGES * C::A_BYTES;
-  float* s_epi = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);   // [NC][64][EPI_LD] staging tiles
+  uint8_t* sR = smem + C::STAGES * C::STAGE_BYTES;       // RES: [NC] shortcut tiles, 1024-byte aligned
+  float* s_epi = reinterpret_cast<float*>(sR + C::RES_BYTES);   // [NC][64][EPI_LD] staging tiles
   float* s_stat = s_epi + NC * EPI_FLOATS;               // [NC][2][BN] per-CTA column sums / sums of squares
   float* s_ss = s_stat + NC * 2 * BN;                    // [NC][2][BN] scale / shift of each warpgroup's current n-tile
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_ss + NC * 2 * BN);   // [STAGES] TMA -> MMA
   uint64_t* empty_bar = full_bar + 8;                    // [STAGES] MMA -> TMA: one arrive per consumer warp of the cluster
                                                          // (ping-pong: of the one warpgroup that read the stage)
+  uint64_t* res_full = empty_bar + 8;                    // RES: [NC] shortcut tile landed
+  uint64_t* res_empty = res_full + NC;                   // RES: [NC] the warpgroup's epilogue has read it (4 warps)
 
   // warp-uniform by construction: ptxas then keeps the ping-pong consumer's 128 accumulators out of local memory
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
@@ -378,6 +400,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // every consumer warp that reads a stage arrives on that stage's empty barrier in every CTA of the cluster (any of
       // them may multicast into it next): ping-pong, the 4 warps of the one warpgroup that read it, in each of MCS CTAs
       mbar_init(&empty_bar[i], PP ? 4 * MCS : 4 * NC * p.cluster);
+    }
+    if constexpr (RES) {
+      tma_prefetch_desc(&p.tmR);
+      for (int i = 0; i < NC; ++i) {
+        mbar_init(&res_full[i], 1);
+        mbar_init(&res_empty[i], 4);
+      }
     }
     fence_barrier_init();
   }
@@ -486,6 +515,31 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
+    if constexpr (RES) {
+      // Shortcut tiles: one thread of warp 1 walks the CTA's units in the same order and loads unit j's tile into
+      // warpgroup (j & 1)'s buffer as soon as that warpgroup's epilogue has released the tile of its previous unit, so
+      // the load has the whole main loop of unit j to land.  Independent of the operand ring: the ring never waits on
+      // an epilogue.  Units wholly past M (cluster ranks past the last m-tile) have nothing to add and are skipped on
+      // both sides.
+      if (threadIdx.x == 32) {
+        uint32_t rphase[NC] = {};
+        int j = 0;
+        for (int unit = cluster_id; unit < nunits; unit += num_clusters, ++j) {
+          int m_idx, n_idx;
+          if constexpr (MCS > 1) unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
+          else unit_coords(p, unit, rank, m_idx, n_idx);
+          const int m0 = m_idx * C::BLOCK_M, n0 = n_idx * BN;
+          if (m0 >= p.M) continue;
+          const int w = j & 1;
+          mbar_wait(&res_empty[w], rphase[w] ^ 1);
+          mbar_arrive_expect_tx(&res_full[w], C::RES_TILE_BYTES);
+#pragma unroll
+          for (int b = 0; b < BN / C::RES_BOX_COLS; ++b)
+            tma_load_2d(sR + w * C::RES_TILE_BYTES + b * C::RES_BOX_BYTES, &p.tmR, &res_full[w], n0 + b * C::RES_BOX_COLS, m0);
+          rphase[w] ^= 1;
+        }
+      }
+    }
   } else {
     // ===================== MMA + epilogue =====================
     // cooperative: warpgroup cw computes rows [64 cw, 64 cw + 64) of every tile of the CTA;
@@ -528,6 +582,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     int cur_n0 = -1, ss_n0 = -1;
     const uint32_t a_off = PP ? 0u : cw * WG_ROWS * BKB;
     const int unit_step = PP ? 2 * num_clusters : num_clusters;
+    uint32_t res_phase = 0;
+    const uint8_t* sres = sR + cw * C::RES_TILE_BYTES;   // RES: this warpgroup's shortcut tile
     for (int unit = cluster_id + (PP ? cw * num_clusters : 0); unit < nunits; unit += unit_step) {
       int m_idx, n_idx;
       if constexpr (MCS > 1) unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
@@ -588,6 +644,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float(&acc_all)[NH * BN / 2] = reinterpret_cast<const float(&)[NH * BN / 2]>(acc);
         const int nvalid = min(BN / 32, (p.cout - n0 + 31) >> 5);   // zero-padded weight rows (cout_pad > cout): not stored
         const int er = t >> 1, eh = t & 1;       // this thread's row of the chunk and its 16-column half
+        if constexpr (RES) {
+          if (m0 < p.M) mbar_wait(&res_full[cw], res_phase);
+        }
 #pragma unroll 1
         for (int h = 0; h < NH; ++h) {
           const int row0 = m0 + (PP ? h : cw) * WG_ROWS;
@@ -612,8 +671,25 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             if (row0 + er < p.M) {
               const int cl = ch * 32 + eh * 16;
-              epi_store16<T>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl);
+              if constexpr (RES) {
+                // row rl of the tile, columns cl..cl+15 = 16-byte chunks c, c+1 of a 128-byte row of box cl / 64,
+                // stored at chunk ^ (rl & 7) (TMA 128B swizzle)
+                const int rl = h * WG_ROWS + er, c = (cl % C::RES_BOX_COLS) >> 3;
+                const uint8_t* rrow = sres + (cl / C::RES_BOX_COLS) * C::RES_BOX_BYTES + rl * 128;
+                epi_store16<T, true>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl,
+                                     reinterpret_cast<const uint4*>(rrow + ((c ^ (rl & 7)) << 4)),
+                                     reinterpret_cast<const uint4*>(rrow + (((c + 1) ^ (rl & 7)) << 4)));
+              } else {
+                epi_store16<T>(p, stg + er * EPI_LD + eh * 16, row0 + er, n0 + cl, sss + cl, sss + BN + cl);
+              }
             }
+          }
+        }
+        if constexpr (RES) {
+          if (m0 < p.M) {                        // this warp's last read of the tile is done: the producer may refill it
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&res_empty[cw]);
+            res_phase ^= 1;
           }
         }
       }
@@ -795,13 +871,13 @@ static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads,
 }
 
 // grid != nullptr: report the grid and the resident-cluster bound (grid[1]) instead of launching
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1>
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1, bool RES = false>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st,
                       int* grid = nullptr) {
-  using C = Cfg<BN, BKB, NC>;
+  using C = Cfg<BN, BKB, NC, RES>;
   static DeviceOnce once;
   static ClusterCapacity capacity;
-  auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN>;
+  auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int cs = p.cluster;
   if (PP && (p.cluster != CM * CN || p.cluster_n != CN)) {
@@ -830,15 +906,26 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv
 }
 
 // ping-pong: the kernel of the cluster shape (cluster / cluster_n) x cluster_n
-template <typename T, int BN, int BKB>
-static int launch_pp(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
+template <typename T, int BN, int BKB, bool RES>
+static int launch_pp_shape(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
   const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
-  if (cm == 1 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true>(tmA, tmB, p, st, grid);
-  if (cm == 2 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 1>(tmA, tmB, p, st, grid);
-  if (cm == 1 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 2>(tmA, tmB, p, st, grid);
-  if (cm == 2 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 2>(tmA, tmB, p, st, grid);
+  if (cm == 1 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 1, RES>(tmA, tmB, p, st, grid);
+  if (cm == 2 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 1, RES>(tmA, tmB, p, st, grid);
+  if (cm == 1 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 2, RES>(tmA, tmB, p, st, grid);
+  if (cm == 2 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 2, RES>(tmA, tmB, p, st, grid);
   set_error("conv: no ping-pong kernel for a %d x %d cluster", cm, cn);
   return YB_ERR_UNSUPPORTED;
+}
+// the shared-memory shortcut variant exists for the 128-column, 128-byte k-block tiles (every residual conv of the
+// network: the 3x3 convs of the darknet residual blocks); conv_select only picks it there
+template <typename T, int BN, int BKB>
+static int launch_pp(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
+  if (p.res_smem) {
+    if constexpr (BN == 128 && BKB == 128) return launch_pp_shape<T, BN, BKB, true>(tmA, tmB, p, st, grid);
+    set_error("conv: no shared-memory shortcut kernel for %d-column tiles with %d-byte k-blocks", BN, BKB);
+    return YB_ERR_UNSUPPORTED;
+  }
+  return launch_pp_shape<T, BN, BKB, false>(tmA, tmB, p, st, grid);
 }
 
 int conv_block_k(int cin) { return (cin % 64 == 0) ? 64 : 32; }
@@ -848,8 +935,10 @@ static int conv_block_kb(int cin, int dtype) {
   return 2 * conv_block_k(cin);
 }
 int conv_block_n(int cout_pad) { return (cout_pad % 128 == 0) ? 128 : 64; }
-// operand-ring depth of the kernel conv_launch runs for (block n, k-block row bytes, consumer warpgroups)
-static int conv_stages(int bn, int kb, int nc) {
+// operand-ring depth of the kernel conv_launch runs for (block n, k-block row bytes, consumer warpgroups, shortcut
+// tile in shared memory)
+static int conv_stages(int bn, int kb, int nc, bool res_smem = false) {
+  if (res_smem) return bn == 128 && kb == 128 && nc == 2 ? Cfg<128, 128, 2, true>::STAGES : 0;
 #define YB_STAGES(BN, KB) \
   if (bn == BN && kb == KB) return nc == 2 ? Cfg<BN, KB, 2>::STAGES : Cfg<BN, KB, 1>::STAGES;
   YB_STAGES(256, 128) YB_STAGES(128, 128) YB_STAGES(128, 64) YB_STAGES(64, 128) YB_STAGES(64, 64)
@@ -963,6 +1052,8 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   //                       small tests give every CTA and warpgroup many work units; the kernel is unchanged
   //   YB_CONV_MCAST=0|2x1|1x2|2x2   ping-pong multicast clusters (below): 0 off everywhere, AxB that shape on every
   //                       16-bit ping-pong launch; unset: the plan rule in inference plans, off elsewhere
+  //   YB_CONV_RES=ldg|smem  launches with a residual: ldg, the epilogue reads it from global memory; smem (or unset),
+  //                       the ping-pong kernel prefetches it into shared memory where it can (below)
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
   p->epi_reg = (!det && !stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
@@ -998,6 +1089,15 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
     p->cluster = cm * cn;
     p->cluster_n = cn;
   }
+  // Shortcut prefetch (conv_prepare_core clears it when the launch has no residual): the 16-bit ping-pong kernel with
+  // 128 x 128 tiles and 64-channel k-blocks, whose epilogue would otherwise wait one global load per 32-column chunk.
+  // The 4-stage operand ring it leaves costs nothing measurable at any residual layer of the network (DESIGN.md §5).
+  // Not for outputs stored elsewhere than at the residual's own row (2x upsample, dgrad parity scatter).
+  const char* ro = opt("YB_CONV_RES");
+  YB_REQUIRE(ro[0] == '\0' || strcmp(ro, "ldg") == 0 || strcmp(ro, "smem") == 0,
+             "conv: YB_CONV_RES must be ldg or smem (got '%s')", ro);
+  p->res_smem = (p->pingpong && !e4m3 && !det && bn == 128 && conv_block_kb(d->cin, d->dtype) == 128 && !scatter &&
+                 !d->upsample2x && !d->out_fp32 && strcmp(ro, "ldg") != 0) ? 1 : 0;
   memset(&p->det, 0, sizeof(p->det));
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
   p->kh = kh; p->kw = kw; p->scatter = scatter;
@@ -1030,6 +1130,12 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   p->scale = scale; p->shift = shift;
   p->out = out; p->out_ld = d->out_ld; p->res = res; p->res_ld = d->res_ld;
   p->stat_sum = stat_sum; p->stat_sqsum = stat_sqsum;
+  if (res == nullptr) p->res_smem = 0;
+  if (p->res_smem) {
+    // the shortcut as a [M, cout] matrix of row pitch res_ld: 128-row x 64-channel boxes, rows past M zero-filled
+    rc = make_tmap_2d(&p->tmR, res, d->dtype, p->M, d->cout, d->res_ld, 64 * p->consumers, 64, 0);
+    if (rc) return rc;
+  }
   if (p->im2col) {
     rc = make_tmap_im2col_px(tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride, pad, bk,
                              a_rows);
@@ -1110,6 +1216,8 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
   const int kb = yb::conv_block_kb(d->cin, d->dtype);
   info->block_k = kb / yb::tm_esize(d->dtype);
   info->stages = yb::conv_stages(info->block_n, kb, p.consumers);
+  info->res_smem = p.res_smem;
+  info->res_stages = p.res_smem ? yb::conv_stages(info->block_n, kb, p.consumers, true) : info->stages;
   info->num_kb = p.kh * p.kw * d->cin / info->block_k;
   info->num_m_tiles = p.num_m_tiles;
   info->num_n_tiles = p.num_n_tiles;

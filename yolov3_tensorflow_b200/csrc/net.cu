@@ -239,17 +239,22 @@ extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count,
   memset(info, 0, sizeof(*info));
   const Layer& L = net->layers[layer];
   if (layer == 0) return YB_OK;                        // the stem (fused into layer 1's halo kernel by default)
+  info->residual = L.res.buf >= 0 ? 1 : 0;
   const yb_conv_desc d = layer_desc(net, L);
   // the default dispatch of forward_layers_impl: the halo kernel for the Cin = 32 BN layers it supports (always for
   // the e4m3 plan's Conv_3), the implicit-GEMM conv for every other layer
   const char* hopt = opt("YB_HALO");
   if (L.info.has_bn && conv_halo_supported(&d) &&
-      ((net->dtype == YB_E4M3 && layer == FP8_FIRST_LAYER - 1) || (hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32))))
+      ((net->dtype == YB_E4M3 && layer == FP8_FIRST_LAYER - 1) || (hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)))) {
+    info->res_smem = info->residual && conv_halo_res_smem(&d);
     return YB_OK;
+  }
   ConvParams p;
   int rc = conv_schedule_params(&d, plan_mcast_rule(net), &p);
   if (rc) return rc;
+  if (!info->residual) p.res_smem = 0;                 // as conv_prepare_core decides it for a launch without one
   info->igemm = 1;
+  info->res_smem = p.res_smem;
   info->pingpong = p.pingpong;
   info->cluster_m = p.cluster / p.cluster_n;
   info->cluster_n = p.cluster_n;
