@@ -416,7 +416,7 @@ typedef struct yb_layer_schedule_info {
   int igemm;         /* 1: the implicit-GEMM conv                                                  */
   int pingpong;      /* 1: ping-pong schedule, 0: cooperative                                       */
   int cluster_m;     /* CTAs of a cluster along M (each a different m-tile)                         */
-  int cluster_n;     /* CTAs of a cluster along N (ping-pong multicast clusters only)               */
+  int cluster_n;     /* CTAs of a cluster along N (1 | 2; 1 under the cooperative schedule)         */
   int block_m, block_n;
   int num_m_tiles, num_n_tiles;
   int units;         /* work units: ceil(num_m_tiles / cluster_m) x num_n_tiles / cluster_n         */

@@ -6,7 +6,9 @@ one on the same operands, and within the float64 bound of tests/conv_ref.py.  Se
 columns outside a written channel slice must keep their sentinel.  Cases: every 3x3 and 1x1 conv shape of the 416^2
 inference plan at batch 8, the 52^2 3x3 layers at batch 64, residual, concat slice, 2x upsample, stride 2, an odd
 number of m-tiles (the last cluster half idle) and a grid capped to one cluster (every warpgroup wraps the ring many
-times).  Then the whole batch-64 detect step of the plan, multicast on against off."""
+times).  The cooperative schedule's clusters (YB_CONV_MODE=2cta, 2 x 1 or 4 x 1) share the same loads and release, so
+the plan shapes and the tails run them too, against the unclustered cooperative bits.  Then the whole batch-64 detect
+step of the plan, multicast on against off."""
 import ctypes as C
 
 import numpy as np
@@ -73,6 +75,28 @@ def _mcast_sweep(L, name, case, pp=None, cap=None, want_cluster=None):
               f"tiles {i.num_m_tiles}x{i.num_n_tiles} num_kb {i.num_kb} worst {worst:.3f}")
 
 
+def _coop_sweep(L, name, case, cap=None):
+    """The cooperative schedule unclustered, then in its 2 x 1 and 4 x 1 clusters (YB_CONV_MODE=2cta, YB_CONV_MC=1),
+    which load and release the ring like the ping-pong clusters: byte-identical outputs, float64 bound on the first."""
+    L.set_option("YB_CONV_PP", "0")
+    L.set_option("YB_CONV_CTAS", cap)
+    i0 = _schedule(L, case.desc)
+    assert i0.cluster == 1 and not i0.pingpong
+    buf, ssum, ssq = case.run()
+    base, worst = case.check(f"{name} coop", buf, ssum, ssq, R.units_per_warpgroup(i0), i0.grid)
+    for mc, cs in ((None, 2), ("1", 4)):
+        L.set_option("YB_CONV_MODE", "2cta")
+        L.set_option("YB_CONV_MC", mc)
+        i = _schedule(L, case.desc)
+        assert i.cluster == cs and not i.pingpong and i.grid % cs == 0, f"{name} coop {cs}: cluster {i.cluster}"
+        buf, _, _ = case.run()
+        assert torch.equal(_out(case, buf), base), f"{name} coop {cs}: output differs from the unclustered bits"
+        print(f"COOP {name} {cs}x1: grid {i.grid} tiles {i.num_m_tiles}x{i.num_n_tiles} num_kb {i.num_kb} "
+              f"worst {worst:.3f}")
+    L.set_option("YB_CONV_MODE", None)
+    L.set_option("YB_CONV_MC", None)
+
+
 DT = (torch.float16, torch.bfloat16)
 _dt_id = {torch.float16: "f16", torch.bfloat16: "bf16"}
 
@@ -108,6 +132,7 @@ def test_mcast_plan_shapes_bit_identical(L, name, dtype):
     _mcast_sweep(L, name, case)
     if k == 1 and not case.desc.out_fp32 and L.lib.yb_conv_cout_pad(cout) % 128 == 0:
         _mcast_sweep(L, name + " pp=1", case, pp="1")
+    _coop_sweep(L, name, case)
 
 
 @pytest.mark.parametrize("dtype", DT, ids=_dt_id.get)
@@ -129,6 +154,8 @@ def test_mcast_tails_and_capped_grid(L, cin, dtype):
     _mcast_sweep(L, f"tail cin{cin}", case)
     for cap in ("4", "2"):
         _mcast_sweep(L, f"tail cin{cin} cap{cap}", case, cap=cap)
+    _coop_sweep(L, f"tail cin{cin}", case)
+    _coop_sweep(L, f"tail cin{cin} cap4", case, cap="4")
     # stride 2, batch tail inside a tile
     case = FwdCase(L, 3, 20, 20, cin, 256, 3, 2, dtype=dtype, seed=cin + 1)
     _mcast_sweep(L, f"tail s2 cin{cin}", case, cap="4")

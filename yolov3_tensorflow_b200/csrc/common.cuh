@@ -206,20 +206,10 @@ __device__ __forceinline__ void cluster_sync_all() {   // every thread of every 
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 ra;\n"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// The same arrive with the default .release.cta semantics.  The consumers' stage release only has to follow their own
-// wgmma reads (already retired by wgmma.wait_group); a .cluster-scope release compiles to MEMBAR.ALL.GPU + ERRBAR per
-// arrive, which in the conv main loop stalls every k-block (DESIGN.md §5).
+// Arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster, with the default .release.cta
+// semantics.  The consumers' stage release only has to follow their own wgmma reads (already retired by
+// wgmma.wait_group); a .cluster-scope release compiles to MEMBAR.ALL.GPU + ERRBAR per arrive, which in the conv main
+// loop stalls every k-block (DESIGN.md §5).
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n"

@@ -14,9 +14,9 @@ struct ConvParams {
   int scatter;            // 0, or 1 + 2a + b: output pixel (p, q) is stored at (2p + a, 2q + b) of a [n, 2P, 2Q] grid
   int im2col;             // 1: A via im2col TMA, 0: A via 2D tiled TMA
   int consumers;          // consumer warpgroups per CTA: 64 output rows each (1 | 2)
-  int cluster;            // CTAs per cluster (1 | 2 | 4): cooperative, along M sharing one multicast weight tile;
-                          // ping-pong, (cluster / cluster_n) x cluster_n m x n tiles multicasting A and B
-  int cluster_n;          // CTAs of a cluster along N (1 | 2; 1 for the cooperative clusters)
+  int cluster;            // CTAs per cluster (1 | 2 | 4), both schedules: (cluster / cluster_n) x cluster_n m x n tiles,
+                          // each CTA multicasting its slice of the A tile along N and of the B tile along M
+  int cluster_n;          // CTAs of a cluster along N (1 | 2; conv_select gives the cooperative schedule 1)
   int epi_reg;            // 1: accumulator fragments stored straight from registers (no staging tile)
   int pingpong;           // 1: the two consumer warpgroups take whole tiles in turn (csrc/conv_igemm.cu)
   int ctas;               // > 0: the persistent grid is capped at this many CTAs (YB_CONV_CTAS; launch_cfg)

@@ -21,8 +21,8 @@
 //   ping-pong (the default): each consumer warpgroup owns whole 128 x BN tiles (two m64 wgmmas per k16 step) and the
 //     two take alternate work units.  A pair of named barriers hands the tensor cores from one warpgroup's main loop
 //     to the other's, so one warpgroup's epilogue runs while the other's MMAs run.
-//   cooperative (fused-decode detection heads, 1x1 convs with 128-column tiles, clusters, 1-warpgroup CTAs, register
-//     epilogue; conv_prepare_core chooses): the NC consumer warpgroups split
+//   cooperative (fused-decode detection heads, 1x1 convs with 128-column tiles, YB_CONV_MODE clusters, 1-warpgroup
+//     CTAs, register epilogue; conv_prepare_core chooses): the NC consumer warpgroups split
 //     every tile by rows (64 each), run the k-loop in lockstep and then the epilogue together.
 // The epilogue stages 32-column chunks of one 64-row accumulator block through shared memory so that each thread then
 // owns 16 consecutive channels of one pixel (two 16-byte stores per output row).  Ping-pong launches with a residual
@@ -87,35 +87,25 @@ struct ConvMma { using type = Wgmma<BN, std::is_same<T, __nv_bfloat16>::value, 0
 template <int BN>
 struct ConvMma<__nv_fp8_e4m3, BN> { using type = WgmmaE4M3<BN>; };
 
-// Work unit -> (m tile, n tile) of this CTA.  A cluster of p.cluster CTAs shares one n-tile (its weight tile is
-// multicast) and takes p.cluster consecutive m-tiles; rank r of the cluster takes the r-th (possibly past the last
-// m-tile: it still takes part in the multicast, its rows are all masked).  Inference walks n fastest (the A tiles
-// stay hot in L2 across their n tiles); with BN statistics on, m runs fastest so a CTA's tiles share their n tile
-// and its per-CTA column sums are flushed to global at most num_n_tiles times.
+// Work unit -> (m tile, n tile) of this CTA.  A cluster of CM x CN CTAs (CM = 0: p.cluster x 1, the shape read at run
+// time) takes a unit of CM consecutive m-tiles x CN consecutive n-tiles, and rank r = rm * CN + rn takes m-tile rm and
+// n-tile rn of it.  The host takes CN = 2 only where the n-tile count is even; ranks past the last m-tile still take
+// part in the multicasts, their rows all masked.  Inference walks n fastest (the A tiles stay hot in L2 across their
+// n tiles); with BN statistics on, m runs fastest so a CTA's tiles share their n tile and its per-CTA column sums are
+// flushed to global at most num_n_tiles times.
+template <int CM, int CN>
 __device__ __forceinline__ int num_units(const ConvParams& p) {
-  return (p.num_m_tiles + p.cluster - 1) / p.cluster * p.num_n_tiles;
-}
-__device__ __forceinline__ void unit_coords(const ConvParams& p, int unit, int rank, int& m_idx, int& n_idx) {
-  const int sm_tiles = (p.num_m_tiles + p.cluster - 1) / p.cluster;
-  int sm;
-  if (p.stat_sum != nullptr) { n_idx = unit / sm_tiles; sm = unit - n_idx * sm_tiles; }
-  else { sm = unit / p.num_n_tiles; n_idx = unit - sm * p.num_n_tiles; }
-  m_idx = sm * p.cluster + rank;
-}
-// Ping-pong multicast clusters of CM x CN CTAs: a unit is CM consecutive m-tiles x CN consecutive n-tiles (n-groups
-// fastest for inference, as above), and rank r = rm * CN + rn takes m-tile rm and n-tile rn of it.  The host takes
-// CN = 2 only where the n-tile count is even; ranks past the last m-tile take part in the multicasts, rows masked.
-template <int CM, int CN>
-__device__ __forceinline__ int num_units_mn(const ConvParams& p) {
-  return (p.num_m_tiles + CM - 1) / CM * (p.num_n_tiles / CN);
+  const int cm = CM ? CM : p.cluster;
+  return (p.num_m_tiles + cm - 1) / cm * (p.num_n_tiles / CN);
 }
 template <int CM, int CN>
-__device__ __forceinline__ void unit_coords_mn(const ConvParams& p, int unit, uint32_t rank, int& m_idx, int& n_idx) {
-  const int m_groups = (p.num_m_tiles + CM - 1) / CM, n_groups = p.num_n_tiles / CN;
+__device__ __forceinline__ void unit_coords(const ConvParams& p, int unit, uint32_t rank, int& m_idx, int& n_idx) {
+  const int cm = CM ? CM : p.cluster;
+  const int m_groups = (p.num_m_tiles + cm - 1) / cm, n_groups = p.num_n_tiles / CN;
   int mg, ng;
   if (p.stat_sum != nullptr) { ng = unit / m_groups; mg = unit - ng * m_groups; }
   else { mg = unit / n_groups; ng = unit - mg * n_groups; }
-  m_idx = mg * CM + (int)rank / CN;
+  m_idx = mg * cm + (int)rank / CN;
   n_idx = ng * CN + (int)rank % CN;
 }
 
@@ -356,21 +346,23 @@ static constexpr int MMA_TURN_BAR = 3;
 
 // DET_E = 5 + classes: detection head with the decode fused in.  PP: ping-pong schedule (NC = 2, staged epilogue, no
 // fused decode; see the top of the file).  BKB: bytes per k-block row (Cfg).
-// CM x CN (ping-pong only): a cluster of CM m-tiles x CN n-tiles.  Each CTA loads 1/CN of its A tile, multicast to the
+// CM x CN: a cluster of CM m-tiles x CN n-tiles, both schedules.  Each CTA loads 1/CN of its A tile, multicast to the
 // CN CTAs of its m-tile, and 1/CM of its B tile, multicast to the CM CTAs of its n-tile: every CTA still receives the
 // full STAGE_BYTES per k-block but reads only A_BYTES / CN + B_BYTES / CM of them from L2.  Each warpgroup computes
 // the same tiles with the same wgmma sequence as without the cluster, so the outputs are the same bit for bit.
+// CM = 0 (the cooperative launches): a p.cluster x 1 cluster, the shape read at run time, so that one instantiation
+// serves the YB_CONV_MODE clusters.  The ping-pong launches, which the inference plans cluster, keep the shape in the
+// template: as a run-time shape it cost their 3x3 layers 2-3 % (DESIGN.md §5).
 // RES (ping-pong, 16-bit, p.res != nullptr, YB_CONV_RES): the shortcut tile of every work unit is prefetched by TMA
 // (p.tmR) into its warpgroup's shared-memory tile while the unit's main loop runs, and the epilogue adds it from there
 // instead of waiting on a global load per 32-column chunk.  Each CTA loads its own tile (never multicast).
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1, bool RES = false>
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
   static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
-  static_assert(PP || (CM == 1 && CN == 1), "multicast cluster shapes are a ping-pong variant");
   static_assert(!RES || (PP && sizeof(T) == 2), "the shared-memory shortcut tile is a 16-bit ping-pong variant");
-  constexpr int MCS = CM * CN;                           // CTAs per ping-pong cluster
+  static_assert(CM != 0 || CN == 1, "a run-time cluster shape is p.cluster x 1");
   constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
   using C = Cfg<BN, BKB, NC, RES>;
   constexpr int BK = BKB / (int)sizeof(T);               // channels per k-block
@@ -398,8 +390,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       // every consumer warp that reads a stage arrives on that stage's empty barrier in every CTA of the cluster (any of
-      // them may multicast into it next): ping-pong, the 4 warps of the one warpgroup that read it, in each of MCS CTAs
-      mbar_init(&empty_bar[i], PP ? 4 * MCS : 4 * NC * p.cluster);
+      // them may multicast into it next): ping-pong, the 4 warps of the one warpgroup that read it
+      mbar_init(&empty_bar[i], 4 * (PP ? 1 : NC) * (CM ? CM * CN : p.cluster));
     }
     if constexpr (RES) {
       tma_prefetch_desc(&p.tmR);
@@ -413,12 +405,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   __syncthreads();
   if (p.cluster > 1) cluster_sync_all();                 // every peer's barriers exist before the first multicast
 
-  const int cs = PP ? MCS : p.cluster;                   // CTAs per cluster (1: no cluster, no multicast)
+  const int cm = CM ? CM : p.cluster;                    // cluster shape cm x CN
+  const int cs = cm * CN;                                // CTAs per cluster (1: no cluster, no multicast)
   const uint32_t rank = cs > 1 ? cluster_ctarank() : 0u;
   const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
-  int nunits;
-  if constexpr (MCS > 1) nunits = num_units_mn<CM, CN>(p);
-  else nunits = num_units(p);
+  const int nunits = num_units<CM, CN>(p);
   const int kb_per_tap = p.cin / BK;
   const int num_kb = p.kh * p.kw * kb_per_tap;
 
@@ -426,89 +417,49 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================== TMA producer =====================
     // One thread runs the whole loop: a k-block costs one barrier wait, one expect_tx and two TMA issues.  The filter
     // tap / channel-chunk coordinates are carried as counters instead of being divided out of the k-block index.
-    // In a cooperative cluster every CTA loads its own A tile and 1/cs of the shared weight tile, multicast to all cs
-    // CTAs.  In a CM x CN ping-pong cluster CTA (rm, rn) loads A rows [rn BLOCK_M / CN, +BLOCK_M / CN) — for a 3x3 conv
-    // an im2col box of BLOCK_M / CN pixels from output pixel m0 + rn BLOCK_M / CN — multicast to the CTAs (rm, *), and
-    // B rows [rm BN / CM, +BN / CM), multicast to the CTAs (*, rn).  The halves start on whole 8-row swizzle groups,
-    // so they land exactly where the whole-tile loads put them.
-    if constexpr (MCS > 1) {
-      if (threadIdx.x == 0) {
-        constexpr int A_ROWS = C::BLOCK_M / CN, B_ROWS = BN / CM;
-        const int rm = (int)rank / CN, rn = (int)rank % CN;
-        const uint16_t a_mask = (uint16_t)(((1u << CN) - 1u) << (rm * CN));
-        uint16_t b_mask = 0;
-#pragma unroll
-        for (int i = 0; i < CM; ++i) b_mask |= (uint16_t)(1u << (i * CN + rn));
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
-          int m_idx, n_idx;
-          unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
-          const int ma = m_idx * C::BLOCK_M + rn * A_ROWS;     // first row of this CTA's A slice
-          const int nb = n_idx * BN + rm * B_ROWS;             // first row of this CTA's B slice
-          const int q = ma % p.Q;
-          const int pp = (ma / p.Q) % p.P;
-          const int img = ma / (p.Q * p.P);
-          const int w_base = q * p.stride - p.pad;
-          const int h_base = pp * p.stride - p.pad;
-          int c0 = 0, tw = 0, th = 0, kcol = 0;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-            uint8_t* a_dst = sA + stage * C::A_BYTES + rn * A_ROWS * BKB;
-            uint8_t* b_dst = sB + stage * C::B_BYTES + rm * B_ROWS * BKB;
-            if constexpr (CN > 1) {
-              if (p.im2col)
-                tma_load_im2col_4d_multicast(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
-                                             (uint16_t)th, a_mask);
-              else
-                tma_load_2d_multicast(a_dst, &tmA, &full_bar[stage], c0, ma, a_mask);
-            } else {
-              if (p.im2col)
-                tma_load_im2col_4d(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw, (uint16_t)th);
-              else
-                tma_load_2d(a_dst, &tmA, &full_bar[stage], c0, ma);
-            }
-            if constexpr (CM > 1) tma_load_2d_multicast(b_dst, &tmB, &full_bar[stage], kcol, nb, b_mask);
-            else tma_load_2d(b_dst, &tmB, &full_bar[stage], kcol, nb);
-            c0 += BK; kcol += BK;
-            if (c0 == p.cin) { c0 = 0; if (++tw == p.kw) { tw = 0; ++th; } }
-            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    } else if (threadIdx.x == 0) {
+    // CTA (rm, rn) of a cm x CN cluster loads A rows [rn BLOCK_M / CN, +BLOCK_M / CN) — for a 3x3 conv an im2col box of
+    // BLOCK_M / CN pixels from output pixel m0 + rn BLOCK_M / CN — multicast to the CTAs (rm, *), and B rows
+    // [rm BN / cm, +BN / cm), multicast to the CTAs (*, rn); a load with one destination is a plain TMA load.  The
+    // slices start on whole 8-row swizzle groups, so they land exactly where the whole-tile loads put them.
+    if (threadIdx.x == 0) {
+      const int a_rows = C::BLOCK_M / CN, b_rows = BN / cm;
+      const int rm = (int)rank / CN, rn = (int)rank % CN;
+      const uint16_t a_mask = (uint16_t)(((1u << CN) - 1u) << (rm * CN));
+      uint16_t b_mask = 0;
+      for (int i = 0; i < cm; ++i) b_mask |= (uint16_t)(1u << (i * CN + rn));
       int stage = 0;
       uint32_t phase = 0;
-      const int b_rows = BN / cs;
-      const uint16_t mask = (uint16_t)((1u << cs) - 1u);
       for (int unit = cluster_id; unit < nunits; unit += num_clusters) {
         int m_idx, n_idx;
-        unit_coords(p, unit, rank, m_idx, n_idx);
-        const int m0 = m_idx * C::BLOCK_M;
-        const int n0 = n_idx * BN;
-        // first output pixel of the tile -> (image, row, col); base input pixel of the filter window
-        const int q = m0 % p.Q;
-        const int pp = (m0 / p.Q) % p.P;
-        const int img = m0 / (p.Q * p.P);
+        unit_coords<CM, CN>(p, unit, rank, m_idx, n_idx);
+        const int ma = m_idx * C::BLOCK_M + rn * a_rows;       // first row of this CTA's A slice
+        const int nb = n_idx * BN + rm * b_rows;               // first row of this CTA's B slice
+        // first output pixel of the slice -> (image, row, col); base input pixel of the filter window
+        const int q = ma % p.Q;
+        const int pp = (ma / p.Q) % p.P;
+        const int img = ma / (p.Q * p.P);
         const int w_base = q * p.stride - p.pad;
         const int h_base = pp * p.stride - p.pad;
         int c0 = 0, tw = 0, th = 0, kcol = 0;                  // channel chunk, tap (tw, th), column in the packed weights
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-          if (p.im2col) {
-            tma_load_im2col_4d(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
-                               (uint16_t)th);
+          uint8_t* a_dst = sA + stage * C::A_BYTES + rn * a_rows * BKB;
+          uint8_t* b_dst = sB + stage * C::B_BYTES + rm * b_rows * BKB;
+          if constexpr (CN > 1) {
+            if (p.im2col)
+              tma_load_im2col_4d_multicast(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw,
+                                           (uint16_t)th, a_mask);
+            else
+              tma_load_2d_multicast(a_dst, &tmA, &full_bar[stage], c0, ma, a_mask);
           } else {
-            tma_load_2d(sA + stage * C::A_BYTES, &tmA, &full_bar[stage], c0, m0);
+            if (p.im2col)
+              tma_load_im2col_4d(a_dst, &tmA, &full_bar[stage], c0, w_base, h_base, img, (uint16_t)tw, (uint16_t)th);
+            else
+              tma_load_2d(a_dst, &tmA, &full_bar[stage], c0, ma);
           }
-          if (cs == 1) {
-            tma_load_2d(sB + stage * C::B_BYTES, &tmB, &full_bar[stage], kcol, n0);
-          } else {
-            tma_load_2d_multicast(sB + stage * C::B_BYTES + rank * b_rows * BKB, &tmB, &full_bar[stage], kcol,
-                                  n0 + (int)rank * b_rows, mask);
-          }
+          if (cm > 1) tma_load_2d_multicast(b_dst, &tmB, &full_bar[stage], kcol, nb, b_mask);
+          else tma_load_2d(b_dst, &tmB, &full_bar[stage], kcol, nb);
           c0 += BK; kcol += BK;
           if (c0 == p.cin) { c0 = 0; if (++tw == p.kw) { tw = 0; ++th; } }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
@@ -526,8 +477,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         int j = 0;
         for (int unit = cluster_id; unit < nunits; unit += num_clusters, ++j) {
           int m_idx, n_idx;
-          if constexpr (MCS > 1) unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
-          else unit_coords(p, unit, rank, m_idx, n_idx);
+          unit_coords<CM, CN>(p, unit, rank, m_idx, n_idx);
           const int m0 = m_idx * C::BLOCK_M, n0 = n_idx * BN;
           if (m0 >= p.M) continue;
           const int w = j & 1;
@@ -556,16 +506,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (p.stat_sum != nullptr)
       for (int c = t; c < 2 * BN; c += 128) sst[c] = 0.f;   // (first read after the scale / shift barriers below)
     // a stage is released on the empty barrier of every CTA of the cluster: any of them may multicast into it next
+    // (unrolled over the largest cluster: no loop in the k-loop when the shape is a run-time one)
     auto release = [&](int st) {
       __syncwarp();
       if (lane == 0) {
-        if constexpr (MCS > 1) {
-#pragma unroll
-          for (int r = 0; r < MCS; ++r) mbar_arrive_remote(&empty_bar[st], (uint32_t)r);
-        } else if (cs == 1) {
+        if (cs == 1) {
           mbar_arrive(&empty_bar[st]);
         } else {
-          for (int r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
+#pragma unroll
+          for (int r = 0; r < 4; ++r)
+            if (r < cs) mbar_arrive_remote(&empty_bar[st], (uint32_t)r);
         }
       }
     };
@@ -586,8 +536,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const uint8_t* sres = sR + cw * C::RES_TILE_BYTES;   // RES: this warpgroup's shortcut tile
     for (int unit = cluster_id + (PP ? cw * num_clusters : 0); unit < nunits; unit += unit_step) {
       int m_idx, n_idx;
-      if constexpr (MCS > 1) unit_coords_mn<CM, CN>(p, unit, rank, m_idx, n_idx);
-      else unit_coords(p, unit, rank, m_idx, n_idx);
+      unit_coords<CM, CN>(p, unit, rank, m_idx, n_idx);
       const int m0 = m_idx * C::BLOCK_M;
       const int n0 = n_idx * BN;
       // Ping-pong: wait until the other warpgroup has issued the previous unit's main loop.  Besides keeping the two
@@ -871,7 +820,7 @@ static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads,
 }
 
 // grid != nullptr: report the grid and the resident-cluster bound (grid[1]) instead of launching
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 1, int CN = 1, bool RES = false>
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st,
                       int* grid = nullptr) {
   using C = Cfg<BN, BKB, NC, RES>;
@@ -880,8 +829,9 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv
   auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES>;
   { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
   const int cs = p.cluster;
-  if (PP && (p.cluster != CM * CN || p.cluster_n != CN)) {
-    set_error("conv: ping-pong cluster %d (%d along N) launched as %d x %d", p.cluster, p.cluster_n, CM, CN);
+  // the cluster shapes the kernel's slices and masks support
+  if (CM ? (cs != CM * CN || p.cluster_n != CN) : ((cs != 1 && cs != 2 && cs != 4) || p.cluster_n != 1)) {
+    set_error("conv: cluster of %d CTAs (%d along N) launched on the %d x %d kernel", cs, p.cluster_n, CM, CN);
     return YB_ERR_INVALID_ARGUMENT;
   }
   int max_clusters = num_sms();
@@ -977,7 +927,7 @@ static int conv_launch_impl(int dtype, int cout_pad, const CUtensorMap& tmA, con
   // e4m3: two consumer warpgroups, no cluster (conv_select), so only the ping-pong and cooperative NC = 2 kernels exist
 #define YB_DISPATCH_E4M3(BN, KB)                                                                       \
   if (bn == BN && kb == KB) {                                                                          \
-    if (p.pingpong) return launch_cfg<__nv_fp8_e4m3, BN, KB, 2, 0, true>(tmA, tmB, p, st, grid);            \
+    if (p.pingpong) return launch_cfg<__nv_fp8_e4m3, BN, KB, 2, 0, true, 1, 1>(tmA, tmB, p, st, grid);      \
     return launch_cfg<__nv_fp8_e4m3, BN, KB, 2>(tmA, tmB, p, st, grid);                                      \
   }
   if (dtype == YB_E4M3 && nc == 2 && p.cluster == 1) {
@@ -1042,7 +992,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   p->M = d->n * P * Q; p->P = P; p->Q = Q;
   // Kernel variants (testing / A-B switches; the detection heads always take the default):
   //   YB_CONV_EG=1        one consumer warpgroup per CTA (64-row tiles) instead of two (128-row tiles)
-  //   YB_CONV_MODE=2cta   clusters of 2 CTAs (YB_CONV_MC=1: 4) along M sharing one TMA-multicast weight tile
+  //   YB_CONV_MODE=2cta   cooperative clusters of 2 x 1 CTAs (YB_CONV_MC=1: 4 x 1), multicasting the weight tile
   //   YB_CONV_EPI=reg     accumulators stored straight from registers (not with BN statistics: those sum columns
   //                       over the staging tile)
   //   YB_CONV_PP=0|1      0: the cooperative schedule wherever ping-pong would run; 1: ping-pong wherever the kernel
@@ -1069,8 +1019,8 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   const int block_m = 64 * p->consumers;
   p->num_m_tiles = ceil_div(p->M, block_m);
   p->num_n_tiles = cout_pad / bn;
-  // Ping-pong multicast clusters, CM m-tiles x CN n-tiles (csrc/conv_igemm.cu, DESIGN.md §4): each CTA reads 1/CN of
-  // its im2col / activation tile and 1/CM of its weight tile from L2.  The plan rule (16-bit inference plans, forward
+  // Ping-pong clusters, CM m-tiles x CN n-tiles (conv_igemm_kernel, DESIGN.md §4): each CTA reads 1/CN of its
+  // im2col / activation tile and 1/CM of its weight tile from L2.  The plan rule (16-bit inference plans, forward
   // layers without statistics): 2 x 2 for the windowed convs with an even n-tile count, 2 x 1 for the other windowed
   // convs; the 1x1 convs, whose activation tile comes from HBM once anyway, stay unclustered.  CN = 2 only where the
   // n-tile count is even (a forced 1x2 / 2x2 falls back to 1x1 / 2x1 elsewhere).
