@@ -19,7 +19,7 @@ struct ConvParams {
   int cluster_n;          // CTAs of a cluster along N (1 | 2; conv_select gives the cooperative schedule 1)
   int epi_reg;            // 1: accumulator fragments stored straight from registers (no staging tile)
   int pingpong;           // 1: the two consumer warpgroups take whole tiles in turn (csrc/conv_igemm.cu)
-  int ctas;               // > 0: the persistent grid is capped at this many CTAs (YB_CONV_CTAS; launch_cfg)
+  int ctas;               // > 0: the persistent grid is capped at this many CTAs (YB_CONV_CTAS; conv_grid)
   int num_m_tiles, num_n_tiles;
   const float* scale;     // [cout_pad]
   const float* shift;     // [cout_pad]
@@ -35,25 +35,31 @@ struct ConvParams {
   float res_scale, out_inv_scale;
   int res_smem;           // 1: the ping-pong kernel TMA-prefetches the residual tile into shared memory (YB_CONV_RES)
   CUtensorMap tmR;        // res_smem: the residual as a [M, cout] matrix, 128-row x 64-channel 128B-swizzled boxes
+  // The rest of the conv_igemm_kernel instantiation conv_select picks (consumers, pingpong, cluster, cluster_n and
+  // res_smem above are the others); host only, after every field the kernel reads.
+  int dtype;              // yb_dtype of the operands
+  int block_n;            // output channels per tile
+  int block_kb;           // bytes of one k-block row
+  int det_e;              // > 0: the fused-decode head kernel for 5 + C = det_e columns per anchor
 };
 
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
                  const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
-                 ConvParams* p, int* cout_pad_out);
+                 ConvParams* p);
 // conv_prepare of a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
 // YB_CONV_MCAST is unset (csrc/conv_igemm.cu)
 int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out);
-// the kernel choice of conv_prepare without pointers (no device work)
-int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, ConvParams* p);
+                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p);
+// the kernel choice of conv_prepare without pointers (no device work); has_res: the launch adds a residual
+int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, bool has_res, ConvParams* p);
 // Window variant used by the stride-2 dgrad: a kh x kw window whose taps sit at offsets (0..kh-1, 0..kw-1) from the
 // output pixel (zero-filled past the border), stride 1, output scattered to parity class `scatter`.
 // w_packed is [cout_pad][kh*kw*cin].
 int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const void* x, const void* w_packed,
                      const float* scale, const float* shift, const void* res, void* out, CUtensorMap* tmA,
-                     CUtensorMap* tmB, ConvParams* p, int* cout_pad_out);
+                     CUtensorMap* tmB, ConvParams* p);
 int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
-                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out);
+                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p);
 // halo-tile conv for the Cin <= 64 3x3 layers (csrc/conv_halo.cu)
 struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; CUtensorMap res; };
 struct HaloParams {
@@ -88,13 +94,13 @@ int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const floa
                            const float* stem_shift, const void* w_packed, const float* scale, const float* shift, void* out,
                            HaloMaps* maps, HaloParams* p);
 int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);
-int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
-                cudaStream_t st);
+int conv_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st);
 // what conv_launch would launch on the current device, without launching: grid (CTAs) and the most clusters of
 // p.cluster CTAs that can be resident at once (cudaOccupancyMaxActiveClusters; the SM count when p.cluster == 1)
-int conv_launch_grid(int dtype, int cout_pad, const ConvParams& p, int* grid, int* max_clusters);
+int conv_launch_grid(const ConvParams& p, int* grid, int* max_clusters);
 // the persistent grid for sms SMs of which at most max_clusters clusters are resident (<= 0: sms / cluster)
 int conv_grid(const ConvParams& p, int sms, int max_clusters);
-int conv_block_n(int cout_pad);   // 128 or 64 output channels per tile
+// work units: one per cluster of (cluster / cluster_n) m-tiles x cluster_n n-tiles
+int conv_units(const ConvParams& p);
 
 }  // namespace yb

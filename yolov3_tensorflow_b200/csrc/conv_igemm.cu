@@ -22,7 +22,7 @@
 //     two take alternate work units.  A pair of named barriers hands the tensor cores from one warpgroup's main loop
 //     to the other's, so one warpgroup's epilogue runs while the other's MMAs run.
 //   cooperative (fused-decode detection heads, 1x1 convs with 128-column tiles, YB_CONV_MODE clusters, 1-warpgroup
-//     CTAs, register epilogue; conv_prepare_core chooses): the NC consumer warpgroups split
+//     CTAs, register epilogue; conv_select chooses): the NC consumer warpgroups split
 //     every tile by rows (64 each), run the k-loop in lockstep and then the epilogue together.
 // The epilogue stages 32-column chunks of one 64-row accumulator block through shared memory so that each thread then
 // owns 16 consecutive channels of one pixel (two 16-byte stores per output row).  Ping-pong launches with a residual
@@ -777,12 +777,17 @@ int make_tmap_im2col_px(CUtensorMap* tm, const void* base, int dtype, int n, int
   return YB_OK;
 }
 
+// the host's count of num_units
+int conv_units(const ConvParams& p) {
+  return ceil_div(p.num_m_tiles, p.cluster / p.cluster_n) * (p.num_n_tiles / p.cluster_n);
+}
+
 // Persistent grid in CTAs: one cluster per work unit, at most one CTA per SM and at most max_clusters resident clusters
 // (cudaOccupancyMaxActiveClusters: an H100's GPCs hold 30, not 33, clusters of 4 of these CTAs), and at most p.ctas
 // CTAs (rounded down to whole clusters, at least one cluster) when YB_CONV_CTAS caps it.
 int conv_grid(const ConvParams& p, int sms, int max_active) {
-  const int cs = p.cluster, cn = p.cluster_n;
-  const int units = ceil_div(p.num_m_tiles, cs / cn) * (p.num_n_tiles / cn);
+  const int cs = p.cluster;
+  const int units = conv_units(p);
   int max_clusters = sms / cs;
   if (max_active > 0 && max_active < max_clusters) max_clusters = max_active;
   if (p.ctas > 0) {
@@ -819,147 +824,138 @@ static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads,
   return YB_OK;
 }
 
-// grid != nullptr: report the grid and the resident-cluster bound (grid[1]) instead of launching
+// One conv_igemm_kernel instantiation: the type conv_kernel_for passes to its functor
 template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false>
-static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st,
-                      int* grid = nullptr) {
+struct ConvKernel {
   using C = Cfg<BN, BKB, NC, RES>;
+  static constexpr auto kernel = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES>;
+};
+
+static int no_conv_kernel(const ConvParams& p) {
+  set_error("conv: no kernel for dtype %d, %d-column tiles, %d-byte k-blocks, %d consumer warpgroups, ping-pong %d, "
+            "%d x %d cluster, shortcut tile %d, fused decode of %d columns", p.dtype, p.block_n, p.block_kb, p.consumers,
+            p.pingpong, p.cluster / p.cluster_n, p.cluster_n, p.res_smem, p.det_e);
+  return YB_ERR_UNSUPPORTED;
+}
+
+// ping-pong: the cluster shape (cluster / cluster_n) x cluster_n is a template parameter; e4m3 runs unclustered
+template <typename T, int BN, int BKB, bool RES, typename F>
+static int conv_kernel_pp(const ConvParams& p, F& f) {
+  const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
+  if (cm == 1 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 1, RES>());
+  if constexpr (sizeof(T) == 2) {
+    if (cm == 2 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 1, RES>());
+    if (cm == 1 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 2, RES>());
+    if (cm == 2 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 2, RES>());
+  }
+  return no_conv_kernel(p);
+}
+
+template <typename T, int BN, int BKB, int DET_E, typename F>
+static int conv_kernel_tile(const ConvParams& p, F& f) {
+  constexpr bool b16 = sizeof(T) == 2;
+  if (p.pingpong) {
+    if constexpr (DET_E == 0) {
+      if (!p.res_smem) return conv_kernel_pp<T, BN, BKB, false>(p, f);
+      // the shared-memory shortcut tile: the 128-column, 128-byte k-block tiles of the 16-bit residual convs
+      if constexpr (b16 && BN == 128 && BKB == 128) return conv_kernel_pp<T, BN, BKB, true>(p, f);
+    }
+    return no_conv_kernel(p);
+  }
+  // cooperative: one instantiation serves every p.cluster x 1 cluster (CM = 0); 16-bit: 2 and 4 CTAs and one consumer
+  // warpgroup as well
+  const bool shape = p.cluster_n == 1 && (p.cluster == 1 || (b16 && (p.cluster == 2 || p.cluster == 4)));
+  if (!shape || p.res_smem) return no_conv_kernel(p);
+  if (p.consumers == 2) return f(ConvKernel<T, BN, BKB, 2, DET_E>());
+  if constexpr (b16 && DET_E == 0) {
+    if (p.consumers == 1) return f(ConvKernel<T, BN, BKB, 1>());
+  }
+  return no_conv_kernel(p);
+}
+
+template <typename T, typename F>
+static int conv_kernel_type(const ConvParams& p, F& f) {
+  const int bn = p.block_n, kb = p.block_kb;
+  if (p.det_e) {
+    // detection heads with the decode fused in: one n-tile holding all 3 * E columns
+    if (p.det_e == 85 && bn == 256 && kb == 128) return conv_kernel_tile<T, 256, 128, 85>(p, f);
+    if (p.det_e == 25 && bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, 25>(p, f);
+    return no_conv_kernel(p);
+  }
+  if (bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, 0>(p, f);
+  if (bn == 128 && kb == 64) return conv_kernel_tile<T, 128, 64, 0>(p, f);
+  if (bn == 64 && kb == 128) return conv_kernel_tile<T, 64, 128, 0>(p, f);
+  if (bn == 64 && kb == 64) return conv_kernel_tile<T, 64, 64, 0>(p, f);
+  return no_conv_kernel(p);
+}
+
+// The instantiation table: every conv_igemm_kernel that exists is named here and nowhere else.  Calls
+// f(ConvKernel<...>()) with the instantiation of the schedule conv_select recorded in p and returns what f returns, or
+// YB_ERR_UNSUPPORTED when there is none.  conv_select, the launch, the grid query and yb_conv_schedule's ring depth all
+// look kernels up here.
+template <typename F>
+static int conv_kernel_for(const ConvParams& p, F&& f) {
+  if (p.dtype == YB_F16) return conv_kernel_type<__half>(p, f);
+  if (p.dtype == YB_BF16) return conv_kernel_type<__nv_bfloat16>(p, f);
+  if (p.dtype == YB_E4M3) return conv_kernel_type<__nv_fp8_e4m3>(p, f);
+  return no_conv_kernel(p);
+}
+
+// the persistent grid of kernel K for p on the current device, and the most clusters of p.cluster CTAs resident at once
+template <typename K>
+static int conv_kernel_grid(const ConvParams& p, int* grid, int* max_clusters) {
   static DeviceOnce once;
   static ClusterCapacity capacity;
-  auto kern = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES>;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-  const int cs = p.cluster;
-  // the cluster shapes the kernel's slices and masks support
-  if (CM ? (cs != CM * CN || p.cluster_n != CN) : ((cs != 1 && cs != 2 && cs != 4) || p.cluster_n != 1)) {
-    set_error("conv: cluster of %d CTAs (%d along N) launched on the %d x %d kernel", cs, p.cluster_n, CM, CN);
-    return YB_ERR_INVALID_ARGUMENT;
-  }
-  int max_clusters = num_sms();
-  if (cs > 1) {
-    const int rc = cluster_capacity(capacity, reinterpret_cast<const void*>(kern), C::THREADS, C::SMEM_BYTES, cs, &max_clusters);
+  const void* kern = reinterpret_cast<const void*>(K::kernel);
+  int rc = ensure_smem_attr(once, kern, K::C::SMEM_BYTES);
+  if (rc) return rc;
+  *max_clusters = num_sms();
+  if (p.cluster > 1) {
+    rc = cluster_capacity(capacity, kern, K::C::THREADS, K::C::SMEM_BYTES, p.cluster, max_clusters);
     if (rc) return rc;
   }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(conv_grid(p, num_sms(), max_clusters));
-  if (grid) { grid[0] = (int)cfg.gridDim.x; grid[1] = max_clusters; return YB_OK; }
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
+  *grid = conv_grid(p, num_sms(), *max_clusters);
   return YB_OK;
 }
 
-// ping-pong: the kernel of the cluster shape (cluster / cluster_n) x cluster_n
-template <typename T, int BN, int BKB, bool RES>
-static int launch_pp_shape(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
-  const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
-  if (cm == 1 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 1, RES>(tmA, tmB, p, st, grid);
-  if (cm == 2 && cn == 1) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 1, RES>(tmA, tmB, p, st, grid);
-  if (cm == 1 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 1, 2, RES>(tmA, tmB, p, st, grid);
-  if (cm == 2 && cn == 2) return launch_cfg<T, BN, BKB, 2, 0, true, 2, 2, RES>(tmA, tmB, p, st, grid);
-  set_error("conv: no ping-pong kernel for a %d x %d cluster", cm, cn);
-  return YB_ERR_UNSUPPORTED;
-}
-// the shared-memory shortcut variant exists for the 128-column, 128-byte k-block tiles (every residual conv of the
-// network: the 3x3 convs of the darknet residual blocks); conv_select only picks it there
-template <typename T, int BN, int BKB>
-static int launch_pp(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st, int* grid) {
-  if (p.res_smem) {
-    if constexpr (BN == 128 && BKB == 128) return launch_pp_shape<T, BN, BKB, true>(tmA, tmB, p, st, grid);
-    set_error("conv: no shared-memory shortcut kernel for %d-column tiles with %d-byte k-blocks", BN, BKB);
-    return YB_ERR_UNSUPPORTED;
-  }
-  return launch_pp_shape<T, BN, BKB, false>(tmA, tmB, p, st, grid);
+// Launch with prebuilt tensor maps (used by the network plan)
+int conv_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
+  return conv_kernel_for(p, [&](auto k) -> int {
+    using K = decltype(k);
+    int grid = 0, max_clusters = 0;
+    const int rc = conv_kernel_grid<K>(p, &grid, &max_clusters);
+    if (rc) return rc;
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(K::C::THREADS);
+    cfg.dynamicSmemBytes = K::C::SMEM_BYTES;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = p.cluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    YB_CUDA(cudaLaunchKernelEx(&cfg, K::kernel, tmA, tmB, p));
+    return YB_OK;
+  });
 }
 
-int conv_block_k(int cin) { return (cin % 64 == 0) ? 64 : 32; }
+int conv_launch_grid(const ConvParams& p, int* grid, int* max_clusters) {
+  return conv_kernel_for(p, [&](auto k) -> int { return conv_kernel_grid<decltype(k)>(p, grid, max_clusters); });
+}
+
 // bytes of one k-block row: 64 / 32 channels of fp16 / bf16, 128 / 64 channels of e4m3
-static int conv_block_kb(int cin, int dtype) {
-  if (dtype == YB_E4M3) return (cin % 128 == 0) ? 128 : 64;
-  return 2 * conv_block_k(cin);
-}
-int conv_block_n(int cout_pad) { return (cout_pad % 128 == 0) ? 128 : 64; }
-// operand-ring depth of the kernel conv_launch runs for (block n, k-block row bytes, consumer warpgroups, shortcut
-// tile in shared memory)
-static int conv_stages(int bn, int kb, int nc, bool res_smem = false) {
-  if (res_smem) return bn == 128 && kb == 128 && nc == 2 ? Cfg<128, 128, 2, true>::STAGES : 0;
-#define YB_STAGES(BN, KB) \
-  if (bn == BN && kb == KB) return nc == 2 ? Cfg<BN, KB, 2>::STAGES : Cfg<BN, KB, 1>::STAGES;
-  YB_STAGES(256, 128) YB_STAGES(128, 128) YB_STAGES(128, 64) YB_STAGES(64, 128) YB_STAGES(64, 64)
-#undef YB_STAGES
-  return 0;
-}
-
-// Launch with prebuilt tensor maps (used by the network plan); grid != nullptr: report instead of launching.
-static int conv_launch_impl(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
-                            cudaStream_t st, int* grid) {
-  const int kb = conv_block_kb(p.cin, dtype);
-  if (p.det.on) {
-    // detection head with the decode fused in: one n-tile holding all 3 * E columns
-#define YB_DISPATCH_DET(T)                                                                             \
-  if (cout_pad == 256 && kb == 128 && p.det.E == 85) return launch_cfg<T, 256, 128, 2, 85>(tmA, tmB, p, st, grid); \
-  if (cout_pad == 128 && kb == 128 && p.det.E == 25) return launch_cfg<T, 128, 128, 2, 25>(tmA, tmB, p, st, grid);
-    if (dtype == YB_F16) { YB_DISPATCH_DET(__half) }
-    else if (dtype == YB_BF16) { YB_DISPATCH_DET(__nv_bfloat16) }
-    else if (dtype == YB_E4M3) { YB_DISPATCH_DET(__nv_fp8_e4m3) }
-#undef YB_DISPATCH_DET
-    set_error("conv_launch: no fused-decode kernel for %d classes (cout_pad %d, k-block %d bytes)", p.det.C, cout_pad, kb);
-    return YB_ERR_UNSUPPORTED;
-  }
-  const int bn = conv_block_n(cout_pad);
-  const int nc = p.consumers;
-#define YB_DISPATCH_BN_KB(T, BN, KB)                                                          \
-  if (bn == BN && kb == KB) {                                                                 \
-    if (p.pingpong) return launch_pp<T, BN, KB>(tmA, tmB, p, st, grid);                        \
-    return nc == 2 ? launch_cfg<T, BN, KB, 2>(tmA, tmB, p, st, grid) : launch_cfg<T, BN, KB, 1>(tmA, tmB, p, st, grid); \
-  }
-#define YB_DISPATCH(T)                                                       \
-  YB_DISPATCH_BN_KB(T, 128, 128) YB_DISPATCH_BN_KB(T, 128, 64) YB_DISPATCH_BN_KB(T, 64, 128) YB_DISPATCH_BN_KB(T, 64, 64)
-  if (dtype == YB_F16) { YB_DISPATCH(__half) }
-  else if (dtype == YB_BF16) { YB_DISPATCH(__nv_bfloat16) }
-#undef YB_DISPATCH
-  // e4m3: two consumer warpgroups, no cluster (conv_select), so only the ping-pong and cooperative NC = 2 kernels exist
-#define YB_DISPATCH_E4M3(BN, KB)                                                                       \
-  if (bn == BN && kb == KB) {                                                                          \
-    if (p.pingpong) return launch_cfg<__nv_fp8_e4m3, BN, KB, 2, 0, true, 1, 1>(tmA, tmB, p, st, grid);      \
-    return launch_cfg<__nv_fp8_e4m3, BN, KB, 2>(tmA, tmB, p, st, grid);                                      \
-  }
-  if (dtype == YB_E4M3 && nc == 2 && p.cluster == 1) {
-    YB_DISPATCH_E4M3(128, 128) YB_DISPATCH_E4M3(128, 64) YB_DISPATCH_E4M3(64, 128) YB_DISPATCH_E4M3(64, 64)
-  }
-#undef YB_DISPATCH_E4M3
-#undef YB_DISPATCH_BN_KB
-  set_error("conv_launch: unsupported dtype %d", dtype);
-  return YB_ERR_UNSUPPORTED;
-}
-
-int conv_launch(int dtype, int cout_pad, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p,
-                cudaStream_t st) {
-  return conv_launch_impl(dtype, cout_pad, tmA, tmB, p, st, nullptr);
-}
-
-int conv_launch_grid(int dtype, int cout_pad, const ConvParams& p, int* grid, int* max_clusters) {
-  CUtensorMap none;
-  memset(&none, 0, sizeof(none));
-  int g[2] = {0, 0};
-  const int rc = conv_launch_impl(dtype, cout_pad, none, none, p, nullptr, g);
-  *grid = g[0];
-  *max_clusters = g[1];
-  return rc;
-}
+static int conv_block_kb(int cin, int dtype) { return cin * tm_esize(dtype) % 128 == 0 ? 128 : 64; }
 
 // Shape checks, tiling and kernel variant of one conv: everything conv_prepare_core decides before it looks at the
-// data pointers.  yb_conv_schedule reports what this picks.
+// data pointers, down to the conv_igemm_kernel instantiation, which must exist.  yb_conv_schedule reports what this
+// picks.
 // win = 0: the forward rule (ksize x ksize, symmetric padding ksize/2); win = 1: kh x kw window at offsets >= 0.
-// det = 1: one n-tile spans the whole padded cout (the fused-decode detection heads).
-static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, int det, bool plan_rule,
-                       ConvParams* p) {
+// det = E > 0: the fused-decode detection head of E = 5 + C columns per anchor, one n-tile spanning the whole padded cout.
+// has_res: the launch adds a residual.
+static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, bool has_res, int det,
+                       bool plan_rule, ConvParams* p) {
   YB_REQUIRE(win || d->ksize == 1 || d->ksize == 3, "conv: ksize must be 1 or 3 (got %d)", d->ksize);
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2 (got %d)", d->stride);
   YB_REQUIRE(!(d->ksize == 1 && d->stride != 1), "conv: 1x1 stride-2 is not on the YOLOv3 path");
@@ -988,7 +984,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   const int P = d->h / d->stride, Q = d->w / d->stride;
   if (!win) { kh = d->ksize; kw = d->ksize; }
   const int pad = win ? 0 : d->ksize / 2;
-  const int bn = det ? cout_pad : conv_block_n(cout_pad);
+  const int bn = det ? cout_pad : (cout_pad % 128 == 0 ? 128 : 64);
   p->M = d->n * P * Q; p->P = P; p->Q = Q;
   // Kernel variants (testing / A-B switches; the detection heads always take the default):
   //   YB_CONV_EG=1        one consumer warpgroup per CTA (64-row tiles) instead of two (128-row tiles)
@@ -1039,14 +1035,18 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
     p->cluster = cm * cn;
     p->cluster_n = cn;
   }
-  // Shortcut prefetch (conv_prepare_core clears it when the launch has no residual): the 16-bit ping-pong kernel with
-  // 128 x 128 tiles and 64-channel k-blocks, whose epilogue would otherwise wait one global load per 32-column chunk.
+  // Shortcut prefetch for launches with a residual: the 16-bit ping-pong kernel with 128 x 128 tiles and 64-channel
+  // k-blocks, whose epilogue would otherwise wait one global load per 32-column chunk.
   // The 4-stage operand ring it leaves costs nothing measurable at any residual layer of the network (DESIGN.md §5).
   // Not for outputs stored elsewhere than at the residual's own row (2x upsample, dgrad parity scatter).
   const char* ro = opt("YB_CONV_RES");
   YB_REQUIRE(ro[0] == '\0' || strcmp(ro, "ldg") == 0 || strcmp(ro, "smem") == 0,
              "conv: YB_CONV_RES must be ldg or smem (got '%s')", ro);
-  p->res_smem = (p->pingpong && !e4m3 && !det && bn == 128 && conv_block_kb(d->cin, d->dtype) == 128 && !scatter &&
+  p->dtype = d->dtype;
+  p->block_n = bn;
+  p->block_kb = conv_block_kb(d->cin, d->dtype);
+  p->det_e = det;
+  p->res_smem = (has_res && p->pingpong && !e4m3 && !det && bn == 128 && p->block_kb == 128 && !scatter &&
                  !d->upsample2x && !d->out_fp32 && strcmp(ro, "ldg") != 0) ? 1 : 0;
   memset(&p->det, 0, sizeof(p->det));
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
@@ -1054,15 +1054,15 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   p->im2col = kh * kw > 1;
   p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
   p->res_scale = 1.f; p->out_inv_scale = 1.f;
-  return YB_OK;
+  return conv_kernel_for(*p, [](auto) -> int { return YB_OK; });
 }
 
 // Build maps + params for one conv.  x/w/out pointers are baked into maps/params.
 static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
                              const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
                              float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
-                             int* cout_pad_out, int det = 0, bool plan_rule = false) {
-  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, det, plan_rule, p);
+                             int det = 0, bool plan_rule = false) {
+  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, res != nullptr, det, plan_rule, p);
   if (rc) return rc;
   YB_REQUIRE(x && w_packed && out && (scale == nullptr) == (shift == nullptr), "conv: null pointer");   // scale = shift = NULL: identity
   YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 &&
@@ -1071,16 +1071,15 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
   if (res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0 && !d->out_fp32, "conv: res_ld %d invalid", d->res_ld);
   YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), "conv: stat_sum/stat_sqsum must both be given");
   const int cout_pad = yb_conv_cout_pad(d->cout);
-  const int bk = conv_block_kb(d->cin, d->dtype) / tm_esize(d->dtype);   // channels per k-block
+  const int bk = p->block_kb / tm_esize(d->dtype);   // channels per k-block
   const int pad = p->pad;
   kh = p->kh; kw = p->kw;
   // TMA boxes: this CTA's share of the A tile (1 / cluster_n of its rows) and of the B tile (1 / (cluster / cluster_n))
   const int a_rows = 64 * p->consumers / p->cluster_n;
-  const int b_rows = (det ? cout_pad : conv_block_n(cout_pad)) / (p->cluster / p->cluster_n);
+  const int b_rows = p->block_n / (p->cluster / p->cluster_n);
   p->scale = scale; p->shift = shift;
   p->out = out; p->out_ld = d->out_ld; p->res = res; p->res_ld = d->res_ld;
   p->stat_sum = stat_sum; p->stat_sqsum = stat_sqsum;
-  if (res == nullptr) p->res_smem = 0;
   if (p->res_smem) {
     // the shortcut as a [M, cout] matrix of row pitch res_ld: 128-row x 64-channel boxes, rows past M zero-filled
     rc = make_tmap_2d(&p->tmR, res, d->dtype, p->M, d->cout, d->res_ld, 64 * p->consumers, 64, 0);
@@ -1093,51 +1092,44 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
     rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, a_rows, bk, 0);
   }
   if (rc) return rc;
-  rc = make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, b_rows, bk, 1);
-  if (rc) return rc;
-  *cout_pad_out = cout_pad;
-  return YB_OK;
+  return make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, b_rows, bk, 1);
 }
 
 int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
                  const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
-                 ConvParams* p, int* cout_pad_out) {
-  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, tmA, tmB, p,
-                           cout_pad_out);
+                 ConvParams* p) {
+  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, tmA, tmB, p);
 }
 
 int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out) {
-  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p,
-                           cout_pad_out, 0, true);
+                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p) {
+  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p, 0, true);
 }
 
-int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, ConvParams* p) {
+int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, bool has_res, ConvParams* p) {
   memset(p, 0, sizeof(*p));
-  return conv_select(d, 0, 0, 0, 0, false, 0, plan_rule, p);
+  return conv_select(d, 0, 0, 0, 0, false, has_res, 0, plan_rule, p);
 }
 
 // Detection head with the decode fused into the epilogue (yb_net_detect): ONE n-tile that holds all 3 * (5 + C)
 // columns; `out` is never written.  YB_ERR_UNSUPPORTED when the class count has no kernel.
 int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
-                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p, int* cout_pad_out) {
+                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p) {
   const int E = 5 + class_num;
-  const int cout_pad = yb_conv_cout_pad(d->cout);
-  if (d->cout != 3 * E || conv_block_k(d->cin) != 64 || !((cout_pad == 256 && E == 85) || (cout_pad == 128 && E == 25))) {
-    set_error("fused decode: no kernel for %d classes", class_num);
+  if (d->cout != 3 * E) {
+    set_error("fused decode: %d output channels are not 3 x (5 + %d classes)", d->cout, class_num);
     return YB_ERR_UNSUPPORTED;
   }
   return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, nullptr, const_cast<void*>(x) /*unused*/, nullptr,
-                           nullptr, tmA, tmB, p, cout_pad_out, 1);
+                           nullptr, tmA, tmB, p, E);
 }
 
 int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const void* x, const void* w_packed,
                      const float* scale, const float* shift, const void* res, void* out, CUtensorMap* tmA,
-                     CUtensorMap* tmB, ConvParams* p, int* cout_pad_out) {
+                     CUtensorMap* tmB, ConvParams* p) {
   YB_REQUIRE(kh >= 1 && kh <= 2 && kw >= 1 && kw <= 2 && scatter >= 0 && scatter <= 4, "conv_prepare_win: bad window");
   YB_REQUIRE(d->stride == 1 && !d->out_fp32 && !d->upsample2x, "conv_prepare_win: stride-1, 16-bit, non-upsampled only");
-  return conv_prepare_core(d, 1, kh, kw, scatter, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p,
-                           cout_pad_out);
+  return conv_prepare_core(d, 1, kh, kw, scatter, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p);
 }
 
 }  // namespace yb
@@ -1154,20 +1146,27 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
     YB_REQUIRE(kh >= 1 && kh <= 2 && kw >= 1 && kw <= 2, "conv_schedule: bad window");
     YB_REQUIRE(d->stride == 1 && !with_stats, "conv_schedule: windows are stride-1 without statistics");
   }
-  yb::ConvParams p;
+  yb::ConvParams p;   // the launch without a residual, then pr: with one
   memset(&p, 0, sizeof(p));
-  const int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, 0, false, &p);
+  int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, false, 0, false, &p);
   if (rc) return rc;
+  yb::ConvParams pr = p;
+  rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, true, 0, false, &pr);
+  if (rc) return rc;
+  auto stages = [](const yb::ConvParams& q, int* s) {
+    return yb::conv_kernel_for(q, [&](auto k) -> int { *s = decltype(k)::C::STAGES; return YB_OK; });
+  };
+  rc = stages(p, &info->stages);
+  if (rc) return rc;
+  rc = stages(pr, &info->res_stages);
+  if (rc) return rc;
+  info->res_smem = pr.res_smem;
   info->pingpong = p.pingpong;
   info->consumers = p.consumers;
   info->cluster = p.cluster;
   info->block_m = 64 * p.consumers;
-  info->block_n = yb::conv_block_n(yb_conv_cout_pad(d->cout));
-  const int kb = yb::conv_block_kb(d->cin, d->dtype);
-  info->block_k = kb / yb::tm_esize(d->dtype);
-  info->stages = yb::conv_stages(info->block_n, kb, p.consumers);
-  info->res_smem = p.res_smem;
-  info->res_stages = p.res_smem ? yb::conv_stages(info->block_n, kb, p.consumers, true) : info->stages;
+  info->block_n = p.block_n;
+  info->block_k = p.block_kb / yb::tm_esize(d->dtype);
   info->num_kb = p.kh * p.kw * d->cin / info->block_k;
   info->num_m_tiles = p.num_m_tiles;
   info->num_n_tiles = p.num_n_tiles;
@@ -1181,10 +1180,9 @@ extern "C" int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w
   if (!d) { yb::set_error("conv: null descriptor"); return YB_ERR_INVALID_ARGUMENT; }
   CUtensorMap tmA, tmB;
   yb::ConvParams p;
-  int cout_pad = 0;
-  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, &tmA, &tmB, &p, &cout_pad);
+  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, &tmA, &tmB, &p);
   if (rc) return rc;
-  return yb::conv_launch(d->dtype, cout_pad, tmA, tmB, p, static_cast<cudaStream_t>(stream));
+  return yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
@@ -1195,12 +1193,11 @@ extern "C" int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const vo
              "conv_e4m3: scales must be positive and finite");
   CUtensorMap tmA, tmB;
   yb::ConvParams p;
-  int cout_pad = 0;
-  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, nullptr, nullptr, &tmA, &tmB, &p, &cout_pad);
+  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, nullptr, nullptr, &tmA, &tmB, &p);
   if (rc) return rc;
   p.res_scale = res_scale;
   p.out_inv_scale = 1.f / out_scale;
-  return yb::conv_launch(d->dtype, cout_pad, tmA, tmB, p, static_cast<cudaStream_t>(stream));
+  return yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int yb_conv2d_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
@@ -1216,12 +1213,11 @@ extern "C" int yb_conv2d_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int d
   for (int c = 0; c < 4; ++c) {
     CUtensorMap tmA, tmB;
     yb::ConvParams p;
-    int cout_pad = 0;
     int rc = yb::conv_prepare_win(&d, 1 + (c >> 1), 1 + (c & 1), 1 + c, dz,
                                   static_cast<const uint8_t*>(w_dgrad_s2) + woff[c] * 2, nullptr, nullptr, res, dx, &tmA,
-                                  &tmB, &p, &cout_pad);
+                                  &tmB, &p);
     if (rc) return rc;
-    rc = yb::conv_launch(d.dtype, cout_pad, tmA, tmB, p, static_cast<cudaStream_t>(stream));
+    rc = yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
   }
   return YB_OK;

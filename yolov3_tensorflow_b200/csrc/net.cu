@@ -200,6 +200,31 @@ static yb_conv_desc layer_desc(const yb_net* net, const Layer& L) {
 // the multicast-cluster rule of conv_select applies to the 16-bit inference plans (not training, not e4m3)
 static bool plan_mcast_rule(const yb_net* net) { return !net->training && net->dtype != YB_E4M3; }
 
+// What the forward launches for layer i.  It reads the options at every call: they may change between forwards of
+// one bound plan.  Layer 0 is FusedStem when layer 1's launch computes it; it then has no launch of its own.
+enum class LayerKernel { FusedStem, Stem, Thin, Halo, Igemm };
+static LayerKernel layer_kernel(const yb_net* net, int i) {
+  if (i == 0) return layer_kernel(net, 1) == LayerKernel::FusedStem ? LayerKernel::FusedStem : LayerKernel::Stem;
+  const Layer& L = net->layers[i];
+  // Cin = 32: 64-byte im2col rows halve the TMA line rate -> the mma.sync halo-tile kernel (csrc/conv_thin.cu), opt-in
+  // (YB_THIN=2); by default these layers take the tensor-core path
+  if (opt("YB_THIN")[0] == '2' && net->dtype != YB_E4M3 && L.info.ksize == 3 && L.info.cin == 32 && L.info.has_bn &&
+      !L.upsample)
+    return LayerKernel::Thin;
+  const yb_conv_desc d = layer_desc(net, L);
+  if (!conv_halo_supported(&d)) return LayerKernel::Igemm;
+  // halo-tile kernel: default on for Cin = 32, whose 64-byte im2col rows make the implicit GEMM TMA-row bound; the
+  // 64->128 layers leave room for only two halo stages beside their weights.  YB_HALO=0: never, YB_HALO=1: wherever
+  // supported.  The fp8 plan's Conv_3 always runs it: only it writes e4m3 from fp16.
+  const char* hopt = opt("YB_HALO");
+  // stem fused into Conv_1 (csrc/conv_halo.cu): layer 0's output is never written.  YB_STEM_FUSE=0: two launches.
+  if (i == 1 && L.info.cin == 32 && L.info.stride == 2 && hopt[0] != '0' && opt("YB_STEM_FUSE")[0] != '0')
+    return LayerKernel::FusedStem;
+  if ((net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1) || (hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)))
+    return LayerKernel::Halo;
+  return LayerKernel::Igemm;
+}
+
 __global__ void fill_kernel(float* p, int n, float v) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -237,38 +262,32 @@ extern "C" int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* in
 extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info) {
   YB_REQUIRE(net && info && layer >= 0 && layer < (int)net->layers.size() && sm_count >= 0, "layer_schedule: bad argument");
   memset(info, 0, sizeof(*info));
+  if (layer == 0) return YB_OK;                        // the stem
   const Layer& L = net->layers[layer];
-  if (layer == 0) return YB_OK;                        // the stem (fused into layer 1's halo kernel by default)
-  info->residual = L.res.buf >= 0 ? 1 : 0;
+  const LayerKernel k = layer_kernel(net, layer);
   const yb_conv_desc d = layer_desc(net, L);
-  // the default dispatch of forward_layers_impl: the halo kernel for the Cin = 32 BN layers it supports (always for
-  // the e4m3 plan's Conv_3), the implicit-GEMM conv for every other layer
-  const char* hopt = opt("YB_HALO");
-  if (L.info.has_bn && conv_halo_supported(&d) &&
-      ((net->dtype == YB_E4M3 && layer == FP8_FIRST_LAYER - 1) || (hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)))) {
-    info->res_smem = info->residual && conv_halo_res_smem(&d);
-    return YB_OK;
-  }
+  info->residual = L.res.buf >= 0 ? 1 : 0;
+  if (k == LayerKernel::Halo) info->res_smem = info->residual && conv_halo_res_smem(&d);
+  if (k != LayerKernel::Igemm) return YB_OK;           // the thin, halo and fused-stem kernels
   ConvParams p;
-  int rc = conv_schedule_params(&d, plan_mcast_rule(net), &p);
+  int rc = conv_schedule_params(&d, plan_mcast_rule(net), info->residual, &p);
   if (rc) return rc;
-  if (!info->residual) p.res_smem = 0;                 // as conv_prepare_core decides it for a launch without one
   info->igemm = 1;
   info->res_smem = p.res_smem;
   info->pingpong = p.pingpong;
   info->cluster_m = p.cluster / p.cluster_n;
   info->cluster_n = p.cluster_n;
   info->block_m = 64 * p.consumers;
-  info->block_n = conv_block_n(L.cout_pad);
+  info->block_n = p.block_n;
   info->num_m_tiles = p.num_m_tiles;
   info->num_n_tiles = p.num_n_tiles;
-  info->units = ceil_div(p.num_m_tiles, info->cluster_m) * (p.num_n_tiles / p.cluster_n);
+  info->units = conv_units(p);
   if (sm_count > 0) {
     info->max_clusters = sm_count / p.cluster;
     info->grid = conv_grid(p, sm_count, 0);
     return YB_OK;
   }
-  return conv_launch_grid(L.dtype, L.cout_pad, p, &info->grid, &info->max_clusters);
+  return conv_launch_grid(p, &info->grid, &info->max_clusters);
 }
 
 extern "C" int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes) {
@@ -290,7 +309,6 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
   for (size_t i = 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
     yb_conv_desc d = layer_desc(net, L);
-    int cp = 0;
     if (net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1) {
       // Conv_3 of the fp8 plan: fp16 in, e4m3 out, only the halo kernel has that form
       YB_REQUIRE(conv_halo_supported(&d), "bind: the e4m3 plan needs the halo kernel for layer %d (w %% 16 == 0)", (int)i);
@@ -300,8 +318,6 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
                                  &L.halo_maps, &L.halo_params);
       if (rc) return rc;
       L.halo_params.out_e4m3 = 1;
-      L.halo_ok = true;
-      L.prepared = false;
       continue;
     }
     const void* res = L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr;
@@ -309,26 +325,23 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
     const float* shift = reinterpret_cast<const float*>(net->par + L.shift);
     int rc = plan_mcast_rule(net)
                  ? conv_prepare_plan(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
-                                     &L.tmA, &L.tmB, &L.params, &cp)
+                                     &L.tmA, &L.tmB, &L.params)
                  : conv_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
-                                nullptr, nullptr, &L.tmA, &L.tmB, &L.params, &cp);
+                                nullptr, nullptr, &L.tmA, &L.tmB, &L.params);
     if (rc) return rc;
-    L.prepared = true;
-    L.halo_ok = false;
-    if (L.info.has_bn && conv_halo_supported(&d)) {
+    if (conv_halo_supported(&d)) {   // every layer layer_kernel may give the halo kernel
       L.halo_desc = d;
       rc = conv_halo_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, reinterpret_cast<const float*>(net->par + L.scale),
                              reinterpret_cast<const float*>(net->par + L.shift),
                              L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), &L.halo_maps, &L.halo_params);
       if (rc) return rc;
-      L.halo_ok = true;
     }
     if (!L.info.has_bn) {
       // fused-decode variant of the head (yb_net_detect); class counts without a kernel keep the unfused pipeline
       L.det_ok = conv_prepare_det(&d, net->class_num, ten_ptr(net, L.in), net->par + L.w_packed,
                                   reinterpret_cast<const float*>(net->par + L.scale),
-                                  reinterpret_cast<const float*>(net->par + L.shift), &L.det_tmA, &L.det_tmB, &L.det_params,
-                                  &L.det_cout_pad) == YB_OK;
+                                  reinterpret_cast<const float*>(net->par + L.shift), &L.det_tmA, &L.det_tmB,
+                                  &L.det_params) == YB_OK;
     }
   }
   if (net->fp8_ready) apply_fp8_scales(net);
@@ -414,7 +427,6 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
   YB_REQUIRE(first >= 0 && first <= last, "forward: bad layer range");
   YB_REQUIRE(net->dtype != YB_E4M3 || net->fp8_ready,
              "forward: the e4m3 plan has no activation scales (yb_net_set_fp8_amax after calibration)");
-  const bool fp8 = net->dtype == YB_E4M3;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* user_fm[3] = {fm1, fm2, fm3};
   if (net->fold_dirty) {   // BN parameters / moving statistics changed by a training step: refold for inference
@@ -430,62 +442,40 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
     YB_CUDA(cudaEventCreateWithFlags(&net->side_fork, cudaEventDisableTiming));
     YB_CUDA(cudaEventCreateWithFlags(&net->side_join, cudaEventDisableTiming));
   }
-  // stem fused into Conv_1 (csrc/conv_halo.cu): layer 0's output is never written.  YB_STEM_FUSE=0: two launches.
-  // (a layer range that stops at layer 0 then launches nothing: the stem no longer exists as a launch of its own)
-  const bool fuse_stem = opt("YB_STEM_FUSE")[0] != '0' && net->layers.size() > 1 && net->layers[1].halo_ok &&
-                         net->layers[1].info.cin == 32 && net->layers[1].info.stride == 2 && opt("YB_HALO")[0] != '0';
-  if (first == 0 && !fuse_stem) {
-    Layer& L = net->layers[0];
-    int rc;
-    if (thin)
-      rc = yb_stem_conv_fwd_tc(images, reinterpret_cast<const float*>(net->par + L.w_master),
-                               reinterpret_cast<const float*>(net->par + L.scale),
-                               reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.dtype, 1,
-                               ten_ptr(net, L.out), stream);
-    else
-      rc = yb_stem_conv_fwd(images, reinterpret_cast<const float*>(net->par + L.w_master),
-                            reinterpret_cast<const float*>(net->par + L.scale),
-                            reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.info.cout,
-                            L.dtype, 1, ten_ptr(net, L.out), stream);
-    if (rc) return rc;
-  }
-  for (size_t i = first > 1 ? first : 1; i < net->layers.size() && (int)i <= last; ++i) {
+  for (size_t i = first; i < net->layers.size() && (int)i <= last; ++i) {
     Layer& L = net->layers[i];
-    // the mma.sync halo kernel for the Cin = 32 layers is opt-in (YB_THIN=2); by default they take the tensor-core path
-    const bool thin_cin32 = opt("YB_THIN")[0] == '2' && !fp8;
-    if (thin_cin32 && L.info.ksize == 3 && L.info.cin == 32 && L.info.has_bn && !L.upsample) {
-      // Cin = 32: 64-byte im2col rows halve the TMA line rate -> direct halo-tile kernel (csrc/conv_thin.cu)
-      yb_conv_desc d;
-      memset(&d, 0, sizeof(d));
-      d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = 32; d.cout = L.info.cout; d.ksize = 3;
-      d.stride = L.info.stride; d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = net->bufs[L.out.buf].ld;
-      d.res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0; d.dtype = net->dtype; d.leaky = 1;
-      int rc = yb_conv3x3_thin_fwd(&d, ten_ptr(net, L.in), net->par + L.w_packed,
-                                   reinterpret_cast<const float*>(net->par + L.scale),
-                                   reinterpret_cast<const float*>(net->par + L.shift),
-                                   L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), stream);
-      if (rc) return rc;
-      continue;
-    }
-    if (i == 1 && fuse_stem && first <= 1) {
-      Layer& L0 = net->layers[0];
-      HaloMaps hm;
-      HaloParams hp;
-      int rc = conv_stem_halo_prepare(&L.halo_desc, images, reinterpret_cast<const float*>(net->par + L0.w_master),
-                                      reinterpret_cast<const float*>(net->par + L0.scale),
-                                      reinterpret_cast<const float*>(net->par + L0.shift), net->par + L.w_packed,
-                                      reinterpret_cast<const float*>(net->par + L.scale),
-                                      reinterpret_cast<const float*>(net->par + L.shift), ten_ptr(net, L.out), &hm, &hp);
-      if (rc) return rc;
-      rc = conv_stem_halo_launch(&L.halo_desc, hm, hp, st);
-      if (rc) return rc;
-      continue;
-    }
-    // halo-tile kernel: default on for Cin = 32, whose 64-byte im2col rows make the implicit GEMM TMA-row bound; the
-    // 64->128 layers leave room for only two halo stages beside their weights.  YB_HALO=0: never, YB_HALO=1: wherever supported.
-    const char* hopt = opt("YB_HALO");
-    if (L.halo_ok && ((hopt[0] != '0' && (hopt[0] == '1' || L.info.cin == 32)) || !L.prepared)) {
-      int rc = conv_halo_launch(&L.halo_desc, L.halo_maps, L.halo_params, st);
+    const LayerKernel k = layer_kernel(net, (int)i);
+    if (k != LayerKernel::Igemm) {   // (layer 0 under FusedStem: nothing, layer 1's launch computes it)
+      int rc = YB_OK;
+      if (k == LayerKernel::Stem && thin) {
+        rc = yb_stem_conv_fwd_tc(images, reinterpret_cast<const float*>(net->par + L.w_master),
+                                 reinterpret_cast<const float*>(net->par + L.scale),
+                                 reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.dtype, 1,
+                                 ten_ptr(net, L.out), stream);
+      } else if (k == LayerKernel::Stem) {
+        rc = yb_stem_conv_fwd(images, reinterpret_cast<const float*>(net->par + L.w_master),
+                              reinterpret_cast<const float*>(net->par + L.scale),
+                              reinterpret_cast<const float*>(net->par + L.shift), net->n, net->h, net->w, L.info.cout,
+                              L.dtype, 1, ten_ptr(net, L.out), stream);
+      } else if (k == LayerKernel::Thin) {
+        const yb_conv_desc d = layer_desc(net, L);
+        rc = yb_conv3x3_thin_fwd(&d, ten_ptr(net, L.in), net->par + L.w_packed,
+                                 reinterpret_cast<const float*>(net->par + L.scale),
+                                 reinterpret_cast<const float*>(net->par + L.shift),
+                                 L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), stream);
+      } else if (k == LayerKernel::FusedStem && i == 1) {
+        Layer& L0 = net->layers[0];
+        HaloMaps hm;
+        HaloParams hp;
+        rc = conv_stem_halo_prepare(&L.halo_desc, images, reinterpret_cast<const float*>(net->par + L0.w_master),
+                                    reinterpret_cast<const float*>(net->par + L0.scale),
+                                    reinterpret_cast<const float*>(net->par + L0.shift), net->par + L.w_packed,
+                                    reinterpret_cast<const float*>(net->par + L.scale),
+                                    reinterpret_cast<const float*>(net->par + L.shift), ten_ptr(net, L.out), &hm, &hp);
+        if (rc == YB_OK) rc = conv_stem_halo_launch(&L.halo_desc, hm, hp, st);
+      } else if (k == LayerKernel::Halo) {
+        rc = conv_halo_launch(&L.halo_desc, L.halo_maps, L.halo_params, st);
+      }
       if (rc) return rc;
       continue;
     }
@@ -505,13 +495,13 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
           hs = net->side_stream;
           forked = true;
         }
-        int rc = conv_launch(L.dtype, L.det_cout_pad, L.det_tmA, L.det_tmB, dp, hs);
+        int rc = conv_launch(L.det_tmA, L.det_tmB, dp, hs);
         if (rc) return rc;
         continue;
       }
       p->out = user_fm[which] ? (void*)user_fm[which] : ten_ptr(net, L.out);
     }
-    int rc = conv_launch(L.dtype, L.cout_pad, L.tmA, L.tmB, *p, st);
+    int rc = conv_launch(L.tmA, L.tmB, *p, st);
     if (rc) return rc;
   }
   if (forked) {

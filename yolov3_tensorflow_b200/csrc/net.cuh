@@ -32,16 +32,13 @@ struct Layer {
   // prepared launch state
   CUtensorMap tmA, tmB;
   ConvParams params;
-  bool prepared = false;
   // Cin <= 64 3x3 layers: halo-tile kernel (csrc/conv_halo.cu), inference forward only
   HaloMaps halo_maps;
   HaloParams halo_params;
   yb_conv_desc halo_desc;
-  bool halo_ok = false;
   // detection heads: the same conv with the decode + NMS candidate filter fused into its epilogue (yb_net_detect)
   CUtensorMap det_tmA, det_tmB;
   ConvParams det_params;
-  int det_cout_pad = 0;
   bool det_ok = false;
   // ---- training plan (net_train.cu) ----
   size_t z_off = 0, dz_off = 0;      // raw conv output z / its gradient (activation arena); dz is zero-inserted for stride 2
@@ -49,7 +46,6 @@ struct Layer {
   int dgrad_parity = 0;              // stride-2 layer whose dgrad runs as 4 parity-class convs on the plain dz
   CUtensorMap d4_tmA[4], d4_tmB[4];
   ConvParams d4_params[4];
-  int d4_cout_pad[4] = {0, 0, 0, 0};
   size_t st_sum = 0, st_sqsum = 0, st_mean = 0, st_invstd = 0, st_scale = 0, st_shift = 0;   // fp32 [cout_pad] each
   size_t x_bwd = 0;                  // fp32 [2][cout_pad]: sync-BN backward exchange slab (sum dact*zhat | sum dact)
   size_t w_dgrad = 0;                // [cin_pad, k, k, k_cout] 16-bit (param arena)
@@ -57,7 +53,6 @@ struct Layer {
   ConvParams tparams;                // training-mode forward conv (raw z + statistics)
   CUtensorMap d_tmA, d_tmB;          // dgrad (forward kernel on dz with flipped/transposed weights)
   ConvParams dparams;
-  int d_cout_pad = 0;
 };
 
 }  // namespace yb

@@ -16,9 +16,6 @@
 
 namespace yb {
 
-int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                 const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
-                 ConvParams* p, int* cout_pad_out);
 // bn.cu: the BN kernels with the row count and the backward exchange slab exposed
 int bn_stats_act_apply_n(const void* z, long z_ld, const float* sum, const float* sqsum, long count, const float* gamma,
                          const float* beta, float eps, float decay, float* moving_mean, float* moving_var, float* scale,
@@ -185,9 +182,9 @@ int train_bind(yb_net* net, cudaStream_t st) {
     d.ksize = L.info.ksize; d.stride = L.info.stride;
     d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = L.info.cout; d.res_ld = 0;
     d.dtype = net->dtype; d.out_fp32 = 0; d.leaky = 0; d.upsample2x = 0;
-    CUtensorMap a, b; int cp = 0;
+    CUtensorMap a, b;
     int rc = conv_prepare(&d, ten_ptr2(net, L.in), net->par + L.w_packed, ones, zeros, nullptr, net->act + L.z_off,
-                          fact(net, L.st_sum), fact(net, L.st_sqsum), &a, &b, &L.tparams, &cp);
+                          fact(net, L.st_sum), fact(net, L.st_sqsum), &a, &b, &L.tparams);
     if (rc) return rc;
   }
   // ---- dgrad convs + residual bookkeeping (reverse order) ----
@@ -223,11 +220,10 @@ int train_bind(yb_net* net, cudaStream_t st) {
       const size_t woff[4] = {0, per, 3 * per, 5 * per};
       for (int c = 0; c < 4 && rc == YB_OK; ++c)
         rc = conv_prepare_win(&d, 1 + (c >> 1), 1 + (c & 1), 1 + c, net->act + L.dz_off, net->par + L.w_dgrad + woff[c] * esz,
-                              ones, zeros, res, gten_ptr(net, L.in), &L.d4_tmA[c], &L.d4_tmB[c], &L.d4_params[c],
-                              &L.d4_cout_pad[c]);
+                              ones, zeros, res, gten_ptr(net, L.in), &L.d4_tmA[c], &L.d4_tmB[c], &L.d4_params[c]);
     } else {
       rc = conv_prepare(&d, net->act + L.dz_off, net->par + L.w_dgrad, ones, zeros, res, gten_ptr(net, L.in), nullptr,
-                        nullptr, &L.d_tmA, &L.d_tmB, &L.dparams, &L.d_cout_pad);
+                        nullptr, &L.d_tmA, &L.d_tmB, &L.dparams);
     }
     if (rc) return rc;
     written[L.in.buf].push_back({L.in.off, L.in.c});
@@ -346,7 +342,7 @@ static int train_fwd_layer(yb_net* net, int i, int phase, const float* images, i
       p.out = user_fm[which] ? (void*)user_fm[which] : (void*)(net->act + net->bufs[L.out.buf].offset);
       net->train_fm[which] = static_cast<float*>(p.out);
     }
-    return conv_launch(dt, L.cout_pad, L.tmA, L.tmB, p, st);
+    return conv_launch(L.tmA, L.tmB, p, st);
   }
   if (!L.info.has_bn) return YB_OK;
   if (!bn_frozen) net->fold_dirty = true;
@@ -460,12 +456,12 @@ static int train_bwd_layer(yb_net* net, int i, int phase, const float* images, i
   if (rc) return rc;
   if (L.dgrad_parity) {
     for (int c = 0; c < 4; ++c) {
-      rc = conv_launch(dt, L.d4_cout_pad[c], L.d4_tmA[c], L.d4_tmB[c], L.d4_params[c], st);
+      rc = conv_launch(L.d4_tmA[c], L.d4_tmB[c], L.d4_params[c], st);
       if (rc) return rc;
     }
     return YB_OK;
   }
-  return conv_launch(dt, L.d_cout_pad, L.d_tmA, L.d_tmB, L.dparams, st);
+  return conv_launch(L.d_tmA, L.d_tmB, L.dparams, st);
 }
 
 // Position of (layer, phase) in the layered step: forward 0..L-1 (LOCAL, GLOBAL each), the loss, backward L-1..0.
