@@ -101,9 +101,8 @@ int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const void* w_packe
 /* Host-only: the implicit-GEMM kernel and persistent grid yb_conv2d_fwd would launch for `d` with the current options
  * (yb_set_option: YB_CONV_EG, YB_CONV_MODE, YB_CONV_EPI, YB_CONV_PP, YB_CONV_CTAS) on a device with sm_count SMs.
  * kh = kw = 0: the forward ksize x ksize window; kh, kw in {1, 2}: one parity class of yb_conv2d_dgrad_s2 (d = its
- * stride-1 descriptor over dz).  with_stats: BN statistics requested.  Work units = ceil(num_m_tiles / cluster) x
- * num_n_tiles; the CTAs of the grid take them round-robin, and under ping-pong the two consumer warpgroups of a CTA
- * take every other one of the CTA's units. */
+ * stride-1 descriptor over dz).  with_stats: BN statistics requested.  The clusters of the grid take the work units
+ * round-robin, and under ping-pong the two consumer warpgroups of a CTA take every other one of its cluster's units. */
 typedef struct yb_conv_schedule_info {
   int pingpong;      /* 1: ping-pong (each consumer warpgroup owns whole tiles), 0: cooperative */
   int consumers;     /* consumer warpgroups per CTA                                             */
@@ -115,6 +114,9 @@ typedef struct yb_conv_schedule_info {
   int grid;          /* CTAs launched                                                           */
   int res_smem;      /* 1: a launch with a residual prefetches it into shared memory (YB_CONV_RES) */
   int res_stages;    /* operand-ring depth of a launch with a residual                          */
+  int cluster_m;     /* CTAs of a cluster along M (each a different m-tile)                     */
+  int cluster_n;     /* CTAs of a cluster along N (1 | 2; 1 under the cooperative schedule)     */
+  int units;         /* work units: ceil(num_m_tiles / cluster_m) x num_n_tiles / cluster_n     */
 } yb_conv_schedule_info;
 int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count, yb_conv_schedule_info* info);
 

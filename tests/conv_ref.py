@@ -116,9 +116,8 @@ def old_criterion_ok(got, ref, dtype):
 
 def units_per_warpgroup(info):
     """Fewest work units any consumer warpgroup runs under a yb_conv_schedule result (ping-pong: the two warpgroups of
-    CTA b take units b + w G + 2 G j; cooperative: both take every unit of their CTA)."""
-    units = -(-info.num_m_tiles // info.cluster) * info.num_n_tiles
-    G = info.grid // info.cluster
+    CTA b take units b + w G + 2 G j of the G clusters' units; cooperative: both take every unit of their CTA)."""
+    units, G = info.units, info.grid // info.cluster
     if info.pingpong:
         return max(0, -(-(units - (2 * G - 1)) // (2 * G)))
     return max(0, -(-(units - (G - 1)) // G))
@@ -126,6 +125,5 @@ def units_per_warpgroup(info):
 
 def last_unit_warpgroup(info):
     """Consumer warpgroup that runs the last work unit (ping-pong; 0 under the cooperative schedule)."""
-    units = -(-info.num_m_tiles // info.cluster) * info.num_n_tiles
-    G = info.grid // info.cluster
+    units, G = info.units, info.grid // info.cluster
     return ((units - 1) // G) % 2 if info.pingpong else 0

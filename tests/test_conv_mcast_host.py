@@ -100,6 +100,9 @@ def test_forced_shape(L, shape):
     info = L.ConvSchedule()
     L.check(L.lib.yb_conv_schedule(C.byref(d), 0, 0, 0, SMS, C.byref(info)), "conv_schedule")
     assert info.pingpong == 1 and info.cluster == cm * cn and info.grid % info.cluster == 0
+    assert (info.cluster_m, info.cluster_n) == (cm, cn)
+    assert info.units == -(-info.num_m_tiles // cm) * (info.num_n_tiles // cn)
+    assert info.grid == min(info.units, SMS // info.cluster) * info.cluster
 
 
 def test_single_conv_default_unclustered(L):

@@ -40,7 +40,8 @@ class ConvDesc(C.Structure):
 
 class ConvSchedule(C.Structure):   # yb_conv_schedule_info
     _fields_ = [(n, i32) for n in ("pingpong", "consumers", "cluster", "block_m", "block_n", "block_k", "stages", "num_kb",
-                                   "num_m_tiles", "num_n_tiles", "grid", "res_smem", "res_stages")]
+                                   "num_m_tiles", "num_n_tiles", "grid", "res_smem", "res_stages", "cluster_m",
+                                   "cluster_n", "units")]
 
 
 class LayerSchedule(C.Structure):  # yb_layer_schedule_info

@@ -43,23 +43,45 @@ struct ConvParams {
   int det_e;              // > 0: the fused-decode head kernel for 5 + C = det_e columns per anchor
 };
 
-int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                 const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
-                 ConvParams* p);
-// conv_prepare of a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
-// YB_CONV_MCAST is unset (csrc/conv_igemm.cu)
-int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p);
-// the kernel choice of conv_prepare without pointers (no device work); has_res: the launch adds a residual
-int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, bool has_res, ConvParams* p);
-// Window variant used by the stride-2 dgrad: a kh x kw window whose taps sit at offsets (0..kh-1, 0..kw-1) from the
-// output pixel (zero-filled past the border), stride 1, output scattered to parity class `scatter`.
-// w_packed is [cout_pad][kh*kw*cin].
-int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const void* x, const void* w_packed,
-                     const float* scale, const float* shift, const void* res, void* out, CUtensorMap* tmA,
-                     CUtensorMap* tmB, ConvParams* p);
-int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
-                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p);
+// One implicit-GEMM launch (host only): the operand tensor maps and the parameters they were encoded for.  The TMA
+// boxes depend on the schedule in p, so maps and parameters are built together (conv_prepare) and travel together.
+struct ConvLaunch {
+  CUtensorMap tmA, tmB;
+  ConvParams p;
+};
+
+// What an implicit-GEMM launch computes, without its data pointers: conv_select picks its kernel from this alone.
+struct ConvRequest {
+  yb_conv_desc d;
+  // 0 x 0: the forward ksize x ksize window, symmetric padding ksize / 2.  1..2 x 1..2: a kh x kw window whose taps sit
+  // at offsets (0..kh-1, 0..kw-1) from the output pixel (zero-filled past the border), stride 1, 16-bit output, output
+  // scattered to parity class `scatter` (ConvParams::scatter; the stride-2 dgrad, conv_prepare_dgrad_s2)
+  int kh = 0, kw = 0, scatter = 0;
+  bool stats = false;      // BN batch statistics of the raw result (stat_sum / stat_sqsum)
+  bool res = false;        // adds a residual
+  int det_e = 0;           // > 0: detection head with the decode fused into the epilogue, 5 + C = det_e columns per
+                           // anchor, d.cout = 3 * det_e; one n-tile spans the whole padded cout and `out` is never written
+  bool plan_rule = false;  // a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
+                           // YB_CONV_MCAST is unset
+};
+
+// The kernel of r, down to its conv_igemm_kernel instantiation, which must exist (no pointers, no device work)
+int conv_select(const ConvRequest& r, ConvParams* p);
+// conv_select, then the tensor maps over the data pointers.  res and stat_sum / stat_sqsum are given exactly when r asks
+// for them; scale = shift = NULL: identity.  Windowed requests take w_packed as [cout_pad][kh*kw*cin].
+int conv_prepare(const ConvRequest& r, const void* x, const void* w_packed, const float* scale, const float* shift,
+                 const void* res, void* out, float* stat_sum, float* stat_sqsum, ConvLaunch* l);
+// Stride-2 dgrad parity class c = 2a + b, the input-gradient pixels (2i + a, 2j + b): its (1 + a) x (1 + b) window's
+// [cin_pad][taps * k_cout] weight matrix starts {0, 1, 3, 5}[c] x cin_pad x k_cout elements into the packed weights
+// (yb_pack_dgrad_weights_s2), which hold the 9 taps exactly once
+inline size_t dgrad_s2_class_offset(int c, int cin_pad, int k_cout) {
+  static constexpr int first[4] = {0, 1, 3, 5};
+  return (size_t)first[c] * cin_pad * k_cout;
+}
+// The data gradient of a 3x3 stride-2 conv `fwd` as the four parity-class window convs over the plain dz
+// [n, h / 2, w / 2, dz_ld], each scattered into its quarter of dx [n, h, w, dx_ld] (+ res, nullable).  l: [4].
+int conv_prepare_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
+                          const void* res, int res_ld, void* dx, int dx_ld, ConvLaunch* l);
 // halo-tile conv for the Cin <= 64 3x3 layers (csrc/conv_halo.cu)
 struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; CUtensorMap res; };
 struct HaloParams {
@@ -94,7 +116,7 @@ int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const floa
                            const float* stem_shift, const void* w_packed, const float* scale, const float* shift, void* out,
                            HaloMaps* maps, HaloParams* p);
 int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);
-int conv_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st);
+int conv_launch(const ConvLaunch& l, cudaStream_t st);
 // what conv_launch would launch on the current device, without launching: grid (CTAs) and the most clusters of
 // p.cluster CTAs that can be resident at once (cudaOccupancyMaxActiveClusters; the SM count when p.cluster == 1)
 int conv_launch_grid(const ConvParams& p, int* grid, int* max_clusters);

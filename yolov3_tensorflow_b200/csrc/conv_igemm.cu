@@ -918,8 +918,9 @@ static int conv_kernel_grid(const ConvParams& p, int* grid, int* max_clusters) {
   return YB_OK;
 }
 
-// Launch with prebuilt tensor maps (used by the network plan)
-int conv_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t st) {
+// Launch a prepared conv (conv_prepare): the kernel conv_select recorded in l.p, with the maps built for it
+int conv_launch(const ConvLaunch& l, cudaStream_t st) {
+  const ConvParams& p = l.p;
   return conv_kernel_for(p, [&](auto k) -> int {
     using K = decltype(k);
     int grid = 0, max_clusters = 0;
@@ -936,7 +937,7 @@ int conv_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams
     attr[0].val.clusterDim.x = p.cluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    YB_CUDA(cudaLaunchKernelEx(&cfg, K::kernel, tmA, tmB, p));
+    YB_CUDA(cudaLaunchKernelEx(&cfg, K::kernel, l.tmA, l.tmB, p));
     return YB_OK;
   });
 }
@@ -948,14 +949,23 @@ int conv_launch_grid(const ConvParams& p, int* grid, int* max_clusters) {
 // bytes of one k-block row: 64 / 32 channels of fp16 / bf16, 128 / 64 channels of e4m3
 static int conv_block_kb(int cin, int dtype) { return cin * tm_esize(dtype) % 128 == 0 ? 128 : 64; }
 
-// Shape checks, tiling and kernel variant of one conv: everything conv_prepare_core decides before it looks at the
-// data pointers, down to the conv_igemm_kernel instantiation, which must exist.  yb_conv_schedule reports what this
-// picks.
-// win = 0: the forward rule (ksize x ksize, symmetric padding ksize/2); win = 1: kh x kw window at offsets >= 0.
-// det = E > 0: the fused-decode detection head of E = 5 + C columns per anchor, one n-tile spanning the whole padded cout.
-// has_res: the launch adds a residual.
-static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatter, bool stats, bool has_res, int det,
-                       bool plan_rule, ConvParams* p) {
+// Shape checks, tiling and kernel variant of one conv: everything conv_prepare decides before it looks at the data
+// pointers, down to the conv_igemm_kernel instantiation, which must exist.  The launches, yb_conv_schedule and
+// yb_net_layer_schedule all select through here.
+int conv_select(const ConvRequest& r, ConvParams* p) {
+  memset(p, 0, sizeof(*p));
+  const yb_conv_desc* d = &r.d;
+  const bool win = r.kh != 0 || r.kw != 0;
+  const int det = r.det_e;
+  if (det && d->cout != 3 * det) {
+    set_error("fused decode: %d output channels are not 3 x (5 + %d classes)", d->cout, det - 5);
+    return YB_ERR_UNSUPPORTED;
+  }
+  if (win) {
+    YB_REQUIRE(r.kh >= 1 && r.kh <= 2 && r.kw >= 1 && r.kw <= 2 && r.scatter >= 0 && r.scatter <= 4, "conv: bad window");
+    YB_REQUIRE(d->stride == 1 && !d->out_fp32 && !d->upsample2x && !r.stats,
+               "conv: windows are stride-1, 16-bit, non-upsampled and without statistics");
+  }
   YB_REQUIRE(win || d->ksize == 1 || d->ksize == 3, "conv: ksize must be 1 or 3 (got %d)", d->ksize);
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride must be 1 or 2 (got %d)", d->stride);
   YB_REQUIRE(!(d->ksize == 1 && d->stride != 1), "conv: 1x1 stride-2 is not on the YOLOv3 path");
@@ -967,7 +977,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
     YB_REQUIRE(d->cin % 64 == 0, "conv: e4m3 needs cin %% 64 == 0 (got %d)", d->cin);
     YB_REQUIRE(d->in_ld % 16 == 0 && (d->out_fp32 || d->out_ld % 16 == 0) && d->res_ld % 16 == 0,
                "conv: e4m3 needs in_ld, out_ld and res_ld to be multiples of 16");
-    YB_REQUIRE(!win && !stats, "conv: e4m3 is a forward inference path (no windows, no statistics)");
+    YB_REQUIRE(!win && !r.stats, "conv: e4m3 is a forward inference path (no windows, no statistics)");
     YB_REQUIRE(opt("YB_CONV_EG")[0] != '1' && opt("YB_CONV_MODE")[0] != '2' && opt("YB_CONV_EPI")[0] != 'r',
                "conv: e4m3 runs with two consumer warpgroups, no cluster and the staged epilogue "
                "(YB_CONV_EG, YB_CONV_MODE, YB_CONV_EPI are 16-bit only)");
@@ -982,7 +992,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
     YB_REQUIRE(d->out_ld >= d->cout, "conv: out_ld %d invalid", d->out_ld);
   }
   const int P = d->h / d->stride, Q = d->w / d->stride;
-  if (!win) { kh = d->ksize; kw = d->ksize; }
+  const int kh = win ? r.kh : d->ksize, kw = win ? r.kw : d->ksize;
   const int pad = win ? 0 : d->ksize / 2;
   const int bn = det ? cout_pad : (cout_pad % 128 == 0 ? 128 : 64);
   p->M = d->n * P * Q; p->P = P; p->Q = Q;
@@ -1002,7 +1012,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   //                       the ping-pong kernel prefetches it into shared memory where it can (below)
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
-  p->epi_reg = (!det && !stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  p->epi_reg = (!det && !r.stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
   p->ctas = opt_int("YB_CONV_CTAS", 0);
   // ping-pong wherever the default variant runs, except
   //  - the fused-decode heads: their 256-column tile does not fit 128 rows per warpgroup in registers;
@@ -1028,7 +1038,7 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
       YB_REQUIRE((mc[0] == '1' || mc[0] == '2') && mc[1] == 'x' && (mc[2] == '1' || mc[2] == '2') && mc[3] == '\0',
                  "conv: YB_CONV_MCAST must be 0, 2x1, 1x2 or 2x2 (got '%s')", mc);
       cm = mc[0] - '0'; cn = mc[2] - '0';
-    } else if (mc[0] == '\0' && plan_rule && kh * kw > 1) {
+    } else if (mc[0] == '\0' && r.plan_rule && kh * kw > 1) {
       cm = 2; cn = 2;
     }
     if (p->num_n_tiles % 2 != 0) cn = 1;
@@ -1046,34 +1056,34 @@ static int conv_select(const yb_conv_desc* d, int win, int kh, int kw, int scatt
   p->block_n = bn;
   p->block_kb = conv_block_kb(d->cin, d->dtype);
   p->det_e = det;
-  p->res_smem = (has_res && p->pingpong && !e4m3 && !det && bn == 128 && p->block_kb == 128 && !scatter &&
+  p->res_smem = (r.res && p->pingpong && !e4m3 && !det && bn == 128 && p->block_kb == 128 && !r.scatter &&
                  !d->upsample2x && !d->out_fp32 && strcmp(ro, "ldg") != 0) ? 1 : 0;
-  memset(&p->det, 0, sizeof(p->det));
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
-  p->kh = kh; p->kw = kw; p->scatter = scatter;
+  p->kh = kh; p->kw = kw; p->scatter = r.scatter;
   p->im2col = kh * kw > 1;
   p->out_fp32 = d->out_fp32; p->leaky = d->leaky; p->upsample = d->upsample2x;
   p->res_scale = 1.f; p->out_inv_scale = 1.f;
   return conv_kernel_for(*p, [](auto) -> int { return YB_OK; });
 }
 
-// Build maps + params for one conv.  x/w/out pointers are baked into maps/params.
-static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int scatter, const void* x,
-                             const void* w_packed, const float* scale, const float* shift, const void* res, void* out,
-                             float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p,
-                             int det = 0, bool plan_rule = false) {
-  int rc = conv_select(d, win, kh, kw, scatter, stat_sum != nullptr, res != nullptr, det, plan_rule, p);
+// conv_select, then the tensor maps over the data pointers, which are baked into maps and parameters.
+int conv_prepare(const ConvRequest& r, const void* x, const void* w_packed, const float* scale, const float* shift,
+                 const void* res, void* out, float* stat_sum, float* stat_sqsum, ConvLaunch* l) {
+  ConvParams* p = &l->p;
+  int rc = conv_select(r, p);
   if (rc) return rc;
+  const yb_conv_desc* d = &r.d;
   YB_REQUIRE(x && w_packed && out && (scale == nullptr) == (shift == nullptr), "conv: null pointer");   // scale = shift = NULL: identity
   YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 &&
                  ((uintptr_t)res & 15) == 0,
              "conv: pointers must be 16-byte aligned");
+  YB_REQUIRE((res != nullptr) == r.res, "conv: a residual pointer is given exactly when the request has a residual");
   if (res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0 && !d->out_fp32, "conv: res_ld %d invalid", d->res_ld);
   YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), "conv: stat_sum/stat_sqsum must both be given");
+  YB_REQUIRE((stat_sum != nullptr) == r.stats, "conv: statistics pointers are given exactly when the request has them");
   const int cout_pad = yb_conv_cout_pad(d->cout);
   const int bk = p->block_kb / tm_esize(d->dtype);   // channels per k-block
-  const int pad = p->pad;
-  kh = p->kh; kw = p->kw;
+  const int kh = p->kh, kw = p->kw;
   // TMA boxes: this CTA's share of the A tile (1 / cluster_n of its rows) and of the B tile (1 / (cluster / cluster_n))
   const int a_rows = 64 * p->consumers / p->cluster_n;
   const int b_rows = p->block_n / (p->cluster / p->cluster_n);
@@ -1086,50 +1096,35 @@ static int conv_prepare_core(const yb_conv_desc* d, int win, int kh, int kw, int
     if (rc) return rc;
   }
   if (p->im2col) {
-    rc = make_tmap_im2col_px(tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride, pad, bk,
-                             a_rows);
+    const bool win = r.kh != 0 || r.kw != 0;
+    rc = make_tmap_im2col_px(&l->tmA, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, win ? 1 : d->ksize, d->stride,
+                             p->pad, bk, a_rows);
   } else {
-    rc = make_tmap_2d(tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, a_rows, bk, 0);
+    rc = make_tmap_2d(&l->tmA, x, d->dtype, (long)d->n * d->h * d->w, d->cin, d->in_ld, a_rows, bk, 0);
   }
   if (rc) return rc;
-  return make_tmap_2d(tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, b_rows, bk, 1);
+  return make_tmap_2d(&l->tmB, w_packed, d->dtype, cout_pad, (long)kh * kw * d->cin, (long)kh * kw * d->cin, b_rows, bk,
+                      1);
 }
 
-int conv_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                 const void* res, void* out, float* stat_sum, float* stat_sqsum, CUtensorMap* tmA, CUtensorMap* tmB,
-                 ConvParams* p) {
-  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, tmA, tmB, p);
-}
-
-int conv_prepare_plan(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p) {
-  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p, 0, true);
-}
-
-int conv_schedule_params(const yb_conv_desc* d, bool plan_rule, bool has_res, ConvParams* p) {
-  memset(p, 0, sizeof(*p));
-  return conv_select(d, 0, 0, 0, 0, false, has_res, 0, plan_rule, p);
-}
-
-// Detection head with the decode fused into the epilogue (yb_net_detect): ONE n-tile that holds all 3 * (5 + C)
-// columns; `out` is never written.  YB_ERR_UNSUPPORTED when the class count has no kernel.
-int conv_prepare_det(const yb_conv_desc* d, int class_num, const void* x, const void* w_packed, const float* scale,
-                     const float* shift, CUtensorMap* tmA, CUtensorMap* tmB, ConvParams* p) {
-  const int E = 5 + class_num;
-  if (d->cout != 3 * E) {
-    set_error("fused decode: %d output channels are not 3 x (5 + %d classes)", d->cout, class_num);
-    return YB_ERR_UNSUPPORTED;
+int conv_prepare_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
+                          const void* res, int res_ld, void* dx, int dx_ld, ConvLaunch* l) {
+  YB_REQUIRE(fwd && dz && w_dgrad_s2 && dx, "dgrad_s2: null pointer");
+  YB_REQUIRE(fwd->ksize == 3 && fwd->stride == 2 && fwd->h % 2 == 0 && fwd->w % 2 == 0, "dgrad_s2: 3x3 stride-2 convs only");
+  YB_REQUIRE(k_cout >= fwd->cout && k_cout % 32 == 0 && dz_ld >= k_cout, "dgrad_s2: dz must hold k_cout (multiple of 32) channels");
+  ConvRequest r{*fwd};
+  yb_conv_desc& d = r.d;
+  d.h = fwd->h / 2; d.w = fwd->w / 2; d.cin = k_cout; d.cout = fwd->cin; d.ksize = 1; d.stride = 1;
+  d.in_ld = dz_ld; d.out_ld = dx_ld; d.res_ld = res_ld; d.out_fp32 = 0; d.leaky = 0; d.upsample2x = 0;
+  r.res = res != nullptr;
+  const int cin_pad = yb_conv_cout_pad(fwd->cin);
+  for (int c = 0; c < 4; ++c) {
+    r.kh = 1 + (c >> 1); r.kw = 1 + (c & 1); r.scatter = 1 + c;
+    const uint8_t* w = static_cast<const uint8_t*>(w_dgrad_s2) + dgrad_s2_class_offset(c, cin_pad, k_cout) * 2;
+    int rc = conv_prepare(r, dz, w, nullptr, nullptr, res, dx, nullptr, nullptr, &l[c]);
+    if (rc) return rc;
   }
-  return conv_prepare_core(d, 0, 0, 0, 0, x, w_packed, scale, shift, nullptr, const_cast<void*>(x) /*unused*/, nullptr,
-                           nullptr, tmA, tmB, p, E);
-}
-
-int conv_prepare_win(const yb_conv_desc* d, int kh, int kw, int scatter, const void* x, const void* w_packed,
-                     const float* scale, const float* shift, const void* res, void* out, CUtensorMap* tmA,
-                     CUtensorMap* tmB, ConvParams* p) {
-  YB_REQUIRE(kh >= 1 && kh <= 2 && kw >= 1 && kw <= 2 && scatter >= 0 && scatter <= 4, "conv_prepare_win: bad window");
-  YB_REQUIRE(d->stride == 1 && !d->out_fp32 && !d->upsample2x, "conv_prepare_win: stride-1, 16-bit, non-upsampled only");
-  return conv_prepare_core(d, 1, kh, kw, scatter, x, w_packed, scale, shift, res, out, nullptr, nullptr, tmA, tmB, p);
+  return YB_OK;
 }
 
 }  // namespace yb
@@ -1141,17 +1136,13 @@ extern "C" int yb_conv_cout_pad(int cout) { return (cout + 63) / 64 * 64; }
 extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count,
                                 yb_conv_schedule_info* info) {
   YB_REQUIRE(d && info && sm_count > 0, "conv_schedule: bad argument");
-  const int win = kh != 0 || kw != 0;
-  if (win) {
-    YB_REQUIRE(kh >= 1 && kh <= 2 && kw >= 1 && kw <= 2, "conv_schedule: bad window");
-    YB_REQUIRE(d->stride == 1 && !with_stats, "conv_schedule: windows are stride-1 without statistics");
-  }
-  yb::ConvParams p;   // the launch without a residual, then pr: with one
-  memset(&p, 0, sizeof(p));
-  int rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, false, 0, false, &p);
+  yb::ConvRequest r{*d};
+  r.kh = kh; r.kw = kw; r.stats = with_stats != 0;
+  yb::ConvParams p, pr;   // the launch without a residual, then pr: with one
+  int rc = yb::conv_select(r, &p);
   if (rc) return rc;
-  yb::ConvParams pr = p;
-  rc = yb::conv_select(d, win, kh, kw, 0, with_stats != 0, true, 0, false, &pr);
+  r.res = true;
+  rc = yb::conv_select(r, &pr);
   if (rc) return rc;
   auto stages = [](const yb::ConvParams& q, int* s) {
     return yb::conv_kernel_for(q, [&](auto k) -> int { *s = decltype(k)::C::STAGES; return YB_OK; });
@@ -1171,6 +1162,9 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
   info->num_m_tiles = p.num_m_tiles;
   info->num_n_tiles = p.num_n_tiles;
   info->grid = yb::conv_grid(p, sm_count, 0);
+  info->cluster_m = p.cluster / p.cluster_n;
+  info->cluster_n = p.cluster_n;
+  info->units = yb::conv_units(p);
   return YB_OK;
 }
 
@@ -1178,11 +1172,13 @@ extern "C" int yb_conv2d_fwd(const yb_conv_desc* d, const void* x, const void* w
                              const float* shift, const void* res, void* out, float* stat_sum, float* stat_sqsum,
                              void* stream) {
   if (!d) { yb::set_error("conv: null descriptor"); return YB_ERR_INVALID_ARGUMENT; }
-  CUtensorMap tmA, tmB;
-  yb::ConvParams p;
-  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, &tmA, &tmB, &p);
+  yb::ConvRequest r{*d};
+  r.stats = stat_sum != nullptr;
+  r.res = res != nullptr;
+  yb::ConvLaunch l;
+  int rc = yb::conv_prepare(r, x, w_packed, scale, shift, res, out, stat_sum, stat_sqsum, &l);
   if (rc) return rc;
-  return yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
+  return yb::conv_launch(l, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
@@ -1191,34 +1187,20 @@ extern "C" int yb_conv2d_fwd_e4m3(const yb_conv_desc* d, const void* x, const vo
   YB_REQUIRE(d && d->dtype == YB_E4M3, "conv_e4m3: descriptor dtype must be YB_E4M3");
   YB_REQUIRE(res_scale > 0.f && out_scale > 0.f && isfinite(res_scale) && isfinite(out_scale),
              "conv_e4m3: scales must be positive and finite");
-  CUtensorMap tmA, tmB;
-  yb::ConvParams p;
-  int rc = yb::conv_prepare(d, x, w_packed, scale, shift, res, out, nullptr, nullptr, &tmA, &tmB, &p);
+  yb::ConvRequest r{*d};
+  r.res = res != nullptr;
+  yb::ConvLaunch l;
+  int rc = yb::conv_prepare(r, x, w_packed, scale, shift, res, out, nullptr, nullptr, &l);
   if (rc) return rc;
-  p.res_scale = res_scale;
-  p.out_inv_scale = 1.f / out_scale;
-  return yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
+  l.p.res_scale = res_scale;
+  l.p.out_inv_scale = 1.f / out_scale;
+  return yb::conv_launch(l, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int yb_conv2d_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
                                   const void* res, int res_ld, void* dx, int dx_ld, void* stream) {
-  YB_REQUIRE(fwd && dz && w_dgrad_s2 && dx, "dgrad_s2: null pointer");
-  YB_REQUIRE(fwd->ksize == 3 && fwd->stride == 2 && fwd->h % 2 == 0 && fwd->w % 2 == 0, "dgrad_s2: 3x3 stride-2 convs only");
-  YB_REQUIRE(k_cout >= fwd->cout && k_cout % 32 == 0 && dz_ld >= k_cout, "dgrad_s2: dz must hold k_cout (multiple of 32) channels");
-  yb_conv_desc d = *fwd;
-  d.h = fwd->h / 2; d.w = fwd->w / 2; d.cin = k_cout; d.cout = fwd->cin; d.ksize = 1; d.stride = 1;
-  d.in_ld = dz_ld; d.out_ld = dx_ld; d.res_ld = res_ld; d.out_fp32 = 0; d.leaky = 0; d.upsample2x = 0;
-  const size_t per = (size_t)yb_conv_cout_pad(fwd->cin) * k_cout;
-  const size_t woff[4] = {0, per, 3 * per, 5 * per};
-  for (int c = 0; c < 4; ++c) {
-    CUtensorMap tmA, tmB;
-    yb::ConvParams p;
-    int rc = yb::conv_prepare_win(&d, 1 + (c >> 1), 1 + (c & 1), 1 + c, dz,
-                                  static_cast<const uint8_t*>(w_dgrad_s2) + woff[c] * 2, nullptr, nullptr, res, dx, &tmA,
-                                  &tmB, &p);
-    if (rc) return rc;
-    rc = yb::conv_launch(tmA, tmB, p, static_cast<cudaStream_t>(stream));
-    if (rc) return rc;
-  }
-  return YB_OK;
+  yb::ConvLaunch l[4];
+  int rc = yb::conv_prepare_dgrad_s2(fwd, dz, dz_ld, k_cout, w_dgrad_s2, res, res_ld, dx, dx_ld, l);
+  for (int c = 0; c < 4 && rc == YB_OK; ++c) rc = yb::conv_launch(l[c], static_cast<cudaStream_t>(stream));
+  return rc;
 }

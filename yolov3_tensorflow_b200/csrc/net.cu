@@ -162,7 +162,7 @@ struct Builder {
   }
 };
 
-static void* ten_ptr(const yb_net* net, const Ten& t) {
+void* ten_ptr(const yb_net* net, const Ten& t) {
   const Buf& b = net->bufs[t.buf];
   return net->act + b.offset + (size_t)t.off * b.esz;
 }
@@ -172,8 +172,8 @@ static void apply_fp8_scales(yb_net* net) {
   for (size_t i = FP8_FIRST_LAYER - 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
     const float so = net->buf_scale[L.out.buf];
-    L.params.res_scale = L.res.buf >= 0 ? net->buf_scale[L.res.buf] : 1.f;
-    L.params.out_inv_scale = 1.f / so;
+    L.fwd.p.res_scale = L.res.buf >= 0 ? net->buf_scale[L.res.buf] : 1.f;
+    L.fwd.p.out_inv_scale = 1.f / so;
     L.halo_params.out_inv_scale = 1.f / so;
   }
 }
@@ -186,8 +186,7 @@ static int fold_e4m3_layer(yb_net* net, Layer& L, cudaStream_t st) {
                   L.info.cout, net->bn_eps, net->buf_scale[L.in.buf], f(L.w_scale), f(L.scale), f(L.shift), st);
 }
 
-// conv descriptor of a tensor-core layer of the plan
-static yb_conv_desc layer_desc(const yb_net* net, const Layer& L) {
+yb_conv_desc layer_desc(const yb_net* net, const Layer& L) {
   yb_conv_desc d;
   memset(&d, 0, sizeof(d));
   d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
@@ -269,8 +268,11 @@ extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count,
   info->residual = L.res.buf >= 0 ? 1 : 0;
   if (k == LayerKernel::Halo) info->res_smem = info->residual && conv_halo_res_smem(&d);
   if (k != LayerKernel::Igemm) return YB_OK;           // the thin, halo and fused-stem kernels
+  ConvRequest r{d};
+  r.res = info->residual;
+  r.plan_rule = plan_mcast_rule(net);
   ConvParams p;
-  int rc = conv_schedule_params(&d, plan_mcast_rule(net), info->residual, &p);
+  int rc = conv_select(r, &p);
   if (rc) return rc;
   info->igemm = 1;
   info->res_smem = p.res_smem;
@@ -323,11 +325,11 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
     const void* res = L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr;
     const float* scale = reinterpret_cast<const float*>(net->par + L.scale);
     const float* shift = reinterpret_cast<const float*>(net->par + L.shift);
-    int rc = plan_mcast_rule(net)
-                 ? conv_prepare_plan(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
-                                     &L.tmA, &L.tmB, &L.params)
-                 : conv_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
-                                nullptr, nullptr, &L.tmA, &L.tmB, &L.params);
+    ConvRequest r{d};
+    r.res = res != nullptr;
+    r.plan_rule = plan_mcast_rule(net);
+    int rc = conv_prepare(r, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out), nullptr,
+                          nullptr, &L.fwd);
     if (rc) return rc;
     if (conv_halo_supported(&d)) {   // every layer layer_kernel may give the halo kernel
       L.halo_desc = d;
@@ -338,10 +340,11 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
     }
     if (!L.info.has_bn) {
       // fused-decode variant of the head (yb_net_detect); class counts without a kernel keep the unfused pipeline
-      L.det_ok = conv_prepare_det(&d, net->class_num, ten_ptr(net, L.in), net->par + L.w_packed,
-                                  reinterpret_cast<const float*>(net->par + L.scale),
-                                  reinterpret_cast<const float*>(net->par + L.shift), &L.det_tmA, &L.det_tmB,
-                                  &L.det_params) == YB_OK;
+      ConvRequest rd{d};
+      rd.det_e = 5 + net->class_num;
+      void* x = ten_ptr(net, L.in);
+      L.det_ok = conv_prepare(rd, x, net->par + L.w_packed, scale, shift, nullptr, x /* never written */, nullptr, nullptr,
+                              &L.det) == YB_OK;
     }
   }
   if (net->fp8_ready) apply_fp8_scales(net);
@@ -479,12 +482,11 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
       if (rc) return rc;
       continue;
     }
-    ConvParams* p = &L.params;
     if (!L.info.has_bn) {
       int which = L.out.buf == net->fm_buf[0] ? 0 : (L.out.buf == net->fm_buf[1] ? 1 : 2);
       if (det) {                                      // decode + candidate filter in the epilogue, no feature map
-        ConvParams dp = L.det_params;
-        dp.det = det[which];
+        ConvLaunch dl = L.det;
+        dl.p.det = det[which];
         // The first two heads are leaves of the graph (nothing but the NMS reads what they produce) and small (43 / 170
         // tiles): they run on the plan's side stream beside the upsampling branch that continues on the caller's stream;
         // the last head is on the critical path.  Every layer output has its own buffer, so the head's input stays intact.
@@ -495,13 +497,13 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
           hs = net->side_stream;
           forked = true;
         }
-        int rc = conv_launch(L.det_tmA, L.det_tmB, dp, hs);
+        int rc = conv_launch(dl, hs);
         if (rc) return rc;
         continue;
       }
-      p->out = user_fm[which] ? (void*)user_fm[which] : ten_ptr(net, L.out);
+      L.fwd.p.out = user_fm[which] ? (void*)user_fm[which] : ten_ptr(net, L.out);
     }
-    int rc = conv_launch(L.tmA, L.tmB, *p, st);
+    int rc = conv_launch(L.fwd, st);
     if (rc) return rc;
   }
   if (forked) {

@@ -29,31 +29,33 @@ struct Layer {
   int dtype = 0;      // yb_dtype of the conv's input and packed weights (e4m3 plan: fp16 for layers 0-3)
   // parameter arena offsets (bytes); w_scale: e4m3 layers' per-output-channel weight scales, fp32 [cout_pad]
   size_t w_master = 0, w_packed = 0, gamma = 0, beta = 0, mean = 0, var = 0, bias = 0, scale = 0, shift = 0, w_scale = 0;
-  // prepared launch state
-  CUtensorMap tmA, tmB;
-  ConvParams params;
+  // prepared implicit-GEMM launch of the inference forward
+  ConvLaunch fwd;
   // Cin <= 64 3x3 layers: halo-tile kernel (csrc/conv_halo.cu), inference forward only
   HaloMaps halo_maps;
   HaloParams halo_params;
   yb_conv_desc halo_desc;
   // detection heads: the same conv with the decode + NMS candidate filter fused into its epilogue (yb_net_detect)
-  CUtensorMap det_tmA, det_tmB;
-  ConvParams det_params;
+  ConvLaunch det;
   bool det_ok = false;
   // ---- training plan (net_train.cu) ----
   size_t z_off = 0, dz_off = 0;      // raw conv output z / its gradient (activation arena); dz is zero-inserted for stride 2
   int dz_ld = 0, dz_dilated = 0, k_cout = 0;
   int dgrad_parity = 0;              // stride-2 layer whose dgrad runs as 4 parity-class convs on the plain dz
-  CUtensorMap d4_tmA[4], d4_tmB[4];
-  ConvParams d4_params[4];
   size_t st_sum = 0, st_sqsum = 0, st_mean = 0, st_invstd = 0, st_scale = 0, st_shift = 0;   // fp32 [cout_pad] each
   size_t x_bwd = 0;                  // fp32 [2][cout_pad]: sync-BN backward exchange slab (sum dact*zhat | sum dact)
   size_t w_dgrad = 0;                // [cin_pad, k, k, k_cout] 16-bit (param arena)
   long g_w = -1, g_gamma = -1, g_beta = -1, g_bias = -1;   // float offsets into the flat gradient / velocity buffers
-  ConvParams tparams;                // training-mode forward conv (raw z + statistics)
-  CUtensorMap d_tmA, d_tmB;          // dgrad (forward kernel on dz with flipped/transposed weights)
-  ConvParams dparams;
+  ConvLaunch train;                  // training-mode forward conv: raw z + statistics (detection heads: fwd)
+  // dgrad: the forward kernel on dz with flipped/transposed weights; stride-2 parity layers: one launch per class
+  ConvLaunch dgrad[4];
+  int num_dgrad = 0;                 // 1 | 4
 };
+
+// the activation view t (16-bit training buffers and inference buffers of any element size)
+void* ten_ptr(const yb_net* net, const Ten& t);
+// conv descriptor of a tensor-core layer's inference forward (the training plan derives its own from it)
+yb_conv_desc layer_desc(const yb_net* net, const Layer& L);
 
 }  // namespace yb
 

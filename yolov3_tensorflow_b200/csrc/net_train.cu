@@ -142,10 +142,6 @@ void train_layout(yb_net* net) {
   net->param_bytes = o;
 }
 
-static void* ten_ptr2(const yb_net* net, const Ten& t) {
-  const Buf& b = net->bufs[t.buf];
-  return net->act + b.offset + (size_t)t.off * 2;
-}
 static void* gten_ptr(const yb_net* net, const Ten& t) {
   return net->act + net->gbuf_offset[t.buf] + (size_t)t.off * 2;
 }
@@ -176,15 +172,12 @@ int train_bind(yb_net* net, cudaStream_t st) {
   // ---- training-mode forward convs: raw z + statistics ----
   for (size_t i = 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
-    if (!L.info.has_bn) { L.tparams = L.params; continue; }   // detection convs run as in inference
-    yb_conv_desc d; memset(&d, 0, sizeof(d));
-    d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
-    d.ksize = L.info.ksize; d.stride = L.info.stride;
-    d.in_ld = net->bufs[L.in.buf].ld; d.out_ld = L.info.cout; d.res_ld = 0;
-    d.dtype = net->dtype; d.out_fp32 = 0; d.leaky = 0; d.upsample2x = 0;
-    CUtensorMap a, b;
-    int rc = conv_prepare(&d, ten_ptr2(net, L.in), net->par + L.w_packed, ones, zeros, nullptr, net->act + L.z_off,
-                          fact(net, L.st_sum), fact(net, L.st_sqsum), &a, &b, &L.tparams);
+    if (!L.info.has_bn) { L.train = L.fwd; continue; }   // detection convs run as in inference
+    ConvRequest r{layer_desc(net, L)};   // raw z [rows, cout]: no activation, residual or upsampling
+    r.d.out_ld = L.info.cout; r.d.res_ld = 0; r.d.leaky = 0; r.d.upsample2x = 0;
+    r.stats = true;
+    int rc = conv_prepare(r, ten_ptr(net, L.in), net->par + L.w_packed, ones, zeros, nullptr, net->act + L.z_off,
+                          fact(net, L.st_sum), fact(net, L.st_sqsum), &L.train);
     if (rc) return rc;
   }
   // ---- dgrad convs + residual bookkeeping (reverse order) ----
@@ -202,28 +195,27 @@ int train_bind(yb_net* net, cudaStream_t st) {
     // this layer's residual input receives dA(out) unchanged
     if (L.res.buf >= 0) pending[{L.res.buf, L.res.off}] = Pending{gten_ptr(net, L.out), (long)net->bufs[L.out.buf].ld};
     // dgrad: dA(in) (+)= conv_s1(dz [zero-inserted if stride 2], Wd)
-    yb_conv_desc d; memset(&d, 0, sizeof(d));
-    d.n = net->n; d.h = L.info.in_h; d.w = L.info.in_w;      // dz (dilated for stride 2) lives at the INPUT resolution
-    d.cin = L.k_cout; d.cout = L.info.cin; d.ksize = L.info.ksize; d.stride = 1;
-    d.in_ld = L.dz_ld; d.out_ld = net->bufs[L.in.buf].ld;
-    d.dtype = net->dtype; d.out_fp32 = 0; d.leaky = 0; d.upsample2x = 0;
     const void* res = nullptr;
+    int res_ld = 0;
     auto pit = pending.find({L.in.buf, L.in.off});
     const bool cov = covered(L.in);
     if (cov && pit != pending.end()) { set_error("train plan: tensor with both a written gradient and a pending residual"); return YB_ERR_UNSUPPORTED; }
-    if (cov) { res = gten_ptr(net, L.in); d.res_ld = d.out_ld; }
-    else if (pit != pending.end()) { res = pit->second.ptr; d.res_ld = (int)pit->second.ld; pending.erase(pit); }
-    int rc = YB_OK;
-    if (L.dgrad_parity) {
-      d.h = L.info.out_h; d.w = L.info.out_w;                // plain dz at the OUTPUT resolution
-      const size_t esz = 2, per = (size_t)yb_conv_cout_pad(L.info.cin) * L.k_cout;
-      const size_t woff[4] = {0, per, 3 * per, 5 * per};
-      for (int c = 0; c < 4 && rc == YB_OK; ++c)
-        rc = conv_prepare_win(&d, 1 + (c >> 1), 1 + (c & 1), 1 + c, net->act + L.dz_off, net->par + L.w_dgrad + woff[c] * esz,
-                              ones, zeros, res, gten_ptr(net, L.in), &L.d4_tmA[c], &L.d4_tmB[c], &L.d4_params[c]);
-    } else {
-      rc = conv_prepare(&d, net->act + L.dz_off, net->par + L.w_dgrad, ones, zeros, res, gten_ptr(net, L.in), nullptr,
-                        nullptr, &L.d_tmA, &L.d_tmB, &L.dparams);
+    if (cov) { res = gten_ptr(net, L.in); res_ld = net->bufs[L.in.buf].ld; }
+    else if (pit != pending.end()) { res = pit->second.ptr; res_ld = (int)pit->second.ld; pending.erase(pit); }
+    const yb_conv_desc fwd = layer_desc(net, L);
+    void* dx = gten_ptr(net, L.in);
+    int rc;
+    if (L.dgrad_parity) {   // plain dz at the OUTPUT resolution
+      L.num_dgrad = 4;
+      rc = conv_prepare_dgrad_s2(&fwd, net->act + L.dz_off, L.dz_ld, L.k_cout, net->par + L.w_dgrad, res, res_ld, dx,
+                                 fwd.in_ld, L.dgrad);
+    } else {                // dz (dilated for stride 2) at the INPUT resolution
+      L.num_dgrad = 1;
+      ConvRequest r{fwd};
+      r.d.cin = L.k_cout; r.d.cout = L.info.cin; r.d.stride = 1;
+      r.d.in_ld = L.dz_ld; r.d.out_ld = fwd.in_ld; r.d.res_ld = res_ld; r.d.out_fp32 = 0; r.d.leaky = 0; r.d.upsample2x = 0;
+      r.res = res != nullptr;
+      rc = conv_prepare(r, net->act + L.dz_off, net->par + L.w_dgrad, ones, zeros, res, dx, nullptr, nullptr, &L.dgrad[0]);
     }
     if (rc) return rc;
     written[L.in.buf].push_back({L.in.off, L.in.c});
@@ -336,25 +328,25 @@ static int train_fwd_layer(yb_net* net, int i, int phase, const float* images, i
       if (rc) return rc;
       return yb_col_stats(net->act + L.z_off, L.info.cout, rows, L.info.cout, dt, fact(net, L.st_sum), fact(net, L.st_sqsum), stream);
     }
-    ConvParams p = L.tparams;
+    ConvLaunch l = L.train;
     if (!L.info.has_bn) {
       const int which = L.out.buf == net->fm_buf[0] ? 0 : (L.out.buf == net->fm_buf[1] ? 1 : 2);
-      p.out = user_fm[which] ? (void*)user_fm[which] : (void*)(net->act + net->bufs[L.out.buf].offset);
-      net->train_fm[which] = static_cast<float*>(p.out);
+      l.p.out = user_fm[which] ? (void*)user_fm[which] : (void*)(net->act + net->bufs[L.out.buf].offset);
+      net->train_fm[which] = static_cast<float*>(l.p.out);
     }
-    return conv_launch(L.tmA, L.tmB, p, st);
+    return conv_launch(l, st);
   }
   if (!L.info.has_bn) return YB_OK;
   if (!bn_frozen) net->fold_dirty = true;
   const long count = (long)replicas * rows;
-  const void* resp = L.res.buf >= 0 ? ten_ptr2(net, L.res) : nullptr;
+  const void* resp = L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr;
   const long res_ld = L.res.buf >= 0 ? net->bufs[L.res.buf].ld : 0;
   if (opt("YB_BN_FIN")[0] != '0') {   // statistics -> scale/shift inside the apply kernel (one launch per BN layer instead of two)
     return bn_stats_act_apply_n(net->act + L.z_off, L.info.cout, bn_frozen ? nullptr : fact(net, L.st_sum),
                                 bn_frozen ? nullptr : fact(net, L.st_sqsum), count, fpar(net, L.gamma), fpar(net, L.beta),
                                 net->bn_eps, bn_decay, fpar(net, L.mean), fpar(net, L.var), fact(net, L.st_scale),
                                 fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), resp, res_ld,
-                                ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w,
+                                ten_ptr(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w,
                                 L.info.cout, dt, 1, L.upsample ? 1 : 0, stream);
   }
   rc = yb_bn_finalize(bn_frozen ? nullptr : fact(net, L.st_sum), bn_frozen ? nullptr : fact(net, L.st_sqsum), count,
@@ -363,7 +355,7 @@ static int train_fwd_layer(yb_net* net, int i, int phase, const float* images, i
                       fact(net, L.st_shift), fact(net, L.st_mean), fact(net, L.st_invstd), stream);
   if (rc) return rc;
   return yb_bn_act_apply(net->act + L.z_off, L.info.cout, fact(net, L.st_scale), fact(net, L.st_shift), resp, res_ld,
-                         ten_ptr2(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1,
+                         ten_ptr(net, L.out), net->bufs[L.out.buf].ld, n, L.info.out_h, L.info.out_w, L.info.cout, dt, 1,
                          L.upsample ? 1 : 0, stream);
 }
 
@@ -449,19 +441,14 @@ static int train_bwd_layer(yb_net* net, int i, int phase, const float* images, i
     wstream = net->side_stream;
     net->side_forked = true;
   }
-  yb_conv_desc d; memset(&d, 0, sizeof(d));
-  d.n = n; d.h = L.info.in_h; d.w = L.info.in_w; d.cin = L.info.cin; d.cout = L.info.cout;
-  d.ksize = L.info.ksize; d.stride = L.info.stride; d.in_ld = net->bufs[L.in.buf].ld; d.dtype = dt;
-  rc = yb_conv2d_wgrad(&d, ten_ptr2(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), wstream);
+  const yb_conv_desc d = layer_desc(net, L);
+  rc = yb_conv2d_wgrad(&d, ten_ptr(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), wstream);
   if (rc) return rc;
-  if (L.dgrad_parity) {
-    for (int c = 0; c < 4; ++c) {
-      rc = conv_launch(L.d4_tmA[c], L.d4_tmB[c], L.d4_params[c], st);
-      if (rc) return rc;
-    }
-    return YB_OK;
+  for (int c = 0; c < L.num_dgrad; ++c) {
+    rc = conv_launch(L.dgrad[c], st);
+    if (rc) return rc;
   }
-  return conv_launch(L.d_tmA, L.d_tmB, L.dparams, st);
+  return YB_OK;
 }
 
 // Position of (layer, phase) in the layered step: forward 0..L-1 (LOCAL, GLOBAL each), the loss, backward L-1..0.
@@ -709,7 +696,7 @@ extern "C" int yb_net_train_buffer(yb_net* net, int layer, int which, void** ptr
     case 1: *ptr = net->act + L.dz_off; *ld = L.dz_ld; if (L.dz_dilated) { h = L.info.in_h; w = L.info.in_w; } break;
     case 2: YB_REQUIRE(L.info.has_bn, "train_buffer: no dA for detection convs"); *ptr = gten_ptr(net, L.out); *ld = net->bufs[L.out.buf].ld;
             if (L.upsample) { h *= 2; w *= 2; } break;
-    case 3: YB_REQUIRE(layer > 0, "train_buffer: layer 0 reads the image"); *ptr = ten_ptr2(net, L.in); *ld = net->bufs[L.in.buf].ld;
+    case 3: YB_REQUIRE(layer > 0, "train_buffer: layer 0 reads the image"); *ptr = ten_ptr(net, L.in); *ld = net->bufs[L.in.buf].ld;
             h = L.info.in_h; w = L.info.in_w; break;
     case 4: YB_REQUIRE(layer > 0 && net->par, "train_buffer: the stem has no dgrad weights");   // [cin_pad * k * k][k_cout], 16-bit
             *ptr = net->par + L.w_dgrad; *ld = L.k_cout; h = yb_conv_cout_pad(L.info.cin); w = L.info.ksize * L.info.ksize; break;
