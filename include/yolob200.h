@@ -568,9 +568,17 @@ int yb_net_train_refresh_dgrad(yb_net* net, void* stream);
 int yb_net_get_conv_params(yb_net* net, int layer, float** w_ohwi, float** gamma, float** beta, float** mean,
                            float** var, float** bias);
 int yb_net_layer_grad(yb_net* net, int layer, float** dw, float** dgamma, float** dbeta, float** dbias);
-/* training scratch of one layer (tests): which = 0 raw conv output z, 1 its gradient dz (zero-inserted at the input
- * resolution for stride-2 layers), 2 gradient w.r.t. the layer output, 3 the layer's input activation.
- * All 16-bit [n, h, w, ld]. */
+/* training scratch of one layer (tests), 16-bit, h x w rows of row pitch ld:
+ *   0  z: the raw conv output, [n, out_h, out_w, ld]
+ *   1  dz: its gradient, [n, out_h, out_w, ld] (YB_DGRAD_S2=dilated stride-2 layers: zero-inserted at the input
+ *      resolution); the detection heads' dz has ld = cout rounded up to 32, the pad columns zero
+ *   2  dA: the gradient w.r.t. the layer output, [n, h, w, ld] (2x upsampled outputs: at the upsampled size)
+ *   3  in: the layer's input activation, [n, in_h, in_w, ld] (a concat slice: ld is the concat buffer's)
+ *   4  the dgrad weights (parameter arena): rows h = cin_pad x w = k * k taps, ld = k_cout (cout rounded up to 32);
+ *      stride-1 layers hold the flip + transpose of the weights, stride-2 parity layers the four class matrices
+ *   5  dX: the gradient w.r.t. the layer's input, the tensor its dgrad writes, [n, in_h, in_w, ld]
+ *   6  w16: the 16-bit forward weights (parameter arena), h = cout_pad rows x w = 1 of ld = k * k * cin (OHWI)
+ * Layer 0 (the stem) has no 3, 4, 5 or 6. */
 int yb_net_train_buffer(yb_net* net, int layer, int which, void** ptr, int* ld, int* h, int* w);
 /* device pointer + geometry of one layer's output activation (tests / debugging). */
 int yb_net_layer_output(const yb_net* net, int layer, void** ptr, int* ld, int* dtype);

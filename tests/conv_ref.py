@@ -85,7 +85,7 @@ def out_bound(ref, S, n16, dtype, scale=None, shift=None, res=None):
 def check_out(got, ref, bound, what=""):
     """Assert |got - ref| <= bound elementwise; returns the worst |got - ref| / bound."""
     err = (got.double() - ref).abs()
-    frac = err / bound
+    frac = torch.where(err == 0, 0.0, err / bound)     # exact where the bound is 0 (all-zero operands): fine
     bad = ~(frac <= 1.0)                               # NaN counts as bad
     if bool(bad.any()):
         idx = tuple(bad.nonzero()[0].tolist())

@@ -433,7 +433,7 @@ def test_train_backward_self_consistency():
             a.backward(dA)
             e_dz = float((dz - z.grad).norm() / z.grad.norm().clamp(min=1e-20))
         w = plan.conv_params(i)["w"].permute(0, 3, 1, 2).contiguous().half().float().requires_grad_(True)   # OHWI -> OIHW
-        xr = xin.permute(0, 3, 1, 2).contiguous().requires_grad_(True)
+        xr = xin.permute(0, 3, 1, 2).contiguous()
         out = F.conv2d(xr, w, None, stride=info.stride, padding=info.ksize // 2)
         out.backward(dz[..., :info.cout].permute(0, 3, 1, 2))
         gw = plan.layer_grads(i)["w"]

@@ -700,7 +700,11 @@ extern "C" int yb_net_train_buffer(yb_net* net, int layer, int which, void** ptr
             h = L.info.in_h; w = L.info.in_w; break;
     case 4: YB_REQUIRE(layer > 0 && net->par, "train_buffer: the stem has no dgrad weights");   // [cin_pad * k * k][k_cout], 16-bit
             *ptr = net->par + L.w_dgrad; *ld = L.k_cout; h = yb_conv_cout_pad(L.info.cin); w = L.info.ksize * L.info.ksize; break;
-    default: set_error("train_buffer: which must be 0..4"); return YB_ERR_INVALID_ARGUMENT;
+    case 5: YB_REQUIRE(layer > 0, "train_buffer: the stem has no dgrad, so no input gradient");   // what the dgrad writes
+            *ptr = gten_ptr(net, L.in); *ld = net->bufs[L.in.buf].ld; h = L.info.in_h; w = L.info.in_w; break;
+    case 6: YB_REQUIRE(layer > 0 && net->par, "train_buffer: the stem reads its fp32 master weights");   // [cout_pad][k * k * cin]
+            *ptr = net->par + L.w_packed; *ld = L.info.ksize * L.info.ksize * L.info.cin; h = L.cout_pad; w = 1; break;
+    default: set_error("train_buffer: which must be 0..6"); return YB_ERR_INVALID_ARGUMENT;
   }
   if (rows_h) *rows_h = h;
   if (rows_w) *rows_w = w;

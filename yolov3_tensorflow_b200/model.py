@@ -94,16 +94,21 @@ class _Plan:
         return out
 
     def train_buffer(self, i, which):
-        """Strided view [n,h,w,c] of layer i's training scratch: which = 'z' | 'dz' | 'dA' | 'in'."""
-        code = {"z": 0, "dz": 1, "dA": 2, "in": 3}[which]
+        """Strided view [n,h,w,c] of layer i's training scratch: which = 'z' | 'dz' | 'dA' | 'in' | 'dX' (the gradient
+        w.r.t. the layer input, which its dgrad writes), or the layer's 16-bit forward weights 'w16' as [cout_pad,
+        k*k*cin] (parameter arena)."""
+        code = {"z": 0, "dz": 1, "dA": 2, "in": 3, "dX": 5, "w16": 6}[which]
         p, ld, hh, ww = C.c_void_p(), C.c_int(), C.c_int(), C.c_int()
         check(lib.yb_net_train_buffer(self.handle, i, code, C.byref(p), C.byref(ld), C.byref(hh), C.byref(ww)), "yb_net_train_buffer")
+        tdt = torch.float16 if self.act_dtype == torch.float16 else torch.bfloat16
+        if which == "w16":
+            off = p.value - self.par.data_ptr()
+            return self.par[off: off + hh.value * ld.value * 2].view(tdt).view(hh.value, ld.value)
         info = self.layer_info(i)
-        c = info.cin if which == "in" else info.cout
+        c = info.cin if which in ("in", "dX") else info.cout
         off = p.value - self.act.data_ptr()
         h, w = hh.value, ww.value
         nelem = (self.n * h * w - 1) * ld.value + c
-        tdt = torch.float16 if self.act_dtype == torch.float16 else torch.bfloat16
         flat = self.act[off: off + nelem * 2].view(tdt)
         return flat.as_strided((self.n, h, w, c), (h * w * ld.value, w * ld.value, ld.value, 1))
 
