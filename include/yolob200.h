@@ -412,8 +412,17 @@ int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* info);
 /* Host-only unless sm_count == 0: the kernel, multicast-cluster shape and persistent grid the forward of a plan
  * (yb_net_forward / yb_net_detect, current options) launches for `layer`.  sm_count > 0: a device with that many SMs,
  * max_clusters = sm_count / (cluster_m * cluster_n); sm_count == 0: the current device, max_clusters from
- * cudaOccupancyMaxActiveClusters for the kernel.  igemm = 0 (all other fields 0): the layer runs the stem or the halo
- * kernel.  The detection heads are reported as yb_net_forward runs them (unfused). */
+ * cudaOccupancyMaxActiveClusters for the kernel.  igemm = 0: the layer runs another kernel, named by `kernel`; of the
+ * other fields only residual and res_smem are then set.  The detection heads are reported as yb_net_forward runs them
+ * (unfused).
+ * kernel (every layer, layer 0 included):
+ *   YB_LAYER_IGEMM       the implicit-GEMM conv (igemm = 1)
+ *   YB_LAYER_HALO        the halo-tile kernel (Cin = 32 layers by default; YB_HALO=0: none, YB_HALO=1: wherever it applies)
+ *   YB_LAYER_FUSED_STEM  layers 0 and 1: the stem is computed inside Conv_1's halo launch, layer 0's output is never
+ *                        written (the default; YB_STEM_FUSE=0 or YB_HALO=0 turn it off)
+ *   YB_LAYER_STEM        layer 0 as its own launch: the mma.sync stem, or the CUDA-core stem under YB_THIN=0
+ *   YB_LAYER_THIN        the mma.sync halo-tile kernel of the Cin = 32 3x3 convs (YB_THIN=2) */
+enum { YB_LAYER_IGEMM = 1, YB_LAYER_HALO = 2, YB_LAYER_FUSED_STEM = 3, YB_LAYER_STEM = 4, YB_LAYER_THIN = 5 };
 typedef struct yb_layer_schedule_info {
   int igemm;         /* 1: the implicit-GEMM conv                                                  */
   int pingpong;      /* 1: ping-pong schedule, 0: cooperative                                       */
@@ -427,6 +436,7 @@ typedef struct yb_layer_schedule_info {
   int residual;      /* 1: the layer adds a shortcut (also reported for the halo-kernel layers)     */
   int res_smem;      /* 1: the shortcut tile is TMA-prefetched into shared memory during the main   */
                      /*    loop (YB_CONV_RES); 0: the epilogue reads it from global memory          */
+  int kernel;        /* YB_LAYER_*: what the forward launches for this layer (above)                */
 } yb_layer_schedule_info;
 int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info);
 int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes);

@@ -17,6 +17,7 @@ YB_OPT_SGD, YB_OPT_MOMENTUM, YB_OPT_RMSPROP, YB_OPT_ADAM = 0, 1, 2, 3
 YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
 YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
 YB_VOC_MAX_GT = 1024
+YB_LAYER_IGEMM, YB_LAYER_HALO, YB_LAYER_FUSED_STEM, YB_LAYER_STEM, YB_LAYER_THIN = 1, 2, 3, 4, 5
 
 
 class YoloB200Error(RuntimeError):
@@ -46,7 +47,7 @@ class ConvSchedule(C.Structure):   # yb_conv_schedule_info
 
 class LayerSchedule(C.Structure):  # yb_layer_schedule_info
     _fields_ = [(n, i32) for n in ("igemm", "pingpong", "cluster_m", "cluster_n", "block_m", "block_n", "num_m_tiles",
-                                   "num_n_tiles", "units", "max_clusters", "grid", "residual", "res_smem")]
+                                   "num_n_tiles", "units", "max_clusters", "grid", "residual", "res_smem", "kernel")]
 
 
 class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info

@@ -261,9 +261,16 @@ extern "C" int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* in
 extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info) {
   YB_REQUIRE(net && info && layer >= 0 && layer < (int)net->layers.size() && sm_count >= 0, "layer_schedule: bad argument");
   memset(info, 0, sizeof(*info));
+  const LayerKernel k = layer_kernel(net, layer);
+  switch (k) {
+    case LayerKernel::FusedStem: info->kernel = YB_LAYER_FUSED_STEM; break;
+    case LayerKernel::Stem: info->kernel = YB_LAYER_STEM; break;
+    case LayerKernel::Thin: info->kernel = YB_LAYER_THIN; break;
+    case LayerKernel::Halo: info->kernel = YB_LAYER_HALO; break;
+    case LayerKernel::Igemm: info->kernel = YB_LAYER_IGEMM; break;
+  }
   if (layer == 0) return YB_OK;                        // the stem
   const Layer& L = net->layers[layer];
-  const LayerKernel k = layer_kernel(net, layer);
   const yb_conv_desc d = layer_desc(net, L);
   info->residual = L.res.buf >= 0 ? 1 : 0;
   if (k == LayerKernel::Halo) info->res_smem = info->residual && conv_halo_res_smem(&d);
