@@ -117,6 +117,9 @@ typedef struct yb_conv_schedule_info {
   int cluster_m;     /* CTAs of a cluster along M (each a different m-tile)                     */
   int cluster_n;     /* CTAs of a cluster along N (1 | 2; 1 under the cooperative schedule)     */
   int units;         /* work units: ceil(num_m_tiles / cluster_m) x num_n_tiles / cluster_n     */
+  int epi_tma;       /* 1: the epilogue packs the accumulator fragments to 16 bits and stores them by TMA */
+                     /*    (YB_CONV_EPI=tma, or unset in a 16-bit inference plan); 0: staged or register. */
+                     /*    A launch with a residual takes it only if res_smem                             */
 } yb_conv_schedule_info;
 int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_stats, int sm_count, yb_conv_schedule_info* info);
 
@@ -437,6 +440,7 @@ typedef struct yb_layer_schedule_info {
   int res_smem;      /* 1: the shortcut tile is TMA-prefetched into shared memory during the main   */
                      /*    loop (YB_CONV_RES); 0: the epilogue reads it from global memory          */
   int kernel;        /* YB_LAYER_*: what the forward launches for this layer (above)                */
+  int epi_tma;       /* 1: the TMA-store epilogue (YB_CONV_EPI); 0: the staged or register epilogue  */
 } yb_layer_schedule_info;
 int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info);
 int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes);

@@ -113,8 +113,9 @@ def main():
             check(lib.yb_net_layer_schedule(plan.handle, i, 0, C.byref(sc)), "yb_net_layer_schedule")
             # shortcut: "ldg" read by the epilogue from global memory, "smem" prefetched into shared memory
             row["res"] = ("smem" if sc.res_smem else "ldg") if sc.residual else ""
-            if kern == "conv_igemm":           # the plan's schedule: ping-pong / cooperative, multicast cluster shape
-                row["sched"] = ("pp " if sc.pingpong else "co ") + f"{sc.cluster_m}x{sc.cluster_n}"
+            if kern == "conv_igemm":           # the plan's schedule: ping-pong / cooperative, multicast cluster shape,
+                row["sched"] = (("pp " if sc.pingpong else "co ") + f"{sc.cluster_m}x{sc.cluster_n}" +   # TMA-store epilogue
+                                (" tma" if sc.epi_tma else ""))
         if i > 0:
             for _ in range(3):
                 run(i)
@@ -130,14 +131,14 @@ def main():
         rows.append(row)
 
     print(f"# card: {card()}   SMs: {sms}   batch {B}, {S}x{S}, fp16, {args.reps} reps per layer")
-    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'sched':<6} {'res':<4} {'tiles':>6} {'kb':>4}"
+    print(f"{'L':>3} {'cin':>5} {'cout':>5} {'k':>2} {'s':>2} {'out':>4} {'kernel':<10} {'sched':<10} {'res':<4} {'tiles':>6} {'kb':>4}"
           f" {'waves':>5} {'ms':>8} {'TFLOP/s':>8}")
     for r in rows:
         if r["layer"] == 0:
             continue
         tf = r["gflop"] / r["ms"] if r["ms"] > 0 else 0.0
         print(f"{r['layer']:>3} {r['cin']:>5} {r['cout']:>5} {r['k']:>2} {r['s']:>2} {r['hw']:>4} {r['kernel']:<10}"
-              f" {r['sched']:<6} {r['res']:<4} {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
+              f" {r['sched']:<10} {r['res']:<4} {r.get('tiles', ''):>6} {r.get('kb', ''):>4} {r.get('waves', ''):>5} {r['ms']:8.4f} {tf:8.1f}")
     conv_ms = sum(r["ms"] for r in rows)
     igemm = [r for r in rows if r["kernel"] == "conv_igemm"]
     igemm_ms = sum(r["ms"] for r in igemm)

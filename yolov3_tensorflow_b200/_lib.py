@@ -42,12 +42,13 @@ class ConvDesc(C.Structure):
 class ConvSchedule(C.Structure):   # yb_conv_schedule_info
     _fields_ = [(n, i32) for n in ("pingpong", "consumers", "cluster", "block_m", "block_n", "block_k", "stages", "num_kb",
                                    "num_m_tiles", "num_n_tiles", "grid", "res_smem", "res_stages", "cluster_m",
-                                   "cluster_n", "units")]
+                                   "cluster_n", "units", "epi_tma")]
 
 
 class LayerSchedule(C.Structure):  # yb_layer_schedule_info
     _fields_ = [(n, i32) for n in ("igemm", "pingpong", "cluster_m", "cluster_n", "block_m", "block_n", "num_m_tiles",
-                                   "num_n_tiles", "units", "max_clusters", "grid", "residual", "res_smem", "kernel")]
+                                   "num_n_tiles", "units", "max_clusters", "grid", "residual", "res_smem", "kernel",
+                                   "epi_tma")]
 
 
 class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info

@@ -195,6 +195,21 @@ __device__ __forceinline__ void bulk_wait_group() {        // at most N most-rec
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// ---- stmatrix / ldmatrix: four 8x8 matrices of 16-bit elements between registers and shared memory ----
+// Lane l gives the address of row l & 7 (16 bytes) of matrix l >> 3; register i of lane l holds row l >> 2, columns
+// 2 (l & 3) and + 1 of matrix i, which is the layout of a wgmma accumulator fragment packed to 16 bits.
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t saddr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(saddr)
+               : "memory");
+}
+
 // ---- clusters: TMA multicast, cluster-wide barrier, remote mbarrier arrive ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

@@ -35,8 +35,10 @@ struct ConvParams {
   float res_scale, out_inv_scale;
   int res_smem;           // 1: the ping-pong kernel TMA-prefetches the residual tile into shared memory (YB_CONV_RES)
   CUtensorMap tmR;        // res_smem: the residual as a [M, cout] matrix, 128-row x 64-channel 128B-swizzled boxes
-  // The rest of the conv_igemm_kernel instantiation conv_select picks (consumers, pingpong, cluster, cluster_n and
-  // res_smem above are the others); host only, after every field the kernel reads.
+  int epi_tma;            // 1: the epilogue stays in the accumulator layout and stores 16-bit boxes by TMA (YB_CONV_EPI)
+  CUtensorMap tmO;        // epi_tma: the output as a [M, cout] matrix of pitch out_ld, 16-row x 64-channel 128B-swizzled boxes
+  // The rest of the conv_igemm_kernel instantiation conv_select picks (consumers, pingpong, cluster, cluster_n,
+  // res_smem and epi_tma above are the others); host only, after every field the kernel reads.
   int dtype;              // yb_dtype of the operands
   int block_n;            // output channels per tile
   int block_kb;           // bytes of one k-block row
@@ -62,7 +64,7 @@ struct ConvRequest {
   int det_e = 0;           // > 0: detection head with the decode fused into the epilogue, 5 + C = det_e columns per
                            // anchor, d.cout = 3 * det_e; one n-tile spans the whole padded cout and `out` is never written
   bool plan_rule = false;  // a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
-                           // YB_CONV_MCAST is unset
+                           // YB_CONV_MCAST is unset, and the TMA-store epilogue when YB_CONV_EPI is
 };
 
 // The kernel of r, down to its conv_igemm_kernel instantiation, which must exist (no pointers, no device work)

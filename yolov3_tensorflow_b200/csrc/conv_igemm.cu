@@ -27,7 +27,8 @@
 // The epilogue stages 32-column chunks of one 64-row accumulator block through shared memory so that each thread then
 // owns 16 consecutive channels of one pixel (two 16-byte stores per output row).  Ping-pong launches with a residual
 // (RES) find it already in shared memory: a second producer thread TMA-loads each unit's shortcut tile while the unit's
-// main loop runs.
+// main loop runs.  The forward layers of the 16-bit inference plans with a plain 16-bit output skip the staging tile
+// (TMA, epilogue_tma): each warp packs its fragments in registers and stores swizzled 16-row slabs by TMA.
 //
 // Replaces: slim.conv2d/batch_norm/leaky_relu (utils/layer_utils.py:20, model.py:43-49),
 // tf.add (utils/layer_utils.py:30), tf.pad (:15-16), resize_nearest_neighbor (:86),
@@ -78,6 +79,7 @@ struct Cfg {
   static constexpr uint32_t SBO = 8 * BKB;        // bytes between 8-row groups
 };
 static_assert(Cfg<256, 128, 2>::SMEM_BYTES <= 227 * 1024, "conv: the widest tile does not fit shared memory");
+static_assert(2 * 4 * 16 * 128 <= 2 * EPI_FLOATS * 4, "conv: the warps' 16-row output slabs do not fit the staging tiles");
 static_assert(Cfg<128, 128, 2, true>::SMEM_BYTES <= 227 * 1024 && Cfg<128, 128, 2, true>::STAGES >= 4,
               "conv: the shortcut tiles leave too short an operand ring");
 
@@ -340,6 +342,73 @@ __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float
   }
 }
 
+// TMA-store epilogue (TMA, 16-bit plain outputs; conv_select): the values never leave the accumulator layout.  Each
+// warp owns 16 rows of a 64-row accumulator block, so it works alone, without a warpgroup barrier: per 64-column box it
+// applies scale / shift (+leaky) (+residual) to its fragments in registers — the operations of epi_store16 in the
+// same order, so the outputs are the same bit for bit — packs them to 16 bits, writes them with four stmatrix.x4 into
+// a 16-row x 64-column slab of 128-byte rows in the TMA's 128B swizzle (conflict-free), and lane 0 stores the slab
+// through p.tmO, which clips rows >= M and columns >= cout.
+//   ss4[4 j + q]: (scale, scale, shift, shift) of columns 8 j + 2 q and + 1 of the tile.
+//   Without RES the warp has one slab (slab_h = slab_b = 0) and waits until the previous store has read it; such a
+//   launch has no residual (conv_select: a residual that is not prefetched keeps the staged epilogue).
+//   RES: the slab of block h, box b is the warp's 16 rows of the shortcut tile itself (slab + h slab_h + b slab_b),
+//   already in that layout: ldmatrix.x4 reads the residual as fragments and the result goes back over it.
+// acc: [NH][BN / 2]; row0: the first of the warp's 16 rows in block 0 (block h: + 64 h).
+template <typename T, int BN, int NH, bool RES>
+__device__ __forceinline__ void epilogue_tma(const ConvParams& p, const float (&acc)[NH][BN / 2], const int row0,
+                                             const int n0, const float4* ss4, uint8_t* slab, const uint32_t slab_h,
+                                             const uint32_t slab_b, const int lane) {
+  // lane = 8 i + r addresses row r + 8 (i & 1), 16-byte chunk (2 q + (i >> 1)) ^ r of the slab for the q-th stmatrix
+  const int r = lane & 7, mi = lane >> 3;
+  const uint32_t lane_off = (uint32_t)((r + 8 * (mi & 1)) * 128 + (((mi >> 1) ^ r) << 4));
+  const float slope = p.leaky ? 0.1f : 1.f;                    // fmaxf(v, 1 v) == v
+#pragma unroll
+  for (int h = 0; h < NH; ++h) {
+#pragma unroll
+    for (int b = 0; b < BN / 64; ++b) {
+      uint8_t* s = slab + h * slab_h + b * slab_b;
+      const uint32_t sa = smem_u32(s) + lane_off;              // the slab is 1024-byte aligned: ^ (q << 5) moves 2 q chunks
+      uint32_t pk[16];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {                            // stmatrix q: 8-column blocks 2 q and 2 q + 1 of the box
+        if constexpr (RES) ldmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+#pragma unroll
+        for (int ih = 0; ih < 2; ++ih) {
+          const int j = 8 * b + 2 * q + ih;                    // 8-column block of the tile
+          const float4 c = ss4[4 * j + (lane & 3)];
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {                     // rows lane >> 2 and + 8
+            float v0 = fmaf(acc[h][4 * j + 2 * hh], c.x, c.z);
+            float v1 = fmaf(acc[h][4 * j + 2 * hh + 1], c.y, c.w);
+            v0 = fmaxf(v0, slope * v0);
+            v1 = fmaxf(v1, slope * v1);
+            uint32_t& w = pk[4 * q + 2 * ih + hh];
+            if constexpr (RES) {
+              const float2 f = Pack2<T>::unpack(w);
+              v0 += f.x; v1 += f.y;
+            }
+            w = Pack2<T>::pack(v0, v1);
+          }
+        }
+        // RES: nothing else reads these rows of the shortcut tile, so each result goes straight back
+        if constexpr (RES) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+      }
+      if constexpr (!RES) {
+        if (lane == 0) bulk_wait_group_read<0>();              // the previous store has read the slab
+        __syncwarp();
+#pragma unroll
+        for (int q = 0; q < 4; ++q) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+      }
+      fence_proxy_async();                                     // the slab as written is what the TMA reads
+      __syncwarp();
+      if (lane == 0 && row0 + h * WG_ROWS < p.M && n0 + b * 64 < p.cout) {
+        tma_store_2d(&p.tmO, s, n0 + b * 64, row0 + h * WG_ROWS);
+        bulk_commit_group();
+      }
+    }
+  }
+}
+
 // named barriers (0 = __syncthreads; 1, 2 = the consumer warpgroups' own barriers): MMA_TURN + w = "warpgroup w may
 // start its next main loop" (ping-pong)
 static constexpr int MMA_TURN_BAR = 3;
@@ -356,13 +425,17 @@ static constexpr int MMA_TURN_BAR = 3;
 // RES (ping-pong, 16-bit, p.res != nullptr, YB_CONV_RES): the shortcut tile of every work unit is prefetched by TMA
 // (p.tmR) into its warpgroup's shared-memory tile while the unit's main loop runs, and the epilogue adds it from there
 // instead of waiting on a global load per 32-column chunk.  Each CTA loads its own tile (never multicast).
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false>
+// TMA (16-bit, NC = 2, no fused decode; p.epi_tma): the TMA-store epilogue (epilogue_tma) in place of the staged one.
+// The warps' output slabs lie where the staging tiles would; with RES they are the shortcut tile itself.
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
+          bool TMA = false>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
   static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
   static_assert(!RES || (PP && sizeof(T) == 2), "the shared-memory shortcut tile is a 16-bit ping-pong variant");
   static_assert(CM != 0 || CN == 1, "a run-time cluster shape is p.cluster x 1");
+  static_assert(!TMA || (sizeof(T) == 2 && NC == 2 && DET_E == 0), "the TMA-store epilogue: 16-bit, 128-row tiles, no fused decode");
   constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
   using C = Cfg<BN, BKB, NC, RES>;
   constexpr int BK = BKB / (int)sizeof(T);               // channels per k-block
@@ -393,6 +466,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // them may multicast into it next): ping-pong, the 4 warps of the one warpgroup that read it
       mbar_init(&empty_bar[i], 4 * (PP ? 1 : NC) * (CM ? CM * CN : p.cluster));
     }
+    if constexpr (TMA) tma_prefetch_desc(&p.tmO);
     if constexpr (RES) {
       tma_prefetch_desc(&p.tmR);
       for (int i = 0; i < NC; ++i) {
@@ -495,7 +569,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // cooperative: warpgroup cw computes rows [64 cw, 64 cw + 64) of every tile of the CTA;
     // ping-pong: warpgroup cw computes all 128 rows of every other tile of the CTA (its j-th unit is the CTA's 2j + cw-th)
     using Mma = typename ConvMma<T, BN>::type;
-    constexpr bool kRegEpi = !PP && !std::is_same<T, __nv_fp8_e4m3>::value;   // YB_CONV_EPI=reg: 16-bit only
+    constexpr bool kRegEpi = !PP && !TMA && !std::is_same<T, __nv_fp8_e4m3>::value;   // YB_CONV_EPI=reg: 16-bit only
     const int cw = wg - 1;
     const int t = threadIdx.x & 127;
     const int lane = t & 31;
@@ -578,14 +652,40 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (n0 != ss_n0) {
         warpgroup_bar(bar_id);                   // nobody still reads the previous n-tile's values
         for (int c = t; c < BN; c += 128) {
-          sss[c] = p.scale ? __ldg(p.scale + n0 + c) : 1.f;      // scale = shift = NULL: identity (dgrad convs)
-          sss[BN + c] = p.shift ? __ldg(p.shift + n0 + c) : 0.f;
+          const float sc = p.scale ? __ldg(p.scale + n0 + c) : 1.f;   // scale = shift = NULL: identity (dgrad convs)
+          const float sh = p.shift ? __ldg(p.shift + n0 + c) : 0.f;
+          if constexpr (TMA) {                   // (scale, scale, shift, shift) per column pair: one load per fragment
+            sss[(c >> 1) * 4 + (c & 1)] = sc;
+            sss[(c >> 1) * 4 + 2 + (c & 1)] = sh;
+          } else {
+            sss[c] = sc;
+            sss[BN + c] = sh;
+          }
         }
         warpgroup_bar(bar_id);
         ss_n0 = n0;
       }
       if constexpr (DET_E > 0) {
         epilogue_detect<BN, DET_E>(p, acc[0], m0 + cw * WG_ROWS, t, stg, sss, bar_id);
+      } else if constexpr (TMA) {
+        if (m0 < p.M) {                          // units wholly past M store nothing
+          const int wrow = 16 * (t >> 5);        // this warp's rows of each 64-row block
+          const int row0 = m0 + (PP ? 0 : cw * WG_ROWS) + wrow;
+          if constexpr (RES) {
+            mbar_wait(&res_full[cw], res_phase);
+            epilogue_tma<T, BN, NH, true>(p, acc, row0, n0, reinterpret_cast<const float4*>(sss),
+                                          sR + cw * C::RES_TILE_BYTES + wrow * 128, WG_ROWS * 128, C::RES_BOX_BYTES, lane);
+            // the stores have read the warp's rows of the tile: the producer may refill it
+            if (lane == 0) {
+              bulk_wait_group_read<0>();
+              mbar_arrive(&res_empty[cw]);
+            }
+            res_phase ^= 1;
+          } else {
+            epilogue_tma<T, BN, NH, false>(p, acc, row0, n0, reinterpret_cast<const float4*>(sss),
+                                           reinterpret_cast<uint8_t*>(s_epi) + (cw * 4 + (t >> 5)) * 2048, 0, 0, lane);
+          }
+        }
       } else if (kRegEpi && p.epi_reg) {
         if constexpr (kRegEpi) epilogue_reg<T, BN>(p, acc[0], m0 + cw * WG_ROWS, n0, sss, t);
       } else {
@@ -644,6 +744,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
     if (p.stat_sum != nullptr && cur_n0 >= 0) stat_flush<BN>(p, sst, cur_n0, t, bar_id);
+    if constexpr (TMA) {
+      if (lane == 0) bulk_wait_group<0>();       // this warp's output stores are complete before the CTA may exit
+    }
   }
   if (cs > 1) cluster_sync_all();                        // no CTA exits while a peer may still multicast into it or arrive on it
 }
@@ -825,29 +928,37 @@ static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads,
 }
 
 // One conv_igemm_kernel instantiation: the type conv_kernel_for passes to its functor
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false>
+template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
+          bool TMA = false>
 struct ConvKernel {
   using C = Cfg<BN, BKB, NC, RES>;
-  static constexpr auto kernel = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES>;
+  static constexpr auto kernel = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES, TMA>;
 };
 
 static int no_conv_kernel(const ConvParams& p) {
   set_error("conv: no kernel for dtype %d, %d-column tiles, %d-byte k-blocks, %d consumer warpgroups, ping-pong %d, "
-            "%d x %d cluster, shortcut tile %d, fused decode of %d columns", p.dtype, p.block_n, p.block_kb, p.consumers,
-            p.pingpong, p.cluster / p.cluster_n, p.cluster_n, p.res_smem, p.det_e);
+            "%d x %d cluster, shortcut tile %d, TMA-store epilogue %d, fused decode of %d columns", p.dtype, p.block_n,
+            p.block_kb, p.consumers, p.pingpong, p.cluster / p.cluster_n, p.cluster_n, p.res_smem, p.epi_tma, p.det_e);
   return YB_ERR_UNSUPPORTED;
 }
 
 // ping-pong: the cluster shape (cluster / cluster_n) x cluster_n is a template parameter; e4m3 runs unclustered
+template <typename T, int BN, int BKB, bool RES, bool TMA, typename F>
+static int conv_kernel_pp_shape(const ConvParams& p, F& f) {
+  const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
+  if (cm == 1 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 1, RES, TMA>());
+  if constexpr (sizeof(T) == 2) {
+    if (cm == 2 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 1, RES, TMA>());
+    if (cm == 1 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 2, RES, TMA>());
+    if (cm == 2 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 2, RES, TMA>());
+  }
+  return no_conv_kernel(p);
+}
+// ... and the epilogue: staged, or (16-bit) the TMA store
 template <typename T, int BN, int BKB, bool RES, typename F>
 static int conv_kernel_pp(const ConvParams& p, F& f) {
-  const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
-  if (cm == 1 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 1, RES>());
-  if constexpr (sizeof(T) == 2) {
-    if (cm == 2 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 1, RES>());
-    if (cm == 1 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 2, RES>());
-    if (cm == 2 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 2, RES>());
-  }
+  if (!p.epi_tma) return conv_kernel_pp_shape<T, BN, BKB, RES, false>(p, f);
+  if constexpr (sizeof(T) == 2) return conv_kernel_pp_shape<T, BN, BKB, RES, true>(p, f);
   return no_conv_kernel(p);
 }
 
@@ -866,9 +977,10 @@ static int conv_kernel_tile(const ConvParams& p, F& f) {
   // warpgroup as well
   const bool shape = p.cluster_n == 1 && (p.cluster == 1 || (b16 && (p.cluster == 2 || p.cluster == 4)));
   if (!shape || p.res_smem) return no_conv_kernel(p);
-  if (p.consumers == 2) return f(ConvKernel<T, BN, BKB, 2, DET_E>());
+  if (p.consumers == 2 && !p.epi_tma) return f(ConvKernel<T, BN, BKB, 2, DET_E>());
   if constexpr (b16 && DET_E == 0) {
-    if (p.consumers == 1) return f(ConvKernel<T, BN, BKB, 1>());
+    if (p.consumers == 2) return f(ConvKernel<T, BN, BKB, 2, 0, false, 0, 1, false, true>());
+    if (p.consumers == 1 && !p.epi_tma) return f(ConvKernel<T, BN, BKB, 1>());
   }
   return no_conv_kernel(p);
 }
@@ -1001,6 +1113,8 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
   //   YB_CONV_MODE=2cta   cooperative clusters of 2 x 1 CTAs (YB_CONV_MC=1: 4 x 1), multicasting the weight tile
   //   YB_CONV_EPI=reg     accumulators stored straight from registers (not with BN statistics: those sum columns
   //                       over the staging tile)
+  //   YB_CONV_EPI=stage|tma  the staged epilogue everywhere | the TMA-store epilogue (epilogue_tma) wherever it can
+  //                       run (below); unset: the TMA store in the 16-bit inference plans, staged elsewhere
   //   YB_CONV_PP=0|1      0: the cooperative schedule wherever ping-pong would run; 1: ping-pong wherever the kernel
   //                       allows it (two consumer warpgroups, no cluster, staged epilogue), the 1x1 convs with
   //                       128-column tiles included; unset: the shape rule below
@@ -1012,13 +1126,18 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
   //                       the ping-pong kernel prefetches it into shared memory where it can (below)
   p->consumers = (!det && opt("YB_CONV_EG")[0] == '1') ? 1 : 2;
   p->cluster = (!det && opt("YB_CONV_MODE")[0] == '2') ? (opt("YB_CONV_MC")[0] == '1' ? 4 : 2) : 1;
-  p->epi_reg = (!det && !r.stats && opt("YB_CONV_EPI")[0] == 'r') ? 1 : 0;
+  const char* eo = opt("YB_CONV_EPI");
+  YB_REQUIRE(eo[0] == '\0' || strcmp(eo, "reg") == 0 || strcmp(eo, "stage") == 0 || strcmp(eo, "tma") == 0,
+             "conv: YB_CONV_EPI must be reg, stage or tma (got '%s')", eo);
+  p->epi_reg = (!det && !r.stats && eo[0] == 'r') ? 1 : 0;
   p->ctas = opt_int("YB_CONV_CTAS", 0);
   // ping-pong wherever the default variant runs, except
   //  - the fused-decode heads: their 256-column tile does not fit 128 rows per warpgroup in registers;
   //  - 1x1 convs with 128-column tiles: their main loop (cin / 64 k-blocks) is too short to hide one warpgroup's
-  //    128 x 128 epilogue, and on H100 they measured 2-7 % slower ping-pong than with two warpgroups sharing the
-  //    epilogue (DESIGN.md §5).  The 1x1 convs with 64-column tiles and every windowed conv gain from it.
+  //    128 x 128 staged epilogue, and on H100 they measured 2-7 % slower ping-pong than with two warpgroups sharing
+  //    the epilogue.  With the TMA-store epilogue ping-pong measured 2-9 % faster on them instead (one clean run of
+  //    two, DESIGN.md §5); the rule is kept until that is measured again.  The 1x1 convs with 64-column tiles and
+  //    every windowed conv gain from ping-pong.
   const char* pp = opt("YB_CONV_PP");
   const bool pp_shape = pp[0] == '1' || (pp[0] != '0' && (kh * kw > 1 || bn != 128));
   p->pingpong = (!det && p->consumers == 2 && p->cluster == 1 && !p->epi_reg && pp_shape) ? 1 : 0;
@@ -1058,6 +1177,12 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
   p->det_e = det;
   p->res_smem = (r.res && p->pingpong && !e4m3 && !det && bn == 128 && p->block_kb == 128 && !r.scatter &&
                  !d->upsample2x && !d->out_fp32 && strcmp(ro, "ldg") != 0) ? 1 : 0;
+  // The TMA-store epilogue writes plain 16-bit [M, cout] boxes of 128-row tiles: no statistics (they sum columns over
+  // the staging tile), no fp32 or fused-decode head, no 2x upsample or dgrad window (rows scattered elsewhere), no e4m3,
+  // and no residual read from global memory (the address arithmetic beside 128 live accumulators spills): a residual
+  // only as the shortcut tile above, which the epilogue updates in place.
+  p->epi_tma = ((eo[0] == 't' || (eo[0] == '\0' && r.plan_rule)) && !e4m3 && !det && !r.stats && p->consumers == 2 &&
+                !d->out_fp32 && !d->upsample2x && !win && (!r.res || p->res_smem)) ? 1 : 0;
   p->cout = d->cout; p->cin = d->cin; p->ksize = d->ksize; p->stride = d->stride; p->pad = pad;
   p->kh = kh; p->kw = kw; p->scatter = r.scatter;
   p->im2col = kh * kw > 1;
@@ -1093,6 +1218,12 @@ int conv_prepare(const ConvRequest& r, const void* x, const void* w_packed, cons
   if (p->res_smem) {
     // the shortcut as a [M, cout] matrix of row pitch res_ld: 128-row x 64-channel boxes, rows past M zero-filled
     rc = make_tmap_2d(&p->tmR, res, d->dtype, p->M, d->cout, d->res_ld, 64 * p->consumers, 64, 0);
+    if (rc) return rc;
+  }
+  if (p->epi_tma) {
+    // the output (a channel slice of its buffer included) as a [M, cout] matrix of row pitch out_ld: one warp's 16 rows
+    // x 64 channels per store, rows >= M and channels >= cout clipped
+    rc = make_tmap_2d(&p->tmO, out, d->dtype, p->M, d->cout, d->out_ld, 16, 64, 0);
     if (rc) return rc;
   }
   if (p->im2col) {
@@ -1152,6 +1283,7 @@ extern "C" int yb_conv_schedule(const yb_conv_desc* d, int kh, int kw, int with_
   rc = stages(pr, &info->res_stages);
   if (rc) return rc;
   info->res_smem = pr.res_smem;
+  info->epi_tma = p.epi_tma;
   info->pingpong = p.pingpong;
   info->consumers = p.consumers;
   info->cluster = p.cluster;

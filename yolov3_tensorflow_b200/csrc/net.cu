@@ -283,6 +283,7 @@ extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count,
   if (rc) return rc;
   info->igemm = 1;
   info->res_smem = p.res_smem;
+  info->epi_tma = p.epi_tma;
   info->pingpong = p.pingpong;
   info->cluster_m = p.cluster / p.cluster_n;
   info->cluster_n = p.cluster_n;
