@@ -141,10 +141,11 @@ int yb_stem_conv_fwd_tc(const float* x, const float* w_ohwi, const float* scale,
 int yb_stem_conv_fwd_tc_stats(const float* x, const float* w_ohwi, const float* scale, const float* shift, int n, int h,
                               int w, int dtype, int leaky, void* out, float* stat_sum, float* stat_sqsum, void* stream);
 
-/* 3x3 convs with cin in {32, 64} and cout in {64, 128} (darknet53_body Conv_1/3/6/8, utils/layer_utils.py:36-44) from
- * a shared-memory HALO tile: one tiled TMA load per 16x8-pixel output tile (four parity planes for stride 2), the nine
- * taps are nine UMMA descriptors into that tile, weights resident in shared memory (csrc/conv_halo.cu).  Same contract
- * as yb_conv2d_fwd without statistics; 16-bit output; (w / stride) % 8 == 0.  yb_conv3x3_halo_supported: 1 if d fits. */
+/* 3x3 convs with cin in {32, 64} and cout in {64, 128}, except 64 -> 128 at stride 2 (darknet53_body Conv_1/3/6/8,
+ * utils/layer_utils.py:36-44) from a shared-memory HALO tile: one tiled TMA load per 16x8-pixel output tile (four parity
+ * planes for stride 2), the nine taps are nine wgmma descriptors into that tile, weights resident in shared memory
+ * (csrc/conv_halo.cu).  Same contract as yb_conv2d_fwd without statistics; fp16 / bf16, 16-bit output;
+ * (w / stride) % 8 == 0.  yb_conv3x3_halo_supported: 1 if d fits. */
 int yb_conv3x3_halo_supported(const yb_conv_desc* d);
 int yb_conv3x3_halo_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
                         const float* shift, const void* res, void* out, void* stream);

@@ -200,3 +200,28 @@ def test_wgrad_schedule_forced_splits_clamp():
     i = _wgrad_schedule(big, sms=4, YB_WGRAD_SPLITS="1000")
     assert (i.splits, i.kb_per_split, i.tiles) == (984, 22, 1)       # 21632 blocks: ceil(21632 / 1000) = 22 per split
     assert _wgrad_schedule(big, YB_WGRAD_SPLITS="1000", YB_WGRAD_TP="1").tiles == 1
+
+
+def test_conv3x3_halo_supported_grid():
+    """yb_conv3x3_halo_supported (csrc/conv_halo.cu): 3x3 convs, stride 1 | 2, cin 32 | 64 and cout 64 | 128 except
+    64 -> 128 at stride 2 (its weights and one parity-plane stage exceed shared memory), fp16 / bf16 operands, a 16-bit
+    non-upsampled output, an output width (w / stride) that is a multiple of 8 and leading dimensions that are multiples
+    of 8."""
+    import ctypes as C
+    import itertools
+    from yolov3_tensorflow_b200 import _lib as L
+    got, want = set(), set()
+    for cin, cout, s, wo, dt, f32, up, bad_ld in itertools.product((32, 64, 96), (32, 64, 128), (1, 2), (16, 24, 20),
+                                                                   (L.YB_F16, L.YB_BF16, L.YB_E4M3), (0, 1), (0, 1),
+                                                                   (None, "in", "out")):
+        d = L.ConvDesc(n=2, h=16 * s, w=wo * s, cin=cin, cout=cout, ksize=3, stride=s,
+                       in_ld=cin + (4 if bad_ld == "in" else 0), out_ld=cout + (4 if bad_ld == "out" else 0), res_ld=0,
+                       dtype=dt, out_fp32=f32, leaky=1, upsample2x=up)
+        key = (cin, cout, s, wo, dt, f32, up, bad_ld)
+        if L.lib.yb_conv3x3_halo_supported(C.byref(d)):
+            got.add(key)
+        if (cin in (32, 64) and cout in (64, 128) and (cin, cout, s) != (64, 128, 2) and wo % 8 == 0
+                and dt in (L.YB_F16, L.YB_BF16) and not f32 and not up and bad_ld is None):
+            want.add(key)
+    assert got == want
+    assert len(want) == 7 * 2 * 2       # 7 (cin, cout, stride) kernels x 2 widths x 2 types

@@ -1,4 +1,5 @@
-// Shared between conv_igemm.cu (kernel + launcher) and net.cu (network plan).
+// Shared between the wgmma conv files (conv_igemm.cu, conv_halo.cu, conv_wgrad.cu) and the network plan (net.cu,
+// net_train.cu).
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
@@ -105,19 +106,63 @@ struct HaloParams {
   // 1: the output is e4m3 codes of value * out_inv_scale (Conv_3 of the fp8 plan: fp16 in, e4m3 out)
   int out_e4m3;
   float out_inv_scale;
-  int res_smem;                // 1: the residual is TMA-loaded with each tile's halo (YB_CONV_RES; conv_halo_res_smem)
+  int res_smem;                // 1: the residual is TMA-loaded with each tile's halo (Conv_3's shape; YB_CONV_RES)
+  // The rest of the conv_halo_kernel instantiation halo_select picks (cout, out_e4m3 and res_smem above are the others);
+  // host only, after every field the kernel reads.
+  int dtype;                   // yb_dtype of the input and the weights
+  int cin, stride;
+  int stem;                    // 1: the stem fused in (stem_w ...)
 };
+// What a halo-tile launch computes, without its data pointers: halo_select picks its kernel from this alone.
+struct HaloRequest {
+  yb_conv_desc d;
+  bool res = false;        // adds a residual
+  bool out_e4m3 = false;   // the output is e4m3 codes of value * out_inv_scale (Conv_3 of the fp8 plan: fp16 in)
+  bool stem = false;       // the stem (3->32, 3x3/1, BN + leaky) fused into Conv_1 (32->64, 3x3/2): d describes Conv_1,
+                           // whose input, the stem's output, is never written; the input is the float32 image [n, d.h, d.w, 3]
+};
+// One halo-tile launch (host only): the tensor maps and the parameters they were encoded for.
+struct HaloLaunch {
+  HaloMaps maps;
+  HaloParams p;
+};
+// The kernel of r, down to its conv_halo_kernel instantiation, which must exist (no pointers, no device work)
+int halo_select(const HaloRequest& r, HaloParams* p);
+// halo_select of the plain request (no residual, 16-bit output, no fused stem) succeeds
 bool conv_halo_supported(const yb_conv_desc* d);
-bool conv_halo_res_smem(const yb_conv_desc* d);
-int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, HaloMaps* maps, HaloParams* p);
-int conv_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);
-// stem (3->32, 3x3/1, BN + leaky) fused into Conv_1 (32->64, 3x3/2): d describes Conv_1 (its input = the stem's output,
-// which is never written); image float32 [n, d->h, d->w, 3].
-int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const float* stem_w, const float* stem_scale,
-                           const float* stem_shift, const void* w_packed, const float* scale, const float* shift, void* out,
-                           HaloMaps* maps, HaloParams* p);
-int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st);
+// halo_select, then the tensor maps over the data pointers.  x is the input activation, or with r.stem the image;
+// res is given exactly when r asks for it, stem_w [32][27] OHWI, stem_scale and stem_shift [32] exactly with r.stem.
+int conv_halo_prepare(const HaloRequest& r, const void* x, const void* w_packed, const float* scale, const float* shift,
+                      const void* res, void* out, const float* stem_w, const float* stem_scale, const float* stem_shift,
+                      HaloLaunch* l);
+int conv_halo_launch(const HaloLaunch& l, cudaStream_t st);
+// weight gradient of a conv (csrc/conv_wgrad.cu)
+struct WgradParams {
+  long P;              // output pixels n*ho*wo
+  int ho, wo;
+  int cin, cout, ksize, stride, pad;
+  int kb_per_split;    // 64-pixel blocks per CTA
+  int num_kb;          // ceil(P / 64)
+  int n_chunks;        // cin / BNW
+  int a_dilated;       // dz lives zero-inserted in an [n, 2ho, 2wo, cout] buffer (stride-2 layers): gather it by im2col
+  float* dw;           // [cout, k*k*cin] fp32, accumulated
+  // The conv_wgrad_kernel instantiation and grid wgrad_select picks; host only, after every field the kernel reads.
+  int dtype;           // yb_dtype of x and dz
+  int bnw, tp;         // input channels per tap and tile, filter taps per CTA
+  int grid_x, grid_y, grid_z;   // pixel splits, tap groups x input-channel chunks, 128-row output-channel tiles
+};
+struct WgradLaunch {
+  CUtensorMap tmA, tmB;
+  WgradParams p;
+};
+// The kernel and grid of the weight gradient of the conv d on a device with sm_count SMs, with the current options
+// (YB_WGRAD_TP, YB_WGRAD_EPI, YB_WGRAD_SPLITS; no pointers, no device work)
+int wgrad_select(const yb_conv_desc* d, int sm_count, WgradParams* p);
+// wgrad_select for the current device, then the tensor maps over x, dz [rows, dz_ld] (dz_dilated: zero-inserted, see
+// yb_conv2d_wgrad) and dw
+int wgrad_prepare(const yb_conv_desc* d, const void* x, const void* dz, int dz_ld, int dz_dilated, float* dw,
+                  WgradLaunch* l);
+int wgrad_launch(const WgradLaunch& l, cudaStream_t st);
 int conv_launch(const ConvLaunch& l, cudaStream_t st);
 // what conv_launch would launch on the current device, without launching: grid (CTAs) and the most clusters of
 // p.cluster CTAs that can be resident at once (cudaOccupancyMaxActiveClusters; the SM count when p.cluster == 1)

@@ -439,103 +439,141 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
   }
 }
 
-template <typename T, int CIN, int COUT, int STRIDE, typename TO = T, bool RES = false>
-static int launch_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-  using C = HaloCfg<CIN, COUT, STRIDE, RES>;
-  static DeviceOnce once;
-  auto kern = conv_halo_kernel<T, CIN, COUT, STRIDE, 0, TO, RES>;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  kern<<<grid, HALO_THREADS, C::SMEM_BYTES, st>>>(maps, p);
-  YB_CUDA(cudaGetLastError());
-  return YB_OK;
-}
-
 static constexpr int STEM_WARPS = 8;           // stem producer warps of the fused kernel (640 threads per CTA)
 
-template <typename T>
-static int launch_stem_halo(const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-  using C = HaloCfg<32, 64, 2>;
-  constexpr int SMEM = C::SMEM_BYTES + StemCfg::NIN * StemCfg::IN_BYTES;
-  static_assert(SMEM <= 227 * 1024, "fused stem + Conv_1 does not fit shared memory");
-  static DeviceOnce once;
-  auto kern = conv_halo_kernel<T, 32, 64, 2, STEM_WARPS>;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), SMEM); if (rc) return rc; }
-  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  kern<<<grid, HALO_THREADS + 32 * STEM_WARPS, SMEM, st>>>(maps, p);
-  YB_CUDA(cudaGetLastError());
-  return YB_OK;
-}
+// One conv_halo_kernel instantiation: the type halo_kernel_for passes to its functor
+template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T, bool RES = false>
+struct HaloKernel {
+  static constexpr int THREADS = HALO_THREADS + 32 * STEMW;
+  static constexpr int SMEM_BYTES =
+      HaloCfg<CIN, COUT, STRIDE, RES>::SMEM_BYTES + (STEMW > 0 ? StemCfg::NIN * StemCfg::IN_BYTES : 0);
+  static_assert(SMEM_BYTES <= 227 * 1024, "halo conv: configuration does not fit shared memory");
+  static constexpr auto kernel = conv_halo_kernel<T, CIN, COUT, STRIDE, STEMW, TO, RES>;
+};
 
-int conv_stem_halo_prepare(const yb_conv_desc* d, const float* image, const float* stem_w, const float* stem_scale,
-                           const float* stem_shift, const void* w_packed, const float* scale, const float* shift, void* out,
-                           HaloMaps* maps, HaloParams* p) {
-  YB_REQUIRE(d->ksize == 3 && d->stride == 2 && d->cin == 32 && d->cout == 64 && !d->out_fp32 && !d->upsample2x,
-             "conv_stem_halo: Conv_1 is 3x3/2 32->64 (got k=%d s=%d %d->%d)", d->ksize, d->stride, d->cin, d->cout);
-  YB_REQUIRE(d->h % 2 == 0 && d->w % 16 == 0 && d->out_ld % 8 == 0 && d->out_ld >= 64, "conv_stem_halo: bad geometry (h=%d w=%d)", d->h, d->w);
-  YB_REQUIRE(image && stem_w && stem_scale && stem_shift && w_packed && scale && shift && out, "conv_stem_halo: null pointer");
-  YB_REQUIRE(((uintptr_t)image & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0, "conv_stem_halo: pointers must be 16-byte aligned");
-  memset(maps, 0, sizeof(*maps));
-  memset(p, 0, sizeof(*p));
-  p->n = d->n; p->ho = d->h / 2; p->wo = d->w / 2;
-  p->tiles_x = p->wo / HT_W; p->tiles_y = ceil_div(p->ho, HT_H);
-  p->num_tiles = p->tiles_x * p->tiles_y * d->n;
-  p->cout = d->cout; p->leaky = d->leaky; p->scale = scale; p->shift = shift;
-  p->res = nullptr; p->res_ld = 0; p->out = out; p->out_ld = d->out_ld;
-  p->stem_w = stem_w; p->stem_scale = stem_scale; p->stem_shift = stem_shift; p->in_h = d->h; p->in_w = d->w;
-  int rc = make_tmap_image3d(&maps->in3d, image, d->n, d->h, d->w, StemCfg::IN_ROWF, StemCfg::IN_ROWS);
-  if (rc) return rc;
-  const long K = 9L * d->cin;
-  return make_tmap_2d(&maps->w, w_packed, d->dtype, yb_conv_cout_pad(d->cout), K, K, d->cout, d->cin, 1);
-}
-
-int conv_stem_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-#define YB_STEM_LAUNCH(T) return launch_stem_halo<T>(maps, p, st);
-  if (d->dtype == YB_F16) { YB_STEM_LAUNCH(__half) }
-  if (d->dtype == YB_BF16) { YB_STEM_LAUNCH(__nv_bfloat16) }
-#undef YB_STEM_LAUNCH
-  set_error("conv_stem_halo: dtype must be f16 or bf16");
+static int no_halo_kernel(const HaloParams& p) {
+  set_error("conv_halo: no kernel for dtype %d, cin=%d cout=%d stride=%d, fused stem %d, e4m3 output %d, residual box %d",
+            p.dtype, p.cin, p.cout, p.stride, p.stem, p.out_e4m3, p.res_smem);
   return YB_ERR_UNSUPPORTED;
 }
 
-// the residual of a launch with one is TMA-loaded with the halo (Conv_3's shape only) unless YB_CONV_RES=ldg
-bool conv_halo_res_smem(const yb_conv_desc* d) {
-  return d->cin == 32 && d->cout == 64 && d->stride == 1 && strcmp(opt("YB_CONV_RES"), "ldg") != 0;
+template <typename T, typename F>
+static int halo_kernel_type(const HaloParams& p, F& f) {
+  const int ci = p.cin, co = p.cout, s = p.stride;
+  if (p.stem) {
+    if (ci == 32 && co == 64 && s == 2 && !p.out_e4m3 && !p.res_smem) return f(HaloKernel<T, 32, 64, 2, STEM_WARPS>());
+    return no_halo_kernel(p);
+  }
+  if (ci == 32 && co == 64 && s == 1) {   // Conv_3: the residual box, and (fp16 in) the fp8 plan's e4m3 output
+    if (!p.out_e4m3) return p.res_smem ? f(HaloKernel<T, 32, 64, 1, 0, T, true>()) : f(HaloKernel<T, 32, 64, 1>());
+    if constexpr (std::is_same<T, __half>::value)
+      return p.res_smem ? f(HaloKernel<T, 32, 64, 1, 0, __nv_fp8_e4m3, true>()) : f(HaloKernel<T, 32, 64, 1, 0, __nv_fp8_e4m3>());
+    return no_halo_kernel(p);
+  }
+  if (p.out_e4m3 || p.res_smem) return no_halo_kernel(p);
+  if (ci == 32 && co == 64 && s == 2) return f(HaloKernel<T, 32, 64, 2>());
+  if (ci == 32 && co == 128 && s == 1) return f(HaloKernel<T, 32, 128, 1>());
+  if (ci == 32 && co == 128 && s == 2) return f(HaloKernel<T, 32, 128, 2>());
+  if (ci == 64 && co == 64 && s == 1) return f(HaloKernel<T, 64, 64, 1>());
+  if (ci == 64 && co == 64 && s == 2) return f(HaloKernel<T, 64, 64, 2>());
+  if (ci == 64 && co == 128 && s == 1) return f(HaloKernel<T, 64, 128, 1>());
+  return no_halo_kernel(p);   // (64 -> 128 at stride 2: the weights and one parity-plane stage exceed shared memory)
 }
 
-bool conv_halo_supported(const yb_conv_desc* d) {
-  if (d->ksize != 3 || (d->stride != 1 && d->stride != 2)) return false;
-  if (!(d->cin == 32 || d->cin == 64) || !(d->cout == 64 || d->cout == 128)) return false;
-  if (d->cin == 64 && d->cout == 128 && d->stride == 2) return false;   // weights + one parity-plane stage exceed shared memory
-  if (d->out_fp32 || d->upsample2x) return false;
-  if (d->h % d->stride || d->w % d->stride || (d->w / d->stride) % HT_W) return false;
-  if (d->in_ld % 8 || d->out_ld % 8 || d->in_ld < d->cin || d->out_ld < d->cout) return false;
-  return d->dtype == YB_F16 || d->dtype == YB_BF16;
+// The instantiation table: every conv_halo_kernel that exists is named here and nowhere else.  Calls
+// f(HaloKernel<...>()) with the instantiation halo_select recorded in p and returns what f returns, or
+// YB_ERR_UNSUPPORTED when there is none.
+template <typename F>
+static int halo_kernel_for(const HaloParams& p, F&& f) {
+  if (p.dtype == YB_F16) return halo_kernel_type<__half>(p, f);
+  if (p.dtype == YB_BF16) return halo_kernel_type<__nv_bfloat16>(p, f);
+  return no_halo_kernel(p);
 }
 
-int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale, const float* shift,
-                      const void* res, void* out, HaloMaps* maps, HaloParams* p) {
-  YB_REQUIRE(conv_halo_supported(d), "conv_halo: unsupported configuration (k=%d s=%d cin=%d cout=%d w=%d)", d->ksize,
-             d->stride, d->cin, d->cout, d->w);
-  YB_REQUIRE(x && w_packed && scale && shift && out, "conv_halo: null pointer");
-  YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 && ((uintptr_t)res & 15) == 0,
-             "conv_halo: pointers must be 16-byte aligned");
-  if (res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0, "conv_halo: res_ld %d invalid", d->res_ld);
-  memset(maps, 0, sizeof(*maps));
+template <typename K>
+static int halo_launch_kernel(const HaloLaunch& l, cudaStream_t st) {
+  static DeviceOnce once;
+  auto kern = K::kernel;
+  const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), K::SMEM_BYTES);
+  if (rc) return rc;
+  const int grid = l.p.num_tiles < num_sms() ? l.p.num_tiles : num_sms();
+  kern<<<grid, K::THREADS, K::SMEM_BYTES, st>>>(l.maps, l.p);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+// Launch a prepared halo-tile conv (conv_halo_prepare): the kernel halo_select recorded in l.p, with the maps built for it
+int conv_halo_launch(const HaloLaunch& l, cudaStream_t st) {
+  return halo_kernel_for(l.p, [&](auto k) -> int { return halo_launch_kernel<decltype(k)>(l, st); });
+}
+
+// Shape checks, tiling and kernel of one halo-tile conv: everything conv_halo_prepare decides before it looks at the
+// data pointers, down to the conv_halo_kernel instantiation, which must exist.  The launches, conv_halo_supported and
+// yb_net_layer_schedule all select through here.
+int halo_select(const HaloRequest& r, HaloParams* p) {
   memset(p, 0, sizeof(*p));
+  const yb_conv_desc* d = &r.d;
+  YB_REQUIRE(d->ksize == 3 && (d->stride == 1 || d->stride == 2), "conv_halo: 3x3 stride 1|2 only (got k=%d s=%d)",
+             d->ksize, d->stride);
+  YB_REQUIRE(!d->out_fp32 && !d->upsample2x, "conv_halo: 16-bit, non-upsampled outputs only");
+  YB_REQUIRE(d->h % d->stride == 0 && d->w % d->stride == 0 && (d->w / d->stride) % HT_W == 0,
+             "conv_halo: h, w must be multiples of the stride and the output width of %d (got %d x %d)", HT_W, d->h, d->w);
+  YB_REQUIRE(d->out_ld >= d->cout && d->out_ld % 8 == 0, "conv_halo: out_ld %d invalid", d->out_ld);
+  if (r.stem) {
+    YB_REQUIRE(!r.res && !r.out_e4m3, "conv_halo: the fused stem's Conv_1 has no residual and a 16-bit output");
+  } else {
+    YB_REQUIRE(d->in_ld >= d->cin && d->in_ld % 8 == 0, "conv_halo: in_ld %d invalid", d->in_ld);
+  }
+  // e4m3 codes are stored 16 channels (16 bytes) at a time
+  if (r.out_e4m3) YB_REQUIRE(d->out_ld % 16 == 0, "conv_halo: an e4m3 output needs out_ld %% 16 == 0 (got %d)", d->out_ld);
+  if (r.res) YB_REQUIRE(d->res_ld >= d->cout && d->res_ld % 8 == 0, "conv_halo: res_ld %d invalid", d->res_ld);
   p->n = d->n; p->ho = d->h / d->stride; p->wo = d->w / d->stride;
   p->tiles_x = p->wo / HT_W; p->tiles_y = ceil_div(p->ho, HT_H);
   p->num_tiles = p->tiles_x * p->tiles_y * d->n;
-  p->cout = d->cout; p->leaky = d->leaky; p->scale = scale; p->shift = shift;
-  p->res = res; p->res_ld = d->res_ld; p->out = out; p->out_ld = d->out_ld;
-  int rc;
-  p->res_smem = res != nullptr && conv_halo_res_smem(d);
+  p->cout = d->cout; p->leaky = d->leaky;
+  p->res_ld = d->res_ld; p->out_ld = d->out_ld;
+  if (r.stem) { p->in_h = d->h; p->in_w = d->w; }
+  p->out_e4m3 = r.out_e4m3;
+  // the residual of Conv_3's shape is TMA-loaded with the halo unless YB_CONV_RES=ldg
+  p->res_smem = (r.res && !r.stem && d->cin == 32 && d->cout == 64 && d->stride == 1 &&
+                 strcmp(opt("YB_CONV_RES"), "ldg") != 0) ? 1 : 0;
+  p->dtype = d->dtype; p->cin = d->cin; p->stride = d->stride; p->stem = r.stem;
+  return halo_kernel_for(*p, [](auto) -> int { return YB_OK; });
+}
+
+bool conv_halo_supported(const yb_conv_desc* d) {
+  HaloParams p;
+  return halo_select(HaloRequest{*d}, &p) == YB_OK;
+}
+
+// halo_select, then the tensor maps over the data pointers, which are baked into maps and parameters.
+int conv_halo_prepare(const HaloRequest& r, const void* x, const void* w_packed, const float* scale, const float* shift,
+                      const void* res, void* out, const float* stem_w, const float* stem_scale, const float* stem_shift,
+                      HaloLaunch* l) {
+  HaloParams* p = &l->p;
+  HaloMaps* maps = &l->maps;
+  int rc = halo_select(r, p);
+  if (rc) return rc;
+  const yb_conv_desc* d = &r.d;
+  YB_REQUIRE(x && w_packed && scale && shift && out, "conv_halo: null pointer");
+  YB_REQUIRE(r.stem ? stem_w && stem_scale && stem_shift : !stem_w && !stem_scale && !stem_shift,
+             "conv_halo: the stem's weights, scale and shift are given exactly when the request fuses the stem");
+  YB_REQUIRE((res != nullptr) == r.res, "conv_halo: a residual pointer is given exactly when the request has a residual");
+  YB_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0 && ((uintptr_t)out & 15) == 0 && ((uintptr_t)res & 15) == 0,
+             "conv_halo: pointers must be 16-byte aligned");
+  memset(maps, 0, sizeof(*maps));
+  p->scale = scale; p->shift = shift; p->res = res; p->out = out;
+  p->stem_w = stem_w; p->stem_scale = stem_scale; p->stem_shift = stem_shift;
   if (p->res_smem) {
     // the residual as {C, W, H, N} = [n, ho, wo, res_ld]: one 64-channel x 8 x 16-pixel box per tile
     rc = make_tmap_tiled4d(&maps->res, res, d->dtype, d->n, p->ho, p->wo, d->cout, d->res_ld, 64, HT_W, HT_H, 1);
     if (rc) return rc;
   }
-  if (d->stride == 1) {
+  if (r.stem) {
+    // the image's float32 halo of a tile (the plane maps stay zeroed: the stem producers write the planes)
+    rc = make_tmap_image3d(&maps->in3d, static_cast<const float*>(x), d->n, d->h, d->w, StemCfg::IN_ROWF, StemCfg::IN_ROWS);
+    if (rc) return rc;
+  } else if (d->stride == 1) {
     rc = make_tmap_tiled4d(&maps->plane[0], x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->cin, HT_W + 2, HT_H + 2, 1);
     if (rc) return rc;
   } else {
@@ -551,31 +589,6 @@ int conv_halo_prepare(const yb_conv_desc* d, const void* x, const void* w_packed
   return make_tmap_2d(&maps->w, w_packed, d->dtype, yb_conv_cout_pad(d->cout), K, K, d->cout, d->cin, 1);
 }
 
-int conv_halo_launch(const yb_conv_desc* d, const HaloMaps& maps, const HaloParams& p, cudaStream_t st) {
-  if (p.out_e4m3) {
-    if (d->dtype == YB_F16 && d->cin == 32 && d->cout == 64 && d->stride == 1 && p.out_ld % 16 == 0)
-      return p.res_smem ? launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3, true>(maps, p, st)
-                        : launch_halo<__half, 32, 64, 1, __nv_fp8_e4m3>(maps, p, st);
-    set_error("conv_halo: e4m3 output only for fp16 3x3/1 32->64 (got dtype %d cin=%d cout=%d stride=%d)", d->dtype, d->cin,
-              d->cout, d->stride);
-    return YB_ERR_UNSUPPORTED;
-  }
-#define YB_HALO(T)                                                                              \
-  if (d->cin == 32 && d->cout == 64 && d->stride == 1)                                          \
-    return p.res_smem ? launch_halo<T, 32, 64, 1, T, true>(maps, p, st) : launch_halo<T, 32, 64, 1>(maps, p, st); \
-  if (d->cin == 32 && d->cout == 64 && d->stride == 2) return launch_halo<T, 32, 64, 2>(maps, p, st);   \
-  if (d->cin == 32 && d->cout == 128 && d->stride == 1) return launch_halo<T, 32, 128, 1>(maps, p, st); \
-  if (d->cin == 32 && d->cout == 128 && d->stride == 2) return launch_halo<T, 32, 128, 2>(maps, p, st); \
-  if (d->cin == 64 && d->cout == 64 && d->stride == 1) return launch_halo<T, 64, 64, 1>(maps, p, st);   \
-  if (d->cin == 64 && d->cout == 64 && d->stride == 2) return launch_halo<T, 64, 64, 2>(maps, p, st);   \
-  if (d->cin == 64 && d->cout == 128 && d->stride == 1) return launch_halo<T, 64, 128, 1>(maps, p, st);
-  if (d->dtype == YB_F16) { YB_HALO(__half) }
-  else { YB_HALO(__nv_bfloat16) }
-#undef YB_HALO
-  set_error("conv_halo: no kernel for cin=%d cout=%d stride=%d", d->cin, d->cout, d->stride);
-  return YB_ERR_UNSUPPORTED;
-}
-
 }  // namespace yb
 
 using namespace yb;
@@ -585,11 +598,12 @@ extern "C" int yb_conv3x3_halo_supported(const yb_conv_desc* d) { return d && co
 extern "C" int yb_conv3x3_halo_fwd(const yb_conv_desc* d, const void* x, const void* w_packed, const float* scale,
                                    const float* shift, const void* res, void* out, void* stream) {
   if (!d) { set_error("conv_halo: null descriptor"); return YB_ERR_INVALID_ARGUMENT; }
-  HaloMaps maps;
-  HaloParams p;
-  int rc = conv_halo_prepare(d, x, w_packed, scale, shift, res, out, &maps, &p);
+  HaloRequest r{*d};
+  r.res = res != nullptr;
+  HaloLaunch l;
+  int rc = conv_halo_prepare(r, x, w_packed, scale, shift, res, out, nullptr, nullptr, nullptr, &l);
   if (rc) return rc;
-  return conv_halo_launch(d, maps, p, static_cast<cudaStream_t>(stream));
+  return conv_halo_launch(l, static_cast<cudaStream_t>(stream));
 }
 
 // Stem + Conv_1 in one kernel (utils/layer_utils.py:35-36): image float32 [n, h, w, 3] -> Conv_1's output [n, h/2, w/2, out_ld].
@@ -598,9 +612,10 @@ extern "C" int yb_stem_conv1_fused_fwd(const yb_conv_desc* d, const float* image
                                        const float* stem_scale, const float* stem_shift, const void* w_packed,
                                        const float* scale, const float* shift, void* out, void* stream) {
   if (!d) { set_error("stem_conv1_fused: null descriptor"); return YB_ERR_INVALID_ARGUMENT; }
-  HaloMaps maps;
-  HaloParams p;
-  int rc = conv_stem_halo_prepare(d, image, stem_w_ohwi, stem_scale, stem_shift, w_packed, scale, shift, out, &maps, &p);
+  HaloRequest r{*d};
+  r.stem = true;
+  HaloLaunch l;
+  int rc = conv_halo_prepare(r, image, w_packed, scale, shift, nullptr, out, stem_w_ohwi, stem_scale, stem_shift, &l);
   if (rc) return rc;
-  return conv_stem_halo_launch(d, maps, p, static_cast<cudaStream_t>(stream));
+  return conv_halo_launch(l, static_cast<cudaStream_t>(stream));
 }

@@ -447,19 +447,65 @@ stem_wgrad_tc_kernel(const float* __restrict__ x, const T* __restrict__ dz, int 
   }
 }
 
+// One conv_thin_kernel instantiation: the type thin_kernel_for passes to its functor
 template <typename T, int COUT, int STRIDE, bool STEM, bool SPLIT = false>
-static int launch_thin(const ThinParams& p, cudaStream_t st) {
+struct ThinKernel {
   using C = ThinCfg<T, COUT, STRIDE, STEM, SPLIT>;
-  auto kern = conv_thin_kernel<T, COUT, STRIDE, STEM, SPLIT>;
+  static constexpr auto kernel = conv_thin_kernel<T, COUT, STRIDE, STEM, SPLIT>;
+};
+
+// The instantiation a conv_thin_kernel launch needs.  Host only: ThinParams is the kernel's by-value parameter.
+struct ThinKey {
+  int dtype;           // yb_dtype of the 16-bit operands and output
+  int cout, stride;
+  bool stem, split;    // the stem (float32 image, 3 input channels); split-precision operands (stem only)
+};
+
+static int no_thin_kernel(const ThinKey& k) {
+  set_error("conv_thin: no kernel for dtype %d, cout=%d stride=%d, stem %d, split operands %d", k.dtype, k.cout, k.stride,
+            (int)k.stem, (int)k.split);
+  return YB_ERR_UNSUPPORTED;
+}
+
+template <typename T, typename F>
+static int thin_kernel_type(const ThinKey& k, F& f) {
+  if (k.stem) {
+    if (k.cout == 32 && k.stride == 1) return k.split ? f(ThinKernel<T, 32, 1, true, true>()) : f(ThinKernel<T, 32, 1, true>());
+    return no_thin_kernel(k);
+  }
+  if (k.split) return no_thin_kernel(k);
+  if (k.cout == 64 && k.stride == 1) return f(ThinKernel<T, 64, 1, false>());
+  if (k.cout == 64 && k.stride == 2) return f(ThinKernel<T, 64, 2, false>());
+  if (k.cout == 32 && k.stride == 1) return f(ThinKernel<T, 32, 1, false>());
+  if (k.cout == 32 && k.stride == 2) return f(ThinKernel<T, 32, 2, false>());
+  return no_thin_kernel(k);
+}
+
+// The instantiation table: every conv_thin_kernel that exists is named here and nowhere else.  Calls
+// f(ThinKernel<...>()) with the instantiation of k and returns what f returns, or YB_ERR_UNSUPPORTED when there is none.
+template <typename F>
+static int thin_kernel_for(const ThinKey& k, F&& f) {
+  if (k.dtype == YB_F16) return thin_kernel_type<__half>(k, f);
+  if (k.dtype == YB_BF16) return thin_kernel_type<__nv_bfloat16>(k, f);
+  return no_thin_kernel(k);
+}
+
+template <typename K>
+static int thin_launch_kernel(const ThinParams& p, cudaStream_t st) {
   static DeviceOnce once;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM); if (rc) return rc; }
-  int per_sm = 227 * 1024 / (C::SMEM + 1024);
+  auto kern = K::kernel;
+  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), K::C::SMEM); if (rc) return rc; }
+  int per_sm = 227 * 1024 / (K::C::SMEM + 1024);
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 8) per_sm = 8;
   const int grid = p.num_tiles < num_sms() * per_sm ? p.num_tiles : num_sms() * per_sm;
-  kern<<<grid, THIN_THREADS, C::SMEM, st>>>(p);
+  kern<<<grid, THIN_THREADS, K::C::SMEM, st>>>(p);
   YB_CUDA(cudaGetLastError());
   return YB_OK;
+}
+
+static int thin_launch(const ThinKey& key, const ThinParams& p, cudaStream_t st) {
+  return thin_kernel_for(key, [&](auto k) -> int { return thin_launch_kernel<decltype(k)>(p, st); });
 }
 
 }  // namespace yb
@@ -483,15 +529,7 @@ extern "C" int yb_conv3x3_thin_fwd(const yb_conv_desc* d, const void* x, const v
   p.tiles_y = ceil_div(p.ho, TH); p.tiles_x = ceil_div(p.wo, TW);
   p.num_tiles = p.tiles_x * p.tiles_y * d->n;
   p.leaky = d->leaky; p.dbg = 0; p.stat_sum = nullptr; p.stat_sqsum = nullptr;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define YB_THIN(T)                                                                         \
-  if (d->cout == 64 && d->stride == 1) return launch_thin<T, 64, 1, false>(p, st);        \
-  if (d->cout == 64 && d->stride == 2) return launch_thin<T, 64, 2, false>(p, st);        \
-  if (d->cout == 32 && d->stride == 1) return launch_thin<T, 32, 1, false>(p, st);        \
-  return launch_thin<T, 32, 2, false>(p, st);
-  if (d->dtype == YB_F16) { YB_THIN(__half) }
-  YB_THIN(__nv_bfloat16)
-#undef YB_THIN
+  return thin_launch(ThinKey{d->dtype, d->cout, d->stride, false, false}, p, static_cast<cudaStream_t>(stream));
 }
 
 // Stem on the warp-level tensor path: float32 image [n,h,w,3] -> 16-bit [n,h,w,32]; w_ohwi float32 [32][27].
@@ -510,14 +548,9 @@ extern "C" int yb_stem_conv_fwd_tc_stats(const float* x, const float* w_ohwi, co
   p.leaky = leaky;
   p.dbg = opt_int("YB_STEM_DBG", 0);
   p.stat_sum = stat_sum; p.stat_sqsum = stat_sqsum;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   // the statistics-producing form is the training forward: split-precision operands (YB_STEM_SPLIT=0: plain 16-bit)
   const bool split = stat_sum != nullptr && opt("YB_STEM_SPLIT")[0] != '0';
-  if (dtype == YB_F16) return split ? launch_thin<__half, 32, 1, true, true>(p, st) : launch_thin<__half, 32, 1, true>(p, st);
-  if (dtype == YB_BF16)
-    return split ? launch_thin<__nv_bfloat16, 32, 1, true, true>(p, st) : launch_thin<__nv_bfloat16, 32, 1, true>(p, st);
-  set_error("stem_tc: dtype must be f16 or bf16");
-  return YB_ERR_UNSUPPORTED;
+  return thin_launch(ThinKey{dtype, 32, 1, true, split}, p, static_cast<cudaStream_t>(stream));
 }
 extern "C" int yb_stem_conv_fwd_tc(const float* x, const float* w_ohwi, const float* scale, const float* shift, int n,
                                    int h, int w, int dtype, int leaky, void* out, void* stream) {

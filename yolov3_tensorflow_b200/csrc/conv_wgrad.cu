@@ -31,17 +31,6 @@ static constexpr int WG_THREADS = 384;  // warpgroup 0: TMA producer (one thread
 static constexpr int WG_BKP = 64;     // pixels per pipeline stage
 static constexpr int WG_BM = 128;     // output channels per tile
 
-struct WgradParams {
-  long P;              // output pixels n*ho*wo
-  int ho, wo;
-  int cin, cout, ksize, stride, pad;
-  int kb_per_split;    // 64-pixel blocks per CTA
-  int num_kb;          // ceil(P / 64)
-  int n_chunks;        // cin / BNW
-  int a_dilated;       // dz lives zero-inserted in an [n, 2ho, 2wo, cout] buffer (stride-2 layers): gather it by im2col
-  float* dw;           // [cout, k*k*cin] fp32, accumulated
-};
-
 template <int BNW, int TP>
 struct WCfg {
   static constexpr int BCH = BNW < 64 ? BNW : 64;            // channels per im2col box / swizzle row
@@ -176,17 +165,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 }
 
-template <typename T, int BNW, int TP>
-static int launch_wgrad(const CUtensorMap& tmA, const CUtensorMap& tmB, const WgradParams& p, dim3 grid, cudaStream_t st) {
-  using C = WCfg<BNW, TP>;
-  static DeviceOnce once;
-  auto kern = conv_wgrad_kernel<T, BNW, TP>;
-  { const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), C::SMEM_BYTES); if (rc) return rc; }
-  kern<<<grid, WG_THREADS, C::SMEM_BYTES, st>>>(tmA, tmB, p);
-  YB_CUDA(cudaGetLastError());
-  return YB_OK;
-}
-
 // Stem wgrad (cin = 3): CUDA cores.  Block = 256 output pixels; thread t accumulates the 27 x 32 products of
 // its pixel ... reduced per block in shared memory, then atomics.
 __global__ void __launch_bounds__(256)
@@ -242,27 +220,49 @@ long wgrad_pick_splits(long num_kb, long tiles, long sms, long epi_blocks) {
   return splits;
 }
 
-// Operand-ring depth of the kernel instantiation a (BNW, TP) pair runs.
-static int wgrad_stages(int bnw, int tp) {
-  if (bnw == 128) return WCfg<128, 1>::STAGES;
-  if (bnw == 64) return tp == 3 ? WCfg<64, 3>::STAGES : WCfg<64, 1>::STAGES;
-  return tp == 3 ? WCfg<32, 3>::STAGES : WCfg<32, 1>::STAGES;
+// One conv_wgrad_kernel instantiation: the type wgrad_kernel_for passes to its functor
+template <typename T, int BNW, int TP>
+struct WgradKernel {
+  using C = WCfg<BNW, TP>;
+  static constexpr auto kernel = conv_wgrad_kernel<T, BNW, TP>;
+};
+
+static int no_wgrad_kernel(const WgradParams& p) {
+  set_error("wgrad: no kernel for dtype %d, %d channels per tap, %d taps per CTA", p.dtype, p.bnw, p.tp);
+  return YB_ERR_UNSUPPORTED;
 }
 
-}  // namespace yb
+template <typename T, typename F>
+static int wgrad_kernel_type(const WgradParams& p, F& f) {
+  if (p.bnw == 128 && p.tp == 1) return f(WgradKernel<T, 128, 1>());
+  if (p.bnw == 64 && p.tp == 3) return f(WgradKernel<T, 64, 3>());
+  if (p.bnw == 64 && p.tp == 1) return f(WgradKernel<T, 64, 1>());
+  if (p.bnw == 32 && p.tp == 3) return f(WgradKernel<T, 32, 3>());
+  if (p.bnw == 32 && p.tp == 1) return f(WgradKernel<T, 32, 1>());
+  return no_wgrad_kernel(p);
+}
 
-using namespace yb;
+// The instantiation table: every conv_wgrad_kernel that exists is named here and nowhere else.  Calls
+// f(WgradKernel<...>()) with the instantiation wgrad_select recorded in p and returns what f returns, or
+// YB_ERR_UNSUPPORTED when there is none.
+template <typename F>
+static int wgrad_kernel_for(const WgradParams& p, F&& f) {
+  if (p.dtype == YB_F16) return wgrad_kernel_type<__half>(p, f);
+  if (p.dtype == YB_BF16) return wgrad_kernel_type<__nv_bfloat16>(p, f);
+  return no_wgrad_kernel(p);
+}
 
-// Host-only: the kernel and grid yb_conv2d_wgrad launches for `d` on a device with sm_count SMs, with the current options
-// (YB_WGRAD_TP, YB_WGRAD_EPI, YB_WGRAD_SPLITS).  yb_conv2d_wgrad calls it with the device's SM count.
-extern "C" int yb_wgrad_schedule(const yb_conv_desc* d, int sm_count, yb_wgrad_schedule_info* info) {
-  YB_REQUIRE(d && info && sm_count > 0, "wgrad_schedule: bad argument");
+// Shape checks, kernel and grid of one weight gradient: everything wgrad_prepare decides before it looks at the data
+// pointers, down to the conv_wgrad_kernel instantiation, which must exist.
+int wgrad_select(const yb_conv_desc* d, int sm_count, WgradParams* p) {
+  memset(p, 0, sizeof(*p));
   YB_REQUIRE(d->ksize == 1 || d->ksize == 3, "wgrad: ksize must be 1 or 3");
   YB_REQUIRE(d->stride == 1 || d->stride == 2, "wgrad: stride must be 1 or 2");
   YB_REQUIRE(d->cin > 0 && d->cin % 32 == 0, "wgrad: cin must be a positive multiple of 32 (got %d)", d->cin);
   YB_REQUIRE(d->cout > 0 && d->n > 0 && d->h >= d->stride && d->w >= d->stride, "wgrad: empty problem");
   YB_REQUIRE(d->dtype == YB_F16 || d->dtype == YB_BF16, "wgrad: dtype must be f16 or bf16");
-  const long P = (long)d->n * (d->h / d->stride) * (d->w / d->stride);
+  const int ho = d->h / d->stride, wo = d->w / d->stride;
+  const long P = (long)d->n * ho * wo;
   const long num_kb = ceil_div(P, WG_BKP);
   YB_REQUIRE(num_kb <= 0x7fffffff, "wgrad: too many output pixels");
   const int taps = d->ksize * d->ksize;
@@ -284,57 +284,90 @@ extern "C" int yb_wgrad_schedule(const yb_conv_desc* d, int sm_count, yb_wgrad_s
   }
   const long kb_per_split = ceil_div(num_kb, splits);
   splits = ceil_div(num_kb, kb_per_split);
-  info->bnw = bnw;
-  info->tp = tp;
-  info->stages = wgrad_stages(bnw, tp);
-  info->num_kb = (int)num_kb;
-  info->kb_per_split = (int)kb_per_split;
-  info->splits = (int)splits;
-  info->tiles = (int)tiles;
-  info->grid_x = (int)splits;
-  info->grid_y = tap_groups * n_chunks;
-  info->grid_z = co_tiles;
+  p->P = P; p->ho = ho; p->wo = wo;
+  p->cin = d->cin; p->cout = d->cout; p->ksize = d->ksize; p->stride = d->stride; p->pad = d->ksize / 2;
+  p->kb_per_split = (int)kb_per_split;
+  p->num_kb = (int)num_kb;
+  p->n_chunks = n_chunks;
+  p->dtype = d->dtype;
+  p->bnw = bnw;
+  p->tp = tp;
+  p->grid_x = (int)splits;
+  p->grid_y = tap_groups * n_chunks;
+  p->grid_z = co_tiles;
+  return wgrad_kernel_for(*p, [](auto) -> int { return YB_OK; });
+}
+
+// wgrad_select, then the tensor maps over the data pointers, which are baked into maps and parameters.
+int wgrad_prepare(const yb_conv_desc* d, const void* x, const void* dz, int dz_ld, int dz_dilated, float* dw,
+                  WgradLaunch* l) {
+  YB_REQUIRE(x && dz && dw, "wgrad: null pointer");
+  WgradParams* p = &l->p;
+  int rc = wgrad_select(d, num_sms(), p);
+  if (rc) return rc;
+  YB_REQUIRE(dz_ld >= d->cout && dz_ld % 8 == 0 && d->in_ld % 8 == 0, "wgrad: bad leading dimensions");
+  p->dw = dw;
+  p->a_dilated = dz_dilated ? 1 : 0;
+  if (dz_dilated) {
+    YB_REQUIRE(d->stride == 2, "wgrad: dz_dilated only applies to stride-2 layers");
+    rc = make_tmap_im2col_px(&l->tmA, dz, d->dtype, d->n, d->h, d->w, d->cout, dz_ld, 1, 2, 0, 64, WG_BKP);
+  } else {
+    rc = make_tmap_2d(&l->tmA, dz, d->dtype, p->P, d->cout, dz_ld, WG_BKP, 64, 0);
+  }
+  if (rc) return rc;
+  return make_tmap_im2col_px(&l->tmB, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->ksize, d->stride, p->pad,
+                             p->bnw < 64 ? p->bnw : 64, WG_BKP);
+}
+
+template <typename K>
+static int wgrad_launch_kernel(const WgradLaunch& l, cudaStream_t st) {
+  static DeviceOnce once;
+  auto kern = K::kernel;
+  const int rc = ensure_smem_attr(once, reinterpret_cast<const void*>(kern), K::C::SMEM_BYTES);
+  if (rc) return rc;
+  const dim3 grid((unsigned)l.p.grid_x, (unsigned)l.p.grid_y, (unsigned)l.p.grid_z);
+  kern<<<grid, WG_THREADS, K::C::SMEM_BYTES, st>>>(l.tmA, l.tmB, l.p);
+  YB_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+// Launch a prepared weight gradient (wgrad_prepare): the kernel and grid wgrad_select recorded in l.p
+int wgrad_launch(const WgradLaunch& l, cudaStream_t st) {
+  return wgrad_kernel_for(l.p, [&](auto k) -> int { return wgrad_launch_kernel<decltype(k)>(l, st); });
+}
+
+}  // namespace yb
+
+using namespace yb;
+
+// Host-only: the kernel and grid yb_conv2d_wgrad launches for `d` on a device with sm_count SMs, with the current options
+// (YB_WGRAD_TP, YB_WGRAD_EPI, YB_WGRAD_SPLITS).
+extern "C" int yb_wgrad_schedule(const yb_conv_desc* d, int sm_count, yb_wgrad_schedule_info* info) {
+  YB_REQUIRE(d && info && sm_count > 0, "wgrad_schedule: bad argument");
+  WgradParams p;
+  int rc = wgrad_select(d, sm_count, &p);
+  if (rc) return rc;
+  info->bnw = p.bnw;
+  info->tp = p.tp;
+  rc = wgrad_kernel_for(p, [&](auto k) -> int { info->stages = decltype(k)::C::STAGES; return YB_OK; });
+  if (rc) return rc;
+  info->num_kb = p.num_kb;
+  info->kb_per_split = p.kb_per_split;
+  info->splits = p.grid_x;
+  info->tiles = p.grid_y * p.grid_z;
+  info->grid_x = p.grid_x;
+  info->grid_y = p.grid_y;
+  info->grid_z = p.grid_z;
   return YB_OK;
 }
 
 extern "C" int yb_conv2d_wgrad(const yb_conv_desc* d, const void* x, const void* dz, int dz_ld, int dz_dilated,
                                float* dw, void* stream) {
-  YB_REQUIRE(d && x && dz && dw, "wgrad: null pointer");
-  yb_wgrad_schedule_info s;
-  { const int rc = yb_wgrad_schedule(d, num_sms(), &s); if (rc) return rc; }
-  YB_REQUIRE(dz_ld >= d->cout && dz_ld % 8 == 0 && d->in_ld % 8 == 0, "wgrad: bad leading dimensions");
-  const int ho = d->h / d->stride, wo = d->w / d->stride;
-  WgradParams p;
-  p.P = (long)d->n * ho * wo; p.ho = ho; p.wo = wo;
-  p.cin = d->cin; p.cout = d->cout; p.ksize = d->ksize; p.stride = d->stride; p.pad = d->ksize / 2;
-  p.num_kb = s.num_kb;
-  p.kb_per_split = s.kb_per_split;
-  p.n_chunks = d->cin / s.bnw;
-  p.dw = dw;
-  const int bnw = s.bnw, tp = s.tp;
-  CUtensorMap tmA, tmB;
-  p.a_dilated = dz_dilated ? 1 : 0;
-  int rc;
-  if (dz_dilated) {
-    YB_REQUIRE(d->stride == 2, "wgrad: dz_dilated only applies to stride-2 layers");
-    rc = make_tmap_im2col_px(&tmA, dz, d->dtype, d->n, d->h, d->w, d->cout, dz_ld, 1, 2, 0, 64, WG_BKP);
-  } else {
-    rc = make_tmap_2d(&tmA, dz, d->dtype, p.P, d->cout, dz_ld, WG_BKP, 64, 0);
-  }
+  YB_REQUIRE(d, "wgrad: null pointer");
+  WgradLaunch l;
+  int rc = wgrad_prepare(d, x, dz, dz_ld, dz_dilated, dw, &l);
   if (rc) return rc;
-  rc = make_tmap_im2col_px(&tmB, x, d->dtype, d->n, d->h, d->w, d->cin, d->in_ld, d->ksize, d->stride, p.pad,
-                           bnw < 64 ? bnw : 64, WG_BKP);
-  if (rc) return rc;
-  dim3 grid((unsigned)s.grid_x, (unsigned)s.grid_y, (unsigned)s.grid_z);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define YB_WG(T)                                                                       \
-  if (bnw == 128) return launch_wgrad<T, 128, 1>(tmA, tmB, p, grid, st);              \
-  if (bnw == 64) return tp == 3 ? launch_wgrad<T, 64, 3>(tmA, tmB, p, grid, st)       \
-                                : launch_wgrad<T, 64, 1>(tmA, tmB, p, grid, st);     \
-  return tp == 3 ? launch_wgrad<T, 32, 3>(tmA, tmB, p, grid, st) : launch_wgrad<T, 32, 1>(tmA, tmB, p, grid, st);
-  if (d->dtype == YB_F16) { YB_WG(__half) }
-  YB_WG(__nv_bfloat16)
-#undef YB_WG
+  return wgrad_launch(l, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int yb_stem_conv_wgrad_tc(const float* x, const void* dz, int dtype, int n, int h, int w, float* dw,

@@ -174,7 +174,7 @@ static void apply_fp8_scales(yb_net* net) {
     const float so = net->buf_scale[L.out.buf];
     L.fwd.p.res_scale = L.res.buf >= 0 ? net->buf_scale[L.res.buf] : 1.f;
     L.fwd.p.out_inv_scale = 1.f / so;
-    L.halo_params.out_inv_scale = 1.f / so;
+    L.halo.p.out_inv_scale = 1.f / so;
   }
 }
 
@@ -198,6 +198,14 @@ yb_conv_desc layer_desc(const yb_net* net, const Layer& L) {
 }
 // the multicast-cluster rule of conv_select applies to the 16-bit inference plans (not training, not e4m3)
 static bool plan_mcast_rule(const yb_net* net) { return !net->training && net->dtype != YB_E4M3; }
+// The halo-tile request of layer i's inference forward: Conv_3 of the fp8 plan reads fp16 and writes e4m3
+static HaloRequest layer_halo_request(const yb_net* net, int i) {
+  const Layer& L = net->layers[i];
+  HaloRequest r{layer_desc(net, L)};
+  r.res = L.res.buf >= 0;
+  r.out_e4m3 = net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1;
+  return r;
+}
 
 // What the forward launches for layer i.  It reads the options at every call: they may change between forwards of
 // one bound plan.  Layer 0 is FusedStem when layer 1's launch computes it; it then has no launch of its own.
@@ -273,7 +281,12 @@ extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count,
   const Layer& L = net->layers[layer];
   const yb_conv_desc d = layer_desc(net, L);
   info->residual = L.res.buf >= 0 ? 1 : 0;
-  if (k == LayerKernel::Halo) info->res_smem = info->residual && conv_halo_res_smem(&d);
+  if (k == LayerKernel::Halo) {
+    HaloParams hp;
+    int rc = halo_select(layer_halo_request(net, layer), &hp);
+    if (rc) return rc;
+    info->res_smem = hp.res_smem;
+  }
   if (k != LayerKernel::Igemm) return YB_OK;           // the thin, halo and fused-stem kernels
   ConvRequest r{d};
   r.res = info->residual;
@@ -319,33 +332,23 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
   for (size_t i = 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
     yb_conv_desc d = layer_desc(net, L);
-    if (net->dtype == YB_E4M3 && i == FP8_FIRST_LAYER - 1) {
-      // Conv_3 of the fp8 plan: fp16 in, e4m3 out, only the halo kernel has that form
-      YB_REQUIRE(conv_halo_supported(&d), "bind: the e4m3 plan needs the halo kernel for layer %d (w %% 16 == 0)", (int)i);
-      L.halo_desc = d;
-      int rc = conv_halo_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, reinterpret_cast<const float*>(net->par + L.scale),
-                                 reinterpret_cast<const float*>(net->par + L.shift), ten_ptr(net, L.res), ten_ptr(net, L.out),
-                                 &L.halo_maps, &L.halo_params);
-      if (rc) return rc;
-      L.halo_params.out_e4m3 = 1;
-      continue;
-    }
     const void* res = L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr;
     const float* scale = reinterpret_cast<const float*>(net->par + L.scale);
     const float* shift = reinterpret_cast<const float*>(net->par + L.shift);
+    // every layer layer_kernel may give the halo kernel; Conv_3 of the fp8 plan (fp16 in, e4m3 out) runs nothing else
+    const HaloRequest hr = layer_halo_request(net, (int)i);
+    if (hr.out_e4m3 || conv_halo_supported(&d)) {
+      int rc = conv_halo_prepare(hr, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out),
+                                 nullptr, nullptr, nullptr, &L.halo);
+      if (rc) return rc;
+      if (hr.out_e4m3) continue;
+    }
     ConvRequest r{d};
     r.res = res != nullptr;
     r.plan_rule = plan_mcast_rule(net);
     int rc = conv_prepare(r, ten_ptr(net, L.in), net->par + L.w_packed, scale, shift, res, ten_ptr(net, L.out), nullptr,
                           nullptr, &L.fwd);
     if (rc) return rc;
-    if (conv_halo_supported(&d)) {   // every layer layer_kernel may give the halo kernel
-      L.halo_desc = d;
-      rc = conv_halo_prepare(&d, ten_ptr(net, L.in), net->par + L.w_packed, reinterpret_cast<const float*>(net->par + L.scale),
-                             reinterpret_cast<const float*>(net->par + L.shift),
-                             L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), &L.halo_maps, &L.halo_params);
-      if (rc) return rc;
-    }
     if (!L.info.has_bn) {
       // fused-decode variant of the head (yb_net_detect); class counts without a kernel keep the unfused pipeline
       ConvRequest rd{d};
@@ -475,17 +478,19 @@ static int forward_layers_impl(yb_net* net, const float* images, float* fm1, flo
                                  reinterpret_cast<const float*>(net->par + L.shift),
                                  L.res.buf >= 0 ? ten_ptr(net, L.res) : nullptr, ten_ptr(net, L.out), stream);
       } else if (k == LayerKernel::FusedStem && i == 1) {
+        // per forward: the image is an argument of the forward
         Layer& L0 = net->layers[0];
-        HaloMaps hm;
-        HaloParams hp;
-        rc = conv_stem_halo_prepare(&L.halo_desc, images, reinterpret_cast<const float*>(net->par + L0.w_master),
-                                    reinterpret_cast<const float*>(net->par + L0.scale),
-                                    reinterpret_cast<const float*>(net->par + L0.shift), net->par + L.w_packed,
-                                    reinterpret_cast<const float*>(net->par + L.scale),
-                                    reinterpret_cast<const float*>(net->par + L.shift), ten_ptr(net, L.out), &hm, &hp);
-        if (rc == YB_OK) rc = conv_stem_halo_launch(&L.halo_desc, hm, hp, st);
+        HaloRequest r{layer_desc(net, L)};
+        r.stem = true;
+        HaloLaunch hl;
+        rc = conv_halo_prepare(r, images, net->par + L.w_packed, reinterpret_cast<const float*>(net->par + L.scale),
+                               reinterpret_cast<const float*>(net->par + L.shift), nullptr, ten_ptr(net, L.out),
+                               reinterpret_cast<const float*>(net->par + L0.w_master),
+                               reinterpret_cast<const float*>(net->par + L0.scale),
+                               reinterpret_cast<const float*>(net->par + L0.shift), &hl);
+        if (rc == YB_OK) rc = conv_halo_launch(hl, st);
       } else if (k == LayerKernel::Halo) {
-        rc = conv_halo_launch(&L.halo_desc, L.halo_maps, L.halo_params, st);
+        rc = conv_halo_launch(L.halo, st);
       }
       if (rc) return rc;
       continue;

@@ -31,10 +31,8 @@ struct Layer {
   size_t w_master = 0, w_packed = 0, gamma = 0, beta = 0, mean = 0, var = 0, bias = 0, scale = 0, shift = 0, w_scale = 0;
   // prepared implicit-GEMM launch of the inference forward
   ConvLaunch fwd;
-  // Cin <= 64 3x3 layers: halo-tile kernel (csrc/conv_halo.cu), inference forward only
-  HaloMaps halo_maps;
-  HaloParams halo_params;
-  yb_conv_desc halo_desc;
+  // Cin <= 64 3x3 layers: prepared halo-tile launch (csrc/conv_halo.cu), inference forward only
+  HaloLaunch halo;
   // detection heads: the same conv with the decode + NMS candidate filter fused into its epilogue (yb_net_detect)
   ConvLaunch det;
   bool det_ok = false;
@@ -50,6 +48,7 @@ struct Layer {
   // dgrad: the forward kernel on dz with flipped/transposed weights; stride-2 parity layers: one launch per class
   ConvLaunch dgrad[4];
   int num_dgrad = 0;                 // 1 | 4
+  WgradLaunch wgrad;                 // weight gradient (layers >= 1; the stem's reads the step's image)
 };
 
 // the activation view t (16-bit training buffers and inference buffers of any element size)

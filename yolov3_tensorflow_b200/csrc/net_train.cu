@@ -169,15 +169,18 @@ int train_bind(yb_net* net, cudaStream_t st) {
     if (L.dz_dilated)
       YB_CUDA(cudaMemsetAsync(net->act + L.dz_off, 0, (size_t)net->n * L.info.in_h * L.info.in_w * L.dz_ld * 2, st));
   }
-  // ---- training-mode forward convs: raw z + statistics ----
+  // ---- training-mode forward convs: raw z + statistics; weight gradients ----
   for (size_t i = 1; i < net->layers.size(); ++i) {
     Layer& L = net->layers[i];
+    const yb_conv_desc d = layer_desc(net, L);
+    int rc = wgrad_prepare(&d, ten_ptr(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), &L.wgrad);
+    if (rc) return rc;
     if (!L.info.has_bn) { L.train = L.fwd; continue; }   // detection convs run as in inference
-    ConvRequest r{layer_desc(net, L)};   // raw z [rows, cout]: no activation, residual or upsampling
+    ConvRequest r{d};   // raw z [rows, cout]: no activation, residual or upsampling
     r.d.out_ld = L.info.cout; r.d.res_ld = 0; r.d.leaky = 0; r.d.upsample2x = 0;
     r.stats = true;
-    int rc = conv_prepare(r, ten_ptr(net, L.in), net->par + L.w_packed, ones, zeros, nullptr, net->act + L.z_off,
-                          fact(net, L.st_sum), fact(net, L.st_sqsum), &L.train);
+    rc = conv_prepare(r, ten_ptr(net, L.in), net->par + L.w_packed, ones, zeros, nullptr, net->act + L.z_off,
+                      fact(net, L.st_sum), fact(net, L.st_sqsum), &L.train);
     if (rc) return rc;
   }
   // ---- dgrad convs + residual bookkeeping (reverse order) ----
@@ -441,8 +444,7 @@ static int train_bwd_layer(yb_net* net, int i, int phase, const float* images, i
     wstream = net->side_stream;
     net->side_forked = true;
   }
-  const yb_conv_desc d = layer_desc(net, L);
-  rc = yb_conv2d_wgrad(&d, ten_ptr(net, L.in), net->act + L.dz_off, L.dz_ld, L.dz_dilated, gradp(net, L.g_w), wstream);
+  rc = wgrad_launch(L.wgrad, static_cast<cudaStream_t>(wstream));
   if (rc) return rc;
   for (int c = 0; c < L.num_dgrad; ++c) {
     rc = conv_launch(L.dgrad[c], st);
