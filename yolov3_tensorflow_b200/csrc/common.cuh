@@ -185,6 +185,12 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                "r"(smem_u32(src)), "r"(c0), "r"(c1)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() {   // at most N most-recent groups still READING shared memory

@@ -86,7 +86,9 @@ inline size_t dgrad_s2_class_offset(int c, int cin_pad, int k_cout) {
 int conv_prepare_dgrad_s2(const yb_conv_desc* fwd, const void* dz, int dz_ld, int k_cout, const void* w_dgrad_s2,
                           const void* res, int res_ld, void* dx, int dx_ld, ConvLaunch* l);
 // halo-tile conv for the Cin <= 64 3x3 layers (csrc/conv_halo.cu)
-struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; CUtensorMap res; };
+// out: the 16-bit output as {C, W, H, N} = [n, ho, wo, out_ld], one {64, 8, 2, 1} box per consumer warp and 64 channels
+// (the TMA-store epilogue; zeroed for an e4m3 output)
+struct HaloMaps { CUtensorMap plane[4]; CUtensorMap w; CUtensorMap in3d; CUtensorMap res; CUtensorMap out; };
 struct HaloParams {
   int n, ho, wo;               // output geometry
   int tiles_x, tiles_y, num_tiles;

@@ -16,7 +16,11 @@
 //     The 128B / 64B swizzle is a function of the shared-memory address bits, so a descriptor may start at any row of
 //     a TMA-written tile;
 //   * all 9 taps' weights [Cout][9 * Cin] stay resident in shared memory for the whole persistent CTA;
-//   * the epilogue is the staging-tile one of conv_igemm.cu, with pixel (not row) addressing.
+//   * 16-bit outputs: the TMA-store epilogue of conv_igemm.cu (epi_box_to_slab): each consumer warp applies scale /
+//     shift, leaky and the residual to its fragments in registers, writes them by stmatrix into a swizzled slab and
+//     stores its 2 output rows x 8 pixels x 64 channels with one 4D TMA store, without a warpgroup barrier.  The
+//     e4m3 output and a residual read from global memory (YB_CONV_RES=ldg) keep the staging-tile epilogue, with
+//     pixel (not row) addressing.
 // Warp roles: warp 0 TMA producer, warps 4..11 (warpgroups 1, 2) MMA + epilogue, fp32 accumulators in registers; the
 // producer keeps up to NST halo tiles in flight ahead of the MMAs.
 // Inference only (folded BN): scale/shift + leaky + optional residual, 16-bit NHWC in and out.  One instantiation
@@ -42,9 +46,33 @@ static constexpr int HT_H = 16, HT_W = 8;       // output tile
 static constexpr int HALO_THREADS = 384;         // warp 0: TMA, warpgroups 1, 2: MMA + epilogue
 static constexpr int HALO_EPI_LD = 33;          // staging row pitch in floats
 
+// Fused stem (darknet53_body/Conv, 3 -> 32, 3x3/1, utils/layer_utils.py:35) as the PRODUCER of Conv_1's parity planes:
+// the 709 MB stem output of a batch-64 step is never written nor re-read.  Per 16x8-pixel tile of Conv_1 the stem is
+// needed on 33 x 17 pixels; their 35 x 19-pixel float32 input halo arrives by one 3D TMA load, STEMW producer warps
+// compute the stem on mma.sync (m16n8k16: A = the 27 -> 32 patch values gathered straight from the halo, B = the stem
+// weights held in registers), apply BN + leaky and store the 16-bit results into the swizzled plane tiles the
+// wgmma descriptors of Conv_1 read.  Stem pixels outside the image are Conv_1's zero padding (utils/layer_utils.py:15-16).
+struct StemCfg {
+  static constexpr int SH = 2 * HT_H + 1, SW = 2 * HT_W + 1;             // stem pixels per tile: 33 x 17
+  static constexpr int NPX = SH * SW;                                     // 561
+  static constexpr int NT16 = (NPX + 15) / 16;                            // 36 m16 tiles
+  static constexpr int IN_ROWS = SH + 2;                                  // 35 image rows
+  static constexpr int IN_ROWF = 60;                                      // floats per halo row: 19 px x 3 = 57, padded to 16 bytes
+  static constexpr int IN_BYTES = (IN_ROWS * IN_ROWF * 4 + 127) / 128 * 128;
+  // The planes are written by producer warps of the same CTA, so two stages (one being filled, one being read) keep
+  // the consumers fed; the image halo is the layer's only HBM load, so the rest of shared memory goes to its ring.
+  // (Measured: 4 plane stages with 3 image stages time the same within 1.5 %; DESIGN.md §5.)
+  static constexpr int NST = 2;                                           // plane stages
+  static constexpr int NIN_MAX = 8;                                       // image-halo stages
+};
+
 // RES (Conv_3: 32 -> 64, stride 1, with a shortcut): every stage also holds the tile's residual, a [16][8] x 64-channel
 // box of 128B-swizzled pixel rows loaded by TMA with the halo, so the epilogue adds it from shared memory.
-template <int CIN, int COUT, int STRIDE, bool RES = false>
+// TMA: the 16-bit outputs' TMA-store epilogue.  Its per-warp output slabs (8 x 2 KB) alias the staging tile, which a
+// launch with a global-read residual still uses; with RES the slabs are the stage's residual box itself, and only the
+// e4m3 output keeps a staging tile of its own.
+// STEMW > 0: the fused stem's plane ring (StemCfg::NST) and image-halo ring (NIN) share the space left by the weights.
+template <int CIN, int COUT, int STRIDE, bool RES = false, bool TMA = false, int STEMW = 0>
 struct HaloCfg {
   static constexpr int ROWB = CIN * 2;                                   // bytes per pixel row of a plane (one swizzle span)
   static constexpr int NPLANE = STRIDE == 1 ? 1 : 4;
@@ -61,35 +89,25 @@ struct HaloCfg {
                                   RES_BYTES;
   static constexpr int B_TAP_BYTES = COUT * ROWB;                        // one tap's [COUT][CIN] weight tile
   static constexpr int B_BYTES = 9 * B_TAP_BYTES;
-  static constexpr int EPI_BYTES = 2 * 64 * HALO_EPI_LD * 4;              // a [64][33] fp32 staging tile per consumer warpgroup
+  // a [64][33] fp32 staging tile per consumer warpgroup, or (TMA) a 16-row x 128-byte output slab per consumer warp
+  static constexpr int EPI_BYTES = (TMA && RES) ? 0 : ((TMA && STEMW > 0) ? 8 * 2048 : 2 * 64 * HALO_EPI_LD * 4);
   static constexpr int MISC_BYTES = 1024;                                // barriers
+  static constexpr int SS_BYTES = 4 * COUT * 4;                          // scale / shift, per column and per column pair
   static constexpr int BUDGET = 227 * 1024 - 1024 /*alignment slack*/;
-  static constexpr int NST_RAW = (BUDGET - B_BYTES - EPI_BYTES - MISC_BYTES - 2 * COUT * 4) / STAGE_BYTES;
-  static constexpr int NST = NST_RAW > 6 ? 6 : NST_RAW;
-  static_assert(NST >= 1, "halo conv: configuration does not fit shared memory");
-  static constexpr int SMEM_BYTES = 1024 + B_BYTES + NST * STAGE_BYTES + EPI_BYTES + MISC_BYTES + 2 * COUT * 4;
+  static constexpr int FIXED = B_BYTES + EPI_BYTES + MISC_BYTES + SS_BYTES;
+  static constexpr int NST_RAW = (BUDGET - FIXED) / STAGE_BYTES;
+  static constexpr int NST = STEMW > 0 ? StemCfg::NST : (NST_RAW > 6 ? 6 : NST_RAW);
+  static_assert(NST >= 1 && NST <= 8, "halo conv: configuration does not fit shared memory");
+  static constexpr int NIN_RAW = STEMW > 0 ? (BUDGET - FIXED - NST * STAGE_BYTES) / StemCfg::IN_BYTES : 0;
+  static constexpr int NIN = NIN_RAW > StemCfg::NIN_MAX ? StemCfg::NIN_MAX : NIN_RAW;   // image-halo stages (STEMW > 0)
+  static_assert(STEMW == 0 || NIN >= 2, "halo conv: the fused stem's image ring does not fit shared memory");
+  static constexpr int SMEM_BYTES = 1024 + FIXED + NST * STAGE_BYTES + NIN * StemCfg::IN_BYTES;
   static constexpr uint32_t SWIZZLE = ROWB;                              // 128B / 64B: a pixel row is one swizzle span
   // tap (r, s) -> plane and row/col offset inside it.  stride 2 (pad 1 + VALID): input row 2i + r - 1:
   //   r = 0 -> odd-row plane, offset 0; r = 1 -> even-row plane, offset 0; r = 2 -> odd-row plane, offset 1
   static constexpr int tap_plane(int r, int s) { return STRIDE == 1 ? 0 : (((r == 1) ? 2 : 0) | ((s == 1) ? 1 : 0)); }
   static constexpr int tap_dr(int r) { return STRIDE == 1 ? r : (r == 2 ? 1 : 0); }
   static constexpr int tap_ds(int s) { return STRIDE == 1 ? s : (s == 2 ? 1 : 0); }
-};
-
-// Fused stem (darknet53_body/Conv, 3 -> 32, 3x3/1, utils/layer_utils.py:35) as the PRODUCER of Conv_1's parity planes:
-// the 709 MB stem output of a batch-64 step is never written nor re-read.  Per 16x8-pixel tile of Conv_1 the stem is
-// needed on 33 x 17 pixels; their 35 x 19-pixel float32 input halo arrives by one 3D TMA load, STEMW producer warps
-// compute the stem on mma.sync (m16n8k16: A = the 27 -> 32 patch values gathered straight from the halo, B = the stem
-// weights held in registers), apply BN + leaky and store the 16-bit results into the swizzled plane tiles the
-// wgmma descriptors of Conv_1 read.  Stem pixels outside the image are Conv_1's zero padding (utils/layer_utils.py:15-16).
-struct StemCfg {
-  static constexpr int SH = 2 * HT_H + 1, SW = 2 * HT_W + 1;             // stem pixels per tile: 33 x 17
-  static constexpr int NPX = SH * SW;                                     // 561
-  static constexpr int NT16 = (NPX + 15) / 16;                            // 36 m16 tiles
-  static constexpr int IN_ROWS = SH + 2;                                  // 35 image rows
-  static constexpr int IN_ROWF = 60;                                      // floats per halo row: 19 px x 3 = 57, padded to 16 bytes
-  static constexpr int IN_BYTES = (IN_ROWS * IN_ROWF * 4 + 127) / 128 * 128;
-  static constexpr int NIN = 2;                                           // input halo stages
 };
 
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
@@ -117,23 +135,27 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
 template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T, bool RES = false>
 __global__ void __launch_bounds__(HALO_THREADS + 32 * STEMW, 1)
 conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ HaloParams p) {
-  using C = HaloCfg<CIN, COUT, STRIDE, RES>;
+  constexpr bool kTMA = !std::is_same<TO, __nv_fp8_e4m3>::value;   // 16-bit output: the TMA-store epilogue
+  using C = HaloCfg<CIN, COUT, STRIDE, RES, kTMA, STEMW>;
   static_assert(!RES || (CIN == 32 && COUT == 64 && STRIDE == 1 && STEMW == 0), "the residual box is Conv_3's");
   constexpr int PROD_WARP0 = HALO_THREADS / 32;  // first stem-producer warp
   static_assert(STEMW == 0 || (CIN == 32 && STRIDE == 2), "the fused stem feeds Conv_1 (32 -> 64, stride 2)");
+  static_assert(STEMW == 0 || kTMA, "the fused stem's Conv_1 has a 16-bit output");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // pointer arithmetic: stays in the shared space
   uint8_t* sB = smem;                                        // [9][COUT][CIN]   swizzled, resident
   uint8_t* sA = smem + C::B_BYTES;                           // [NST][planes]    swizzled halo tiles
-  float* sE = reinterpret_cast<float*>(sA + C::NST * C::STAGE_BYTES);   // [2 warpgroups][64][HALO_EPI_LD] staging
+  // [2 warpgroups][64][HALO_EPI_LD] staging, or (TMA, not RES) [8 consumer warps][16][128 B] output slabs (1024-byte aligned)
+  float* sE = reinterpret_cast<float*>(sA + C::NST * C::STAGE_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sE) + C::EPI_BYTES);
   uint64_t* full_bar = bars;            // [NST]
   uint64_t* empty_bar = bars + 8;       // [NST] one arrive per consumer warp
   uint64_t* b_bar = bars + 20;
+  uint64_t* in_full = bars + 32;        // [NIN] float32 input halo landed (TMA -> stem producers)
+  uint64_t* in_empty = bars + 48;       // [NIN] stem producers -> TMA
   float* s_ss = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sE) + C::EPI_BYTES + C::MISC_BYTES);   // [2][COUT] scale / shift
-  uint64_t* in_full = bars + 24;        // [NIN] float32 input halo landed (TMA -> stem producers)
-  uint64_t* in_empty = bars + 26;       // [NIN] stem producers -> TMA
-  uint8_t* sIn = reinterpret_cast<uint8_t*>(s_ss + 2 * COUT);                  // [NIN][35][60] float32 (STEMW > 0 only; 128-byte aligned)
+  float* s_ss4 = s_ss + 2 * COUT;       // [COUT / 2] (scale, scale, shift, shift) per column pair: the TMA epilogue's
+  uint8_t* sIn = reinterpret_cast<uint8_t*>(s_ss + 4 * COUT);                  // [NIN][35][60] float32 (STEMW > 0 only; 128-byte aligned)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -144,17 +166,21 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
     }
     tma_prefetch_desc(&maps.w);
     if (RES) tma_prefetch_desc(&maps.res);
+    if (kTMA) tma_prefetch_desc(&maps.out);
     for (int i = 0; i < C::NST; ++i) { mbar_init(&full_bar[i], STEMW > 0 ? STEMW : 1); mbar_init(&empty_bar[i], 8); }
     if (STEMW > 0) {
       tma_prefetch_desc(&maps.in3d);
-      for (int i = 0; i < StemCfg::NIN; ++i) { mbar_init(&in_full[i], 1); mbar_init(&in_empty[i], STEMW); }
+      for (int i = 0; i < C::NIN; ++i) { mbar_init(&in_full[i], 1); mbar_init(&in_empty[i], STEMW); }
     }
     mbar_init(b_bar, 1);
     fence_barrier_init();
   }
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
-    s_ss[c] = c < p.cout ? __ldg(p.scale + c) : 0.f;
-    s_ss[COUT + c] = c < p.cout ? __ldg(p.shift + c) : 0.f;
+    const float sc = c < p.cout ? __ldg(p.scale + c) : 0.f, sh = c < p.cout ? __ldg(p.shift + c) : 0.f;
+    s_ss[c] = sc;
+    s_ss[COUT + c] = sh;
+    s_ss4[(c >> 1) * 4 + (c & 1)] = sc;
+    s_ss4[(c >> 1) * 4 + 2 + (c & 1)] = sh;
   }
   __syncthreads();
 
@@ -178,7 +204,7 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
           // (the innermost TMA coordinate must be 16-byte aligned — an unaligned start is an illegal instruction; the halo's
           //  first float (2 tx 8 - 2) * 3 is always 2 mod 4, so the box starts 2 floats earlier: 2 + 57 <= 60 floats per row)
           tma_load_3d(sIn + stage * StemCfg::IN_BYTES, &maps.in3d, &in_full[stage], (2 * tx * HT_W - 2) * 3 - 2, 2 * ty * HT_H - 2, img);
-          if (++stage == StemCfg::NIN) { stage = 0; phase ^= 1; }
+          if (++stage == C::NIN) { stage = 0; phase ^= 1; }
         }
       }
       for (int tile = blockIdx.x; STEMW == 0 && tile < p.num_tiles; tile += gridDim.x) {
@@ -212,6 +238,7 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
     float* stg = sE + cw * 64 * HALO_EPI_LD;
     const bool has_res = STEMW == 0 && p.res != nullptr;      // (Conv_1 has no shortcut: the residual code is compiled out of the fused kernel)
     const int er = t >> 1, eh = t & 1;                         // epilogue: this thread's pixel of the chunk and its 16-channel half
+    const float slope = p.leaky ? 0.1f : 1.f;                  // TMA epilogue: fmaxf(v, 1 v) == v
     const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
     float acc[COUT / 2];
     mbar_wait(b_bar, 0);
@@ -251,6 +278,30 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       const int tx = tile % p.tiles_x;
       const int ty = (tile / p.tiles_x) % p.tiles_y;
       const int img = tile / (p.tiles_x * p.tiles_y);
+      if constexpr (kTMA) {
+        if (RES || !has_res) {
+          // TMA-store epilogue (epi_box_to_slab): warp wq of the warpgroup owns accumulator rows 16 wq .. 16 wq + 15,
+          // which are output rows 8 cw + 2 wq and + 1 of the tile, so each 64 channels of them are one {64, 8, 2, 1}
+          // box of maps.out (rows at or past ho are clipped by the TMA).  No warpgroup barrier: each warp works alone.
+          const int wq = (warp - 4) & 3, oh0 = ty * HT_H + 8 * cw + 2 * wq;
+          uint8_t* slab = RES ? sA + rel_stage * C::STAGE_BYTES + C::RES_OFF + (64 * cw + 16 * wq) * 128
+                              : reinterpret_cast<uint8_t*>(sE) + (warp - 4) * 2048;
+#pragma unroll
+          for (int b = 0; b < COUT / 64; ++b) {
+            epi_box_to_slab<T, COUT, RES>(acc, b, reinterpret_cast<const float4*>(s_ss4), slab, slope, lane);
+            if (lane == 0 && oh0 < p.ho) {
+              tma_store_4d(&maps.out, slab, 64 * b, tx * HT_W, oh0, img);
+              bulk_commit_group();
+            }
+          }
+          if (RES && lane == 0) {                // the store has read the residual box: the stage may be refilled
+            bulk_wait_group_read<0>();
+            mbar_arrive(&empty_bar[rel_stage]);
+          }
+          continue;
+        }
+      }
+      // staged epilogue: the e4m3 output, and a residual read from global memory (YB_CONV_RES=ldg)
       const int oh = ty * HT_H + 8 * cw + (er >> 3), ow = tx * HT_W + (er & 7);
       const bool ok = oh < p.ho && ow < p.wo;
       const long off = ((long)img * p.ho + oh) * p.wo + ow;
@@ -303,6 +354,9 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[rel_stage]);
       }
+    }
+    if constexpr (kTMA) {
+      if (lane == 0) bulk_wait_group<0>();       // this warp's output stores are complete before the CTA may exit
     }
   } else if (STEMW > 0 && warp >= PROD_WARP0) {
     // ===================== stem producers (warps PROD_WARP0 .. PROD_WARP0 + STEMW - 1) =====================
@@ -418,8 +472,8 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
       };
       // The 561 stem pixels are walked PLANE BY PLANE in m16 tiles (10 + 9 + 9 + 8 = 36): a tile lies inside one plane, so
       // the plane's constants are warp-uniform and consecutive fragment rows are consecutive 64-byte rows of the plane tile.
-      // The producers are latency-bound, not issue-bound: 12 warps beat 8 (408 vs 465 us); keeping TWO tiles in flight per
-      // warp lost to the register pressure (498 / 538 us) and was dropped.
+      // The producers are latency-bound, not issue-bound: 12 warps (3 m16 tiles each) beat 8 (4 or 5 tiles) and 9 (4
+      // tiles); keeping TWO tiles in flight per warp lost to the register pressure and was dropped (DESIGN.md §5).
 #pragma unroll 1
       for (int t = pw_id; t < StemCfg::NT16; t += STEMW) {
         M16 m0;
@@ -433,20 +487,20 @@ conv_halo_kernel(const __grid_constant__ HaloMaps maps, const __grid_constant__ 
         mbar_arrive(&full_bar[stage]);
         mbar_arrive(&in_empty[in_stage]);
       }
-      if (++in_stage == StemCfg::NIN) { in_stage = 0; in_phase ^= 1; }
+      if (++in_stage == C::NIN) { in_stage = 0; in_phase ^= 1; }
       if (++stage == C::NST) { stage = 0; phase ^= 1; }
     }
   }
 }
 
-static constexpr int STEM_WARPS = 8;           // stem producer warps of the fused kernel (640 threads per CTA)
+static constexpr int STEM_WARPS = 12;          // stem producer warps of the fused kernel (768 threads per CTA)
 
 // One conv_halo_kernel instantiation: the type halo_kernel_for passes to its functor
 template <typename T, int CIN, int COUT, int STRIDE, int STEMW = 0, typename TO = T, bool RES = false>
 struct HaloKernel {
   static constexpr int THREADS = HALO_THREADS + 32 * STEMW;
   static constexpr int SMEM_BYTES =
-      HaloCfg<CIN, COUT, STRIDE, RES>::SMEM_BYTES + (STEMW > 0 ? StemCfg::NIN * StemCfg::IN_BYTES : 0);
+      HaloCfg<CIN, COUT, STRIDE, RES, !std::is_same<TO, __nv_fp8_e4m3>::value, STEMW>::SMEM_BYTES;
   static_assert(SMEM_BYTES <= 227 * 1024, "halo conv: configuration does not fit shared memory");
   static constexpr auto kernel = conv_halo_kernel<T, CIN, COUT, STRIDE, STEMW, TO, RES>;
 };
@@ -567,6 +621,11 @@ int conv_halo_prepare(const HaloRequest& r, const void* x, const void* w_packed,
   if (p->res_smem) {
     // the residual as {C, W, H, N} = [n, ho, wo, res_ld]: one 64-channel x 8 x 16-pixel box per tile
     rc = make_tmap_tiled4d(&maps->res, res, d->dtype, d->n, p->ho, p->wo, d->cout, d->res_ld, 64, HT_W, HT_H, 1);
+    if (rc) return rc;
+  }
+  if (!p->out_e4m3) {
+    // the output as {C, W, H, N}: a consumer warp's 16 accumulator rows are 2 output rows of 8 pixels
+    rc = make_tmap_tiled4d(&maps->out, out, d->dtype, d->n, p->ho, p->wo, d->cout, d->out_ld, 64, HT_W, 2, 1);
     if (rc) return rc;
   }
   if (r.stem) {

@@ -346,8 +346,8 @@ __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float
 // warp owns 16 rows of a 64-row accumulator block, so it works alone, without a warpgroup barrier: per 64-column box it
 // applies scale / shift (+leaky) (+residual) to its fragments in registers — the operations of epi_store16 in the
 // same order, so the outputs are the same bit for bit — packs them to 16 bits, writes them with four stmatrix.x4 into
-// a 16-row x 64-column slab of 128-byte rows in the TMA's 128B swizzle (conflict-free), and lane 0 stores the slab
-// through p.tmO, which clips rows >= M and columns >= cout.
+// a 16-row x 64-column slab of 128-byte rows in the TMA's 128B swizzle (conflict-free; epi_box_to_slab, wgmma.cuh),
+// and lane 0 stores the slab through p.tmO, which clips rows >= M and columns >= cout.
 //   ss4[4 j + q]: (scale, scale, shift, shift) of columns 8 j + 2 q and + 1 of the tile.
 //   Without RES the warp has one slab (slab_h = slab_b = 0) and waits until the previous store has read it; such a
 //   launch has no residual (conv_select: a residual that is not prefetched keeps the staged epilogue).
@@ -358,49 +358,13 @@ template <typename T, int BN, int NH, bool RES>
 __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const float (&acc)[NH][BN / 2], const int row0,
                                              const int n0, const float4* ss4, uint8_t* slab, const uint32_t slab_h,
                                              const uint32_t slab_b, const int lane) {
-  // lane = 8 i + r addresses row r + 8 (i & 1), 16-byte chunk (2 q + (i >> 1)) ^ r of the slab for the q-th stmatrix
-  const int r = lane & 7, mi = lane >> 3;
-  const uint32_t lane_off = (uint32_t)((r + 8 * (mi & 1)) * 128 + (((mi >> 1) ^ r) << 4));
   const float slope = p.leaky ? 0.1f : 1.f;                    // fmaxf(v, 1 v) == v
 #pragma unroll
   for (int h = 0; h < NH; ++h) {
 #pragma unroll
     for (int b = 0; b < BN / 64; ++b) {
       uint8_t* s = slab + h * slab_h + b * slab_b;
-      const uint32_t sa = smem_u32(s) + lane_off;              // the slab is 1024-byte aligned: ^ (q << 5) moves 2 q chunks
-      uint32_t pk[16];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {                            // stmatrix q: 8-column blocks 2 q and 2 q + 1 of the box
-        if constexpr (RES) ldmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-#pragma unroll
-        for (int ih = 0; ih < 2; ++ih) {
-          const int j = 8 * b + 2 * q + ih;                    // 8-column block of the tile
-          const float4 c = ss4[4 * j + (lane & 3)];
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {                     // rows lane >> 2 and + 8
-            float v0 = fmaf(acc[h][4 * j + 2 * hh], c.x, c.z);
-            float v1 = fmaf(acc[h][4 * j + 2 * hh + 1], c.y, c.w);
-            v0 = fmaxf(v0, slope * v0);
-            v1 = fmaxf(v1, slope * v1);
-            uint32_t& w = pk[4 * q + 2 * ih + hh];
-            if constexpr (RES) {
-              const float2 f = Pack2<T>::unpack(w);
-              v0 += f.x; v1 += f.y;
-            }
-            w = Pack2<T>::pack(v0, v1);
-          }
-        }
-        // RES: nothing else reads these rows of the shortcut tile, so each result goes straight back
-        if constexpr (RES) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-      }
-      if constexpr (!RES) {
-        if (lane == 0) bulk_wait_group_read<0>();              // the previous store has read the slab
-        __syncwarp();
-#pragma unroll
-        for (int q = 0; q < 4; ++q) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-      }
-      fence_proxy_async();                                     // the slab as written is what the TMA reads
-      __syncwarp();
+      epi_box_to_slab<T, BN, RES>(acc[h], b, ss4, s, slope, lane);
       if (lane == 0 && row0 + h * WG_ROWS < p.M && n0 + b * 64 < p.cout) {
         tma_store_2d(&p.tmO, s, n0 + b * 64, row0 + h * WG_ROWS);
         bulk_commit_group();

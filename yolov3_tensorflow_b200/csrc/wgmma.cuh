@@ -154,4 +154,56 @@ __device__ __forceinline__ void wgmma_stage_chunk(const float (&acc)[N / 2], con
   }
 }
 
+// One 64-column box of a warp's 16 accumulator rows -> a 16-row x 128-byte slab (1024-byte aligned) in the TMA's 128B
+// swizzle, for a TMA store (the TMA-store epilogues of conv_igemm.cu and conv_halo.cu).  The values never leave the
+// accumulator layout: scale / shift, leaky (slope 0.1; 1 = none, fmaxf(v, v) == v), + residual, packed to 16 bits —
+// the staged epilogues' operations in their order, so the results are the same bit for bit — and written with four
+// conflict-free stmatrix.x4.  Needs common.cuh (stmatrix / ldmatrix, the bulk-group waits, Pack2).
+//   acc: the warp's accumulator row (wgmma layout above); box b: columns 64 b .. 64 b + 63 of it.
+//   ss4[4 j + q]: (scale, scale, shift, shift) of columns 8 j + 2 q and + 1.
+//   RES: the slab holds the residual rows already (ldmatrix.x4 reads them as fragments) and the result goes over them.
+//   Otherwise the slab is the warp's own: lane 0 waits until the warp's previous store has read it (after the
+//   arithmetic, so that the wait overlaps it).
+// Ends with the slab written and fenced for the async proxy; the caller issues the store.
+template <typename T, int N, bool RES>
+__device__ __forceinline__ void epi_box_to_slab(const float (&acc)[N / 2], const int b, const float4* ss4, uint8_t* slab,
+                                                const float slope, const int lane) {
+  // lane = 8 i + r addresses row r + 8 (i & 1), 16-byte chunk (2 q + (i >> 1)) ^ r of the slab for the q-th stmatrix
+  const int r = lane & 7, mi = lane >> 3;
+  const uint32_t sa = smem_u32(slab) + (uint32_t)((r + 8 * (mi & 1)) * 128 + (((mi >> 1) ^ r) << 4));
+  uint32_t pk[16];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {                            // stmatrix q: 8-column blocks 2 q and 2 q + 1 of the box
+    if constexpr (RES) ldmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+#pragma unroll
+    for (int ih = 0; ih < 2; ++ih) {
+      const int j = 8 * b + 2 * q + ih;                    // 8-column block of the accumulator row
+      const float4 c = ss4[4 * j + (lane & 3)];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {                     // rows lane >> 2 and + 8
+        float v0 = fmaf(acc[4 * j + 2 * hh], c.x, c.z);
+        float v1 = fmaf(acc[4 * j + 2 * hh + 1], c.y, c.w);
+        v0 = fmaxf(v0, slope * v0);
+        v1 = fmaxf(v1, slope * v1);
+        uint32_t& w = pk[4 * q + 2 * ih + hh];
+        if constexpr (RES) {
+          const float2 f = Pack2<T>::unpack(w);
+          v0 += f.x; v1 += f.y;
+        }
+        w = Pack2<T>::pack(v0, v1);
+      }
+    }
+    // RES: nothing else reads these rows of the residual, so each result goes straight back
+    if constexpr (RES) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+  }
+  if constexpr (!RES) {
+    if (lane == 0) bulk_wait_group_read<0>();              // the previous store has read the slab
+    __syncwarp();
+#pragma unroll
+    for (int q = 0; q < 4; ++q) stmatrix_x4(sa ^ (q << 5), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+  }
+  fence_proxy_async();                                     // the slab as written is what the TMA reads
+  __syncwarp();
+}
+
 }  // namespace yb
