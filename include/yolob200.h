@@ -575,6 +575,11 @@ int yb_net_train_reset_state(yb_net* net, int optimizer_kind, void* stream);
  * {non-finite flag of the running step, updates applied, steps skipped} (checkpoint save/restore of save_optimizer,
  * train.py:101-104,118-121). */
 int yb_net_opt_state(yb_net* net, float** slots, size_t* count_per_slot, int* num_slots, int** ctrl);
+/* Read-only view of the per-tensor squared norms the last yb_net_train_update computed and clipped with: float
+ * sqnorm[count], the fp32 sum over a tensor's elements of (grad_scale*grad + weight_decay*w)^2 (0 for a tensor excluded
+ * by yb_net_set_trainable).  count = 2 + 3 * 72 = 222: per layer in creation order, w, then gamma and beta (BN layers)
+ * or bias (detection convs). */
+int yb_net_opt_norms(yb_net* net, float** sqnorm, int* count);
 /* train.py:81 update_part: exclude a conv (weights + gamma/beta | bias) from / include it in the update. */
 int yb_net_set_trainable(yb_net* net, int layer, int trainable, void* stream);
 /* Re-derive the dgrad weight layouts from the fp32 master weights (after the arena's weights were replaced). */

@@ -153,6 +153,7 @@ _SIGS = {
     "yb_net_train_update": ([vp, C.POINTER(Optimizer), vp], i32),
     "yb_net_train_reset_state": ([vp, i32, vp], i32),
     "yb_net_opt_state": ([vp, C.POINTER(vp), C.POINTER(sz), C.POINTER(i32), C.POINTER(vp)], i32),
+    "yb_net_opt_norms": ([vp, C.POINTER(vp), C.POINTER(i32)], i32),
     "yb_net_set_trainable": ([vp, i32, i32, vp], i32),
     "yb_net_train_refresh_dgrad": ([vp, vp], i32),
     "yb_net_get_conv_params": ([vp, i32] + [C.POINTER(vp)] * 6, i32),

@@ -616,6 +616,13 @@ extern "C" int yb_net_opt_state(yb_net* net, float** slots, size_t* count_per_sl
   return YB_OK;
 }
 
+extern "C" int yb_net_opt_norms(yb_net* net, float** sqnorm, int* count) {
+  YB_REQUIRE(net && net->training && net->par && sqnorm && count, "opt_norms: not a bound training plan");
+  *sqnorm = fpar(net, net->opt_norm_off);
+  *count = net->num_opt_tensors;
+  return YB_OK;
+}
+
 // train.py:81 `update_part`: restrict the update to some convs (their weights, gamma/beta or bias)
 extern "C" int yb_net_set_trainable(yb_net* net, int layer, int trainable, void* stream) {
   YB_REQUIRE(net && net->training && net->par && layer >= 0 && layer < (int)net->layers.size(), "set_trainable: bad argument");

@@ -135,6 +135,12 @@ class _Plan:
         off = p.value - self.act.data_ptr()
         return self.act[off: off + n.value * 4].view(torch.float32)
 
+    def opt_norms(self):
+        """Per-tensor squared norms of the last update, float32 [222] view (include/yolob200.h: yb_net_opt_norms)."""
+        p, n = C.c_void_p(), C.c_int()
+        check(lib.yb_net_opt_norms(self.handle, C.byref(p), C.byref(n)), "yb_net_opt_norms")
+        return self._view(p.value, (n.value,))
+
     def grad_flat(self):
         p, n = C.c_void_p(), C.c_size_t()
         check(lib.yb_net_grad_buffer(self.handle, C.byref(p), C.byref(n)), "yb_net_grad_buffer")
