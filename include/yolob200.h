@@ -418,7 +418,7 @@ int yb_net_layer_info(const yb_net* net, int layer, yb_layer_info* info);
  * max_clusters = sm_count / (cluster_m * cluster_n); sm_count == 0: the current device, max_clusters from
  * cudaOccupancyMaxActiveClusters for the kernel.  igemm = 0: the layer runs another kernel, named by `kernel`; of the
  * other fields only residual and res_smem are then set.  The detection heads are reported as yb_net_forward runs them
- * (unfused).
+ * (unfused); det_block_n gives the tile width of their fused-decode launch in yb_net_detect.
  * kernel (every layer, layer 0 included):
  *   YB_LAYER_IGEMM       the implicit-GEMM conv (igemm = 1)
  *   YB_LAYER_HALO        the halo-tile kernel (Cin = 32 layers by default; YB_HALO=0: none, YB_HALO=1: wherever it applies)
@@ -442,6 +442,8 @@ typedef struct yb_layer_schedule_info {
                      /*    loop (YB_CONV_RES); 0: the epilogue reads it from global memory          */
   int kernel;        /* YB_LAYER_*: what the forward launches for this layer (above)                */
   int epi_tma;       /* 1: the TMA-store epilogue (YB_CONV_EPI); 0: the staged or register epilogue  */
+  int det_block_n;   /* detection heads: columns of the one n-tile of the fused-decode launch, the   */
+                     /*    narrowest of 64, 128, 256 that holds 3 (5 + C); 0: none (C > 80), or not a head */
 } yb_layer_schedule_info;
 int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count, yb_layer_schedule_info* info);
 int yb_net_arena_bytes(const yb_net* net, size_t* activation_bytes, size_t* param_bytes);
@@ -472,8 +474,8 @@ int yb_net_forward(yb_net* net, const float* images, float* fm1, float* fm2, flo
  *   anchors9x2 host float[18] (w,h pixels, small -> large);  boxes [n, B, 4] float32 out: every decoded box
  *   (xmin,ymin,xmax,ymax), B = 3*(h/32*w/32 + h/16*w/16 + h/8*w/8);  workspace >= yb_net_detect_workspace_bytes;
  *   out_* as yb_nms (fixed shape [n, class_num*max_boxes(,4)], out_counts [n]).
- * yb_net_detect_supported: 1 when a fused kernel exists for the plan's class count (80 and 20), else 0 — callers
- * then use the three separate calls. */
+ * yb_net_detect_supported: 1 when the plan is bound and its class count has fused heads (1 to 80 classes, every
+ * dtype), else 0 — callers then use the three separate calls. */
 int yb_net_detect_supported(const yb_net* net);
 int yb_net_detect_workspace_bytes(const yb_net* net, int max_boxes, size_t* bytes);
 int yb_net_detect(yb_net* net, const float* images, const float* anchors9x2, int max_boxes, float score_thresh,

@@ -48,7 +48,7 @@ class ConvSchedule(C.Structure):   # yb_conv_schedule_info
 class LayerSchedule(C.Structure):  # yb_layer_schedule_info
     _fields_ = [(n, i32) for n in ("igemm", "pingpong", "cluster_m", "cluster_n", "block_m", "block_n", "num_m_tiles",
                                    "num_n_tiles", "units", "max_clusters", "grid", "residual", "res_smem", "kernel",
-                                   "epi_tma")]
+                                   "epi_tma", "det_block_n")]
 
 
 class WgradSchedule(C.Structure):  # yb_wgrad_schedule_info

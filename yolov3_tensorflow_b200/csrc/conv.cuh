@@ -63,7 +63,8 @@ struct ConvRequest {
   bool stats = false;      // BN batch statistics of the raw result (stat_sum / stat_sqsum)
   bool res = false;        // adds a residual
   int det_e = 0;           // > 0: detection head with the decode fused into the epilogue, 5 + C = det_e columns per
-                           // anchor, d.cout = 3 * det_e; one n-tile spans the whole padded cout and `out` is never written
+                           // anchor, d.cout = 3 * det_e <= 256; one n-tile of 64, 128 or 256 columns holds all of them and
+                           // `out` is never written
   bool plan_rule = false;  // a forward layer of a 16-bit inference plan: the plan's multicast-cluster rule applies when
                            // YB_CONV_MCAST is unset, and the TMA-store epilogue when YB_CONV_EPI is
 };

@@ -264,12 +264,15 @@ __device__ __forceinline__ void epilogue_reg(const ConvParams& p, const float (&
 // per-(image, class) candidate lists of the NMS (csrc/nms.cu).  Same arithmetic as predict_kernel (decode.cuh), so
 // boxes and scores are bit-identical to the unfused path; the feature maps and the [n, B, C] score tensor never exist.
 // The columns arrive chunk by chunk through the staging tile; threads 0..63 of the warpgroup (warps 0 and 1) own one
-// row each and walk its columns with (anchor, element) carried as warp-uniform counters.
-template <int BN, int E>
+// row each and walk it anchor by anchor: the 5 box logits, then the C class logits, staging the next chunk when a column
+// leaves the staged one.  A warp without a candidate for an anchor stages past its class logits without reading them.
+// E = 5 + C is read at run time: one instantiation per tile width serves every class count whose 3 E columns fit it
+// (conv_select).
+template <int BN>
 __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float (&acc)[BN / 2], const int row0, const int t,
                                                 float* stg, const float* s_ss, const int bar_id) {
-  static_assert(3 * E <= BN, "all three anchors must lie in one n-tile");
   const DetParams& d = p.det;
+  const int E = d.E;
   const int lane = t & 31;
   const bool walker = t < WG_ROWS;                             // warp-uniform
   const int row = row0 + t;
@@ -281,63 +284,64 @@ __device__ __forceinline__ void epilogue_detect(const ConvParams& p, const float
   const unsigned lt = (1u << lane) - 1u;
   const float offx = (float)(cell % p.Q), offy = (float)(cell / p.Q);
   const int box0 = d.box_off + cell * 3;
-  constexpr int NCH = (3 * E + 31) / 32;
-  int a = 0, e = 0;
-  float h0 = 0.f, h1 = 0.f, h2 = 0.f, h3 = 0.f;               // the anchor's x, y, w, h logits
-  float cconf = 0.f;
-  bool cok = false, cany = false;
-#pragma unroll 1
-  for (int ch = 0; ch < NCH; ++ch) {
+  const int NCH = (3 * E + 31) / 32;
+  // chunk ch of the accumulator block -> the staging tile (every thread of the warpgroup, chunks in increasing order)
+  auto stage = [&](int ch) {
     warpgroup_bar(bar_id);                                     // the previous chunk's readers are done with the tile
     wgmma_stage_chunk<BN>(acc, ch, stg, EPI_LD, t);
     warpgroup_bar(bar_id);
-    if (!walker) continue;
-    const float* myrow = stg + t * EPI_LD;
-    const int ncol = min(32, 3 * E - ch * 32);
+  };
+  if (!walker) {                                               // warps 2 and 3 only help stage
 #pragma unroll 1
-    for (int j = 0; j < ncol; ++j) {
-      const int col = ch * 32 + j;
-      const float v = fmaf(myrow[j], s_ss[col], s_ss[BN + col]);   // scale 1, shift = bias
-      if (e < 5) {
-        if (e == 0) h0 = v;
-        else if (e == 1) h1 = v;
-        else if (e == 2) h2 = v;
-        else if (e == 3) h3 = v;
-        else {
-          cconf = sigmoid_ref(v);                              // model.py:167
-          cok = row_ok && cconf >= d.thr;                      // score = conf * prob <= conf: nothing below thr can pass
-          if (row_ok) {
-            float4 b;
-            decode_axis(h0, h2, offx, d.ratio_w, d.anchor_w[a], b.x, b.z);
-            decode_axis(h1, h3, offy, d.ratio_h, d.anchor_h[a], b.y, b.w);
-            reinterpret_cast<float4*>(d.boxes)[(long)img * d.B + box0 + a] = b;
-          }
-          cany = __any_sync(0xffffffffu, cok);
-        }
-      } else if (cany) {
-        bool pass = false;
-        float sc = 0.f;
-        if (cok && v >= d.logit_lo) {
-          sc = __fmul_rn(cconf, sigmoid_ref(v));               // model.py:168, test_single_image.py:55
-          pass = sc >= d.thr;                                  // utils/nms_utils.py:30
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, pass);
-        if (m != 0u) {                                         // warp-uniform
-          const int c = e - 5;
-          const unsigned mine = m & same;
-          const int leader = pass ? __ffs(mine) - 1 : lane;
-          int base = 0;
-          if (pass && lane == leader) base = atomicAdd(d.cand_count + img * d.C + c, __popc(mine));
-          base = __shfl_sync(0xffffffffu, base, leader);
-          if (pass) {
-            const long seg = ((long)img * d.C + c) * d.B;
-            const int slot = base + __popc(mine & lt);
-            d.cand_score[seg + slot] = sc;
-            d.cand_idx[seg + slot] = box0 + a;
-          }
+    for (int ch = 0; ch < NCH; ++ch) stage(ch);
+    return;
+  }
+  const float* myrow = stg + t * EPI_LD;
+  int staged = -1;                                             // the chunk in the staging tile
+  // logit of tile column col (col <= 32 (staged + 1)): its chunk is staged first if it is not there yet
+  auto logit = [&](int col) -> float {
+    if ((col >> 5) != staged) stage(++staged);
+    return fmaf(myrow[col & 31], s_ss[col], s_ss[BN + col]);   // scale 1, shift = bias
+  };
+#pragma unroll 1
+  for (int a = 0; a < 3; ++a) {
+    const int c0 = a * E;                                      // x, y, w, h, conf, then the C class logits
+    const float h0 = logit(c0), h1 = logit(c0 + 1), h2 = logit(c0 + 2), h3 = logit(c0 + 3);
+    const float cconf = sigmoid_ref(logit(c0 + 4));            // model.py:167
+    const bool cok = row_ok && cconf >= d.thr;                 // score = conf * prob <= conf: nothing below thr can pass
+    if (row_ok) {
+      float4 b;
+      decode_axis(h0, h2, offx, d.ratio_w, d.anchor_w[a], b.x, b.z);
+      decode_axis(h1, h3, offy, d.ratio_h, d.anchor_h[a], b.y, b.w);
+      reinterpret_cast<float4*>(d.boxes)[(long)img * d.B + box0 + a] = b;
+    }
+    if (!__any_sync(0xffffffffu, cok)) {                       // no candidate in this warp: stage past the class logits
+      while (staged < (c0 + E - 1) >> 5) stage(++staged);
+      continue;
+    }
+#pragma unroll 1
+    for (int c = 0; c < d.C; ++c) {
+      const float v = logit(c0 + 5 + c);
+      bool pass = false;
+      float sc = 0.f;
+      if (cok && v >= d.logit_lo) {
+        sc = __fmul_rn(cconf, sigmoid_ref(v));                 // model.py:168, test_single_image.py:55
+        pass = sc >= d.thr;                                    // utils/nms_utils.py:30
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, pass);
+      if (m != 0u) {                                           // warp-uniform
+        const unsigned mine = m & same;
+        const int leader = pass ? __ffs(mine) - 1 : lane;
+        int base = 0;
+        if (pass && lane == leader) base = atomicAdd(d.cand_count + img * d.C + c, __popc(mine));
+        base = __shfl_sync(0xffffffffu, base, leader);
+        if (pass) {
+          const long seg = ((long)img * d.C + c) * d.B;
+          const int slot = base + __popc(mine & lt);
+          d.cand_score[seg + slot] = sc;
+          d.cand_idx[seg + slot] = box0 + a;
         }
       }
-      if (++e == E) { e = 0; ++a; }
     }
   }
 }
@@ -377,8 +381,8 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const float (&
 // start its next main loop" (ping-pong)
 static constexpr int MMA_TURN_BAR = 3;
 
-// DET_E = 5 + classes: detection head with the decode fused in.  PP: ping-pong schedule (NC = 2, staged epilogue, no
-// fused decode; see the top of the file).  BKB: bytes per k-block row (Cfg).
+// DET: detection head with the decode fused in (epilogue_detect), all 3 (5 + C) columns in the one n-tile.  PP:
+// ping-pong schedule (NC = 2, staged epilogue, no fused decode; see the top of the file).  BKB: bytes per k-block row (Cfg).
 // CM x CN: a cluster of CM m-tiles x CN n-tiles, both schedules.  Each CTA loads 1/CN of its A tile, multicast to the
 // CN CTAs of its m-tile, and 1/CM of its B tile, multicast to the CM CTAs of its n-tile: every CTA still receives the
 // full STAGE_BYTES per k-block but reads only A_BYTES / CN + B_BYTES / CM of them from L2.  Each warpgroup computes
@@ -391,15 +395,15 @@ static constexpr int MMA_TURN_BAR = 3;
 // instead of waiting on a global load per 32-column chunk.  Each CTA loads its own tile (never multicast).
 // TMA (16-bit, NC = 2, no fused decode; p.epi_tma): the TMA-store epilogue (epilogue_tma) in place of the staged one.
 // The warps' output slabs lie where the staging tiles would; with RES they are the shortcut tile itself.
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
+template <typename T, int BN, int BKB, int NC, bool DET = false, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
           bool TMA = false>
 __global__ void __launch_bounds__(128 * (NC + 1), 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ ConvParams p) {
-  static_assert(!PP || (NC == 2 && DET_E == 0), "ping-pong: two consumer warpgroups, no fused decode");
+  static_assert(!PP || (NC == 2 && !DET), "ping-pong: two consumer warpgroups, no fused decode");
   static_assert(!RES || (PP && sizeof(T) == 2), "the shared-memory shortcut tile is a 16-bit ping-pong variant");
   static_assert(CM != 0 || CN == 1, "a run-time cluster shape is p.cluster x 1");
-  static_assert(!TMA || (sizeof(T) == 2 && NC == 2 && DET_E == 0), "the TMA-store epilogue: 16-bit, 128-row tiles, no fused decode");
+  static_assert(!TMA || (sizeof(T) == 2 && NC == 2 && !DET), "the TMA-store epilogue: 16-bit, 128-row tiles, no fused decode");
   constexpr int NH = PP ? 2 : 1;                         // 64-row accumulator blocks per consumer warpgroup
   using C = Cfg<BN, BKB, NC, RES>;
   constexpr int BK = BKB / (int)sizeof(T);               // channels per k-block
@@ -616,8 +620,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (n0 != ss_n0) {
         warpgroup_bar(bar_id);                   // nobody still reads the previous n-tile's values
         for (int c = t; c < BN; c += 128) {
-          const float sc = p.scale ? __ldg(p.scale + n0 + c) : 1.f;   // scale = shift = NULL: identity (dgrad convs)
-          const float sh = p.shift ? __ldg(p.shift + n0 + c) : 0.f;
+          // scale = shift = NULL: identity (dgrad convs).  A fused-decode head's tile may be wider than its cout_pad
+          // parameters (C 38-59: 192 on a 256-column tile); it reads only its first cout = 3 E columns.
+          const bool in = !DET || c < p.cout;
+          const float sc = p.scale && in ? __ldg(p.scale + n0 + c) : 1.f;
+          const float sh = p.shift && in ? __ldg(p.shift + n0 + c) : 0.f;
           if constexpr (TMA) {                   // (scale, scale, shift, shift) per column pair: one load per fragment
             sss[(c >> 1) * 4 + (c & 1)] = sc;
             sss[(c >> 1) * 4 + 2 + (c & 1)] = sh;
@@ -629,8 +636,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         warpgroup_bar(bar_id);
         ss_n0 = n0;
       }
-      if constexpr (DET_E > 0) {
-        epilogue_detect<BN, DET_E>(p, acc[0], m0 + cw * WG_ROWS, t, stg, sss, bar_id);
+      if constexpr (DET) {
+        epilogue_detect<BN>(p, acc[0], m0 + cw * WG_ROWS, t, stg, sss, bar_id);
       } else if constexpr (TMA) {
         if (m0 < p.M) {                          // units wholly past M store nothing
           const int wrow = 16 * (t >> 5);        // this warp's rows of each 64-row block
@@ -892,11 +899,11 @@ static int cluster_capacity(ClusterCapacity& cap, const void* kern, int threads,
 }
 
 // One conv_igemm_kernel instantiation: the type conv_kernel_for passes to its functor
-template <typename T, int BN, int BKB, int NC, int DET_E = 0, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
+template <typename T, int BN, int BKB, int NC, bool DET = false, bool PP = false, int CM = 0, int CN = 1, bool RES = false,
           bool TMA = false>
 struct ConvKernel {
   using C = Cfg<BN, BKB, NC, RES>;
-  static constexpr auto kernel = conv_igemm_kernel<T, BN, BKB, NC, DET_E, PP, CM, CN, RES, TMA>;
+  static constexpr auto kernel = conv_igemm_kernel<T, BN, BKB, NC, DET, PP, CM, CN, RES, TMA>;
 };
 
 static int no_conv_kernel(const ConvParams& p) {
@@ -910,11 +917,11 @@ static int no_conv_kernel(const ConvParams& p) {
 template <typename T, int BN, int BKB, bool RES, bool TMA, typename F>
 static int conv_kernel_pp_shape(const ConvParams& p, F& f) {
   const int cn = p.cluster_n, cm = p.cluster / p.cluster_n;
-  if (cm == 1 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 1, RES, TMA>());
+  if (cm == 1 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, false, true, 1, 1, RES, TMA>());
   if constexpr (sizeof(T) == 2) {
-    if (cm == 2 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 1, RES, TMA>());
-    if (cm == 1 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 1, 2, RES, TMA>());
-    if (cm == 2 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, 0, true, 2, 2, RES, TMA>());
+    if (cm == 2 && cn == 1) return f(ConvKernel<T, BN, BKB, 2, false, true, 2, 1, RES, TMA>());
+    if (cm == 1 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, false, true, 1, 2, RES, TMA>());
+    if (cm == 2 && cn == 2) return f(ConvKernel<T, BN, BKB, 2, false, true, 2, 2, RES, TMA>());
   }
   return no_conv_kernel(p);
 }
@@ -926,11 +933,11 @@ static int conv_kernel_pp(const ConvParams& p, F& f) {
   return no_conv_kernel(p);
 }
 
-template <typename T, int BN, int BKB, int DET_E, typename F>
+template <typename T, int BN, int BKB, bool DET, typename F>
 static int conv_kernel_tile(const ConvParams& p, F& f) {
   constexpr bool b16 = sizeof(T) == 2;
   if (p.pingpong) {
-    if constexpr (DET_E == 0) {
+    if constexpr (!DET) {
       if (!p.res_smem) return conv_kernel_pp<T, BN, BKB, false>(p, f);
       // the shared-memory shortcut tile: the 128-column, 128-byte k-block tiles of the 16-bit residual convs
       if constexpr (b16 && BN == 128 && BKB == 128) return conv_kernel_pp<T, BN, BKB, true>(p, f);
@@ -941,9 +948,9 @@ static int conv_kernel_tile(const ConvParams& p, F& f) {
   // warpgroup as well
   const bool shape = p.cluster_n == 1 && (p.cluster == 1 || (b16 && (p.cluster == 2 || p.cluster == 4)));
   if (!shape || p.res_smem) return no_conv_kernel(p);
-  if (p.consumers == 2 && !p.epi_tma) return f(ConvKernel<T, BN, BKB, 2, DET_E>());
-  if constexpr (b16 && DET_E == 0) {
-    if (p.consumers == 2) return f(ConvKernel<T, BN, BKB, 2, 0, false, 0, 1, false, true>());
+  if (p.consumers == 2 && !p.epi_tma) return f(ConvKernel<T, BN, BKB, 2, DET>());
+  if constexpr (b16 && !DET) {
+    if (p.consumers == 2) return f(ConvKernel<T, BN, BKB, 2, false, false, 0, 1, false, true>());
     if (p.consumers == 1 && !p.epi_tma) return f(ConvKernel<T, BN, BKB, 1>());
   }
   return no_conv_kernel(p);
@@ -953,15 +960,17 @@ template <typename T, typename F>
 static int conv_kernel_type(const ConvParams& p, F& f) {
   const int bn = p.block_n, kb = p.block_kb;
   if (p.det_e) {
-    // detection heads with the decode fused in: one n-tile holding all 3 * E columns
-    if (p.det_e == 85 && bn == 256 && kb == 128) return conv_kernel_tile<T, 256, 128, 85>(p, f);
-    if (p.det_e == 25 && bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, 25>(p, f);
+    // detection heads with the decode fused in: one n-tile holding all 3 (5 + C) columns, the class count read at run
+    // time (conv_select picks the width)
+    if (bn == 64 && kb == 128) return conv_kernel_tile<T, 64, 128, true>(p, f);
+    if (bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, true>(p, f);
+    if (bn == 256 && kb == 128) return conv_kernel_tile<T, 256, 128, true>(p, f);
     return no_conv_kernel(p);
   }
-  if (bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, 0>(p, f);
-  if (bn == 128 && kb == 64) return conv_kernel_tile<T, 128, 64, 0>(p, f);
-  if (bn == 64 && kb == 128) return conv_kernel_tile<T, 64, 128, 0>(p, f);
-  if (bn == 64 && kb == 64) return conv_kernel_tile<T, 64, 64, 0>(p, f);
+  if (bn == 128 && kb == 128) return conv_kernel_tile<T, 128, 128, false>(p, f);
+  if (bn == 128 && kb == 64) return conv_kernel_tile<T, 128, 64, false>(p, f);
+  if (bn == 64 && kb == 128) return conv_kernel_tile<T, 64, 128, false>(p, f);
+  if (bn == 64 && kb == 64) return conv_kernel_tile<T, 64, 64, false>(p, f);
   return no_conv_kernel(p);
 }
 
@@ -1037,6 +1046,9 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
     set_error("fused decode: %d output channels are not 3 x (5 + %d classes)", d->cout, det - 5);
     return YB_ERR_UNSUPPORTED;
   }
+  // the three anchors of a cell share one n-tile of at most 256 columns: 1 to 80 classes
+  YB_REQUIRE(det >= 0 && 3 * det <= 256, "fused decode: the %d columns of %d classes do not fit one 256-column tile "
+             "(at most 80 classes; more take forward + predict + nms)", 3 * det, det - 5);
   if (win) {
     YB_REQUIRE(r.kh >= 1 && r.kh <= 2 && r.kw >= 1 && r.kw <= 2 && r.scatter >= 0 && r.scatter <= 4, "conv: bad window");
     YB_REQUIRE(d->stride == 1 && !d->out_fp32 && !d->upsample2x && !r.stats,
@@ -1070,7 +1082,9 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
   const int P = d->h / d->stride, Q = d->w / d->stride;
   const int kh = win ? r.kh : d->ksize, kw = win ? r.kw : d->ksize;
   const int pad = win ? 0 : d->ksize / 2;
-  const int bn = det ? cout_pad : (cout_pad % 128 == 0 ? 128 : 64);
+  // fused-decode heads: the narrowest wgmma width that holds all 3 E columns (C 1-16: 64, 17-37: 128, 38-80: 256; a
+  // 256-column tile over cout_pad = 192 rows of weights, C 38-59, gets its last 64 rows zero-filled by the TMA)
+  const int bn = det ? (3 * det <= 64 ? 64 : 3 * det <= 128 ? 128 : 256) : (cout_pad % 128 == 0 ? 128 : 64);
   p->M = d->n * P * Q; p->P = P; p->Q = Q;
   // Kernel variants (testing / A-B switches; the detection heads always take the default):
   //   YB_CONV_EG=1        one consumer warpgroup per CTA (64-row tiles) instead of two (128-row tiles)
@@ -1107,7 +1121,7 @@ int conv_select(const ConvRequest& r, ConvParams* p) {
   p->pingpong = (!det && p->consumers == 2 && p->cluster == 1 && !p->epi_reg && pp_shape) ? 1 : 0;
   const int block_m = 64 * p->consumers;
   p->num_m_tiles = ceil_div(p->M, block_m);
-  p->num_n_tiles = cout_pad / bn;
+  p->num_n_tiles = det ? 1 : cout_pad / bn;
   // Ping-pong clusters, CM m-tiles x CN n-tiles (conv_igemm_kernel, DESIGN.md §4): each CTA reads 1/CN of its
   // im2col / activation tile and 1/CM of its weight tile from L2.  The plan rule (16-bit inference plans, forward
   // layers without statistics): 2 x 2 for the windowed convs with an even n-tile count, 2 x 1 for the other windowed

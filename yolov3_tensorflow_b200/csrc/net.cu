@@ -294,6 +294,14 @@ extern "C" int yb_net_layer_schedule(const yb_net* net, int layer, int sm_count,
   ConvParams p;
   int rc = conv_select(r, &p);
   if (rc) return rc;
+  if (!L.info.has_bn && 3 * (5 + net->class_num) <= 256) {   // the head's fused-decode launch (yb_net_detect)
+    ConvRequest rd{d};
+    rd.det_e = 5 + net->class_num;
+    ConvParams pd;
+    rc = conv_select(rd, &pd);
+    if (rc) return rc;
+    info->det_block_n = pd.block_n;
+  }
   info->igemm = 1;
   info->res_smem = p.res_smem;
   info->epi_tma = p.epi_tma;
@@ -350,7 +358,7 @@ extern "C" int yb_net_bind(yb_net* net, void* activation_arena, size_t activatio
                           nullptr, &L.fwd);
     if (rc) return rc;
     if (!L.info.has_bn) {
-      // fused-decode variant of the head (yb_net_detect); class counts without a kernel keep the unfused pipeline
+      // fused-decode variant of the head (yb_net_detect), for 1 to 80 classes; more keep the unfused pipeline
       ConvRequest rd{d};
       rd.det_e = 5 + net->class_num;
       void* x = ten_ptr(net, L.in);
