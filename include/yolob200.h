@@ -369,6 +369,32 @@ int yb_voc_ap(const uint64_t* pool, long pool_size, const uint64_t* class_counts
               void* workspace, size_t workspace_bytes, double* out, void* stream);
 
 /* ---------------------------------------------------------------------------------
+ * k-means anchors  (replaces get_kmeans.py:32-41 avg_iou and :59-93 kmeans, run by `python get_kmeans.py`,
+ * README.md:121-133): one Lloyd iteration is yb_kmeans_assign, a [k + 1] read on the host, then yb_kmeans_median.
+ * boxes [rows, 2] float64 (w, h), 16-byte aligned, every value finite and > 0 (the caller checks this: the median
+ * orders values by their bits); clusters [k, 2] float64.  1 <= k <= YB_KMEANS_MAX_K, k <= rows < 2^31.
+ * All three share one workspace of yb_kmeans_workspace_bytes(rows, k) bytes (too small: YB_ERR_WORKSPACE).
+ * --------------------------------------------------------------------------------- */
+enum { YB_KMEANS_MAX_K = 32 };
+int yb_kmeans_workspace_bytes(long rows, int k, size_t* bytes);
+/* get_kmeans.py:80-83: assign[i] = np.argmin over c of 1 - iou(boxes[i], clusters) (float64 in the reference's
+ * operation order, first minimum).  result [k + 1] int32 is overwritten: result[c] = boxes assigned to c,
+ * result[k] = boxes whose assignment differs from last_assign (get_kmeans.py:85 stops when it is 0).
+ * last_assign may be assign itself. */
+int yb_kmeans_assign(const double* boxes, long rows, const double* clusters, int k, const int32_t* last_assign,
+                     int32_t* assign, int32_t* result, void* workspace, size_t workspace_bytes, void* stream);
+/* get_kmeans.py:88-89: clusters_out[c] = np.median(boxes[assign == c], axis=0), bit for bit (a radix select of ranks
+ * (m-1)/2 and m/2 per column; an even count averages them as numpy does).  counts [k] = result[0..k) of the
+ * yb_kmeans_assign that wrote assign.  A cluster with count 0 gets NaN, as np.median of nothing does. */
+int yb_kmeans_median(const double* boxes, long rows, const int32_t* assign, const int32_t* counts, int k,
+                     double* clusters_out, void* workspace, size_t workspace_bytes, void* stream);
+/* get_kmeans.py:32-41: out (one device double) = np.mean of every box's max IoU over the clusters, bit for bit: the
+ * same pairwise summation tree numpy uses, then / rows.  Needs rows >= 1 only, and a workspace of
+ * yb_kmeans_workspace_bytes(rows, 1) bytes whatever k is. */
+int yb_kmeans_avg_iou(const double* boxes, long rows, const double* clusters, int k, double* out, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------
  * Loss  (replaces model.py:192-304 loss_layer, :307-345 box_iou, :348-365 compute_loss and
  * the part of TF autodiff (train.py:112) that differentiates them)
  * --------------------------------------------------------------------------------- */

@@ -17,6 +17,7 @@ YB_OPT_SGD, YB_OPT_MOMENTUM, YB_OPT_RMSPROP, YB_OPT_ADAM = 0, 1, 2, 3
 YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
 YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
 YB_VOC_MAX_GT = 1024
+YB_KMEANS_MAX_K = 32
 YB_LAYER_IGEMM, YB_LAYER_HALO, YB_LAYER_FUSED_STEM, YB_LAYER_STEM, YB_LAYER_THIN = 1, 2, 3, 4, 5
 
 
@@ -122,6 +123,10 @@ _SIGS = {
     "yb_voc_match": ([vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, C.c_double, vp, C.c_long, C.c_long, vp, vp], i32),
     "yb_voc_ap_workspace_bytes": ([C.c_long, i32, C.POINTER(sz)], i32),
     "yb_voc_ap": ([vp, C.c_long, vp, i32, i32, vp, sz, vp, vp], i32),
+    "yb_kmeans_workspace_bytes": ([C.c_long, i32, C.POINTER(sz)], i32),
+    "yb_kmeans_assign": ([vp, C.c_long, vp, i32, vp, vp, vp, vp, sz, vp], i32),
+    "yb_kmeans_median": ([vp, C.c_long, vp, vp, i32, vp, vp, sz, vp], i32),
+    "yb_kmeans_avg_iou": ([vp, C.c_long, vp, i32, vp, vp, sz, vp], i32),
     "yb_loss_workspace_bytes": ([i32, i32, i32, C.POINTER(sz)], i32),
     "yb_loss_layer": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32, i32, f32, f32, vp, sz, vp, vp, i32, i32, vp], i32),
     "yb_loss_finalize": ([vp, vp, vp], i32),
