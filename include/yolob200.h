@@ -395,6 +395,52 @@ int yb_kmeans_avg_iou(const double* boxes, long rows, const double* clusters, in
                       size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------
+ * JPEG decode  (replaces cv2.imread(pic_path) at utils/data_utils.py:130 and test_single_image.py:38): baseline
+ * JPEG files -> uint8 BGR pixels equal to cv2.imread of OpenCV 4.13 (IMREAD_COLOR, EXIF orientation applied), in
+ * the yb_resize_batch / PackedImages layout.  Supported: SOF0 / SOF1, 8-bit Huffman, 1 component (grey, replicated
+ * to BGR) or 3 components YCbCr, luma sampling 1x1, 2x1, 1x2 or 2x2 with chroma 1x1, one interleaved scan, restart
+ * intervals, EXIF orientation 1-8.  Everything else (also an SOS that lists the components in another order than SOF,
+ * or a stream past 2^32 bits once each restart segment is padded to a subsequence) is YB_ERR_UNSUPPORTED with the
+ * reason; a malformed header is
+ * YB_ERR_INVALID_ARGUMENT.  Batch calls prefix the reason with "image <index>: ".
+ * --------------------------------------------------------------------------------- */
+typedef struct yb_jpeg_info {
+  int height, width;           /* of the decoded (EXIF-oriented) image                           */
+  int src_height, src_width;   /* as stored in SOF                                               */
+  int components;              /* 1 or 3                                                         */
+  int h_samp, v_samp;          /* luma sampling factors (chroma is 1x1); 1x1 for grey           */
+  int restart_interval;        /* MCUs per restart interval, 0 = none                            */
+  int orientation;             /* EXIF orientation 1-8 (1 without an Exif block)                 */
+  int mode;                    /* 0 baseline (SOF0), 1 extended sequential Huffman (SOF1)        */
+} yb_jpeg_info;
+/* per-image decode status (int32, bits may combine); the image's pixels are unspecified when it is nonzero,
+ * libjpeg would warn and fill grey.  Only that image's slot is written. */
+enum {
+  YB_JPEG_OK = 0,
+  YB_JPEG_BAD_MARKER = 1,   /* a marker other than RSTn / EOI inside the entropy-coded data             */
+  YB_JPEG_BAD_RST = 2,      /* RST markers out of sequence or more than the restart interval implies    */
+  YB_JPEG_BAD_CODE = 4,     /* a Huffman code no table holds (the segment's decode stops there)         */
+  YB_JPEG_BAD_INDEX = 8,    /* a coefficient index past 63 (likewise)                                   */
+  YB_JPEG_TRUNCATED = 16    /* data (or restart segments) end before the last MCU                       */
+};
+/* host only: one file's header. */
+int yb_jpeg_parse(const void* data, size_t bytes, yb_jpeg_info* info);
+/* host only: the blob of n files (data[i], bytes[i]) that is the batch's one H2D copy: descriptors, quantisation
+ * and Huffman decode tables, compressed bytes.  It records the subsequence size of the Huffman decode
+ * (YB_JPEG_SUBSEQ_BITS) at pack time.  desc_host (optional) receives the int64 [n, 4] output table (pixel byte
+ * offset, height, width, row pitch), each image 16-byte aligned as PackedImages packs them. */
+int yb_jpeg_pack_bytes(const void* const* data, const size_t* bytes, int n, size_t* blob_bytes);
+int yb_jpeg_pack(const void* const* data, const size_t* bytes, int n, void* host_blob, size_t blob_bytes,
+                 int64_t* desc_host);
+/* host only: workspace bytes of yb_jpeg_decode for this blob (destuffed streams, sync records, coefficient blocks,
+ * component planes) and the pixel bytes out_pixels must hold (optional). */
+int yb_jpeg_workspace_bytes(const void* host_blob, int n, size_t* bytes, size_t* pixel_bytes);
+/* dev_blob: the device copy of host_blob (16-byte aligned).  Writes out_pixels and out_desc (int64 [n, 4], the
+ * table yb_jpeg_pack returns) and status int32 [n].  Six launches for the whole batch, no host synchronisation. */
+int yb_jpeg_decode(const void* dev_blob, const void* host_blob, int n, uint8_t* out_pixels, int64_t* out_desc,
+                   int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------
  * Loss  (replaces model.py:192-304 loss_layer, :307-345 box_iou, :348-365 compute_loss and
  * the part of TF autodiff (train.py:112) that differentiates them)
  * --------------------------------------------------------------------------------- */

@@ -18,6 +18,7 @@ YB_TRAIN_FORWARD_ONLY, YB_TRAIN_BN_FROZEN, YB_TRAIN_NO_BACKWARD = 1, 2, 4
 YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
 YB_VOC_MAX_GT = 1024
 YB_KMEANS_MAX_K = 32
+YB_JPEG_BAD_MARKER, YB_JPEG_BAD_RST, YB_JPEG_BAD_CODE, YB_JPEG_BAD_INDEX, YB_JPEG_TRUNCATED = 1, 2, 4, 8, 16
 YB_LAYER_IGEMM, YB_LAYER_HALO, YB_LAYER_FUSED_STEM, YB_LAYER_STEM, YB_LAYER_THIN = 1, 2, 3, 4, 5
 
 
@@ -65,6 +66,11 @@ class BnSchedule(C.Structure):     # yb_bn_schedule_info
 class LayerInfo(C.Structure):
     _fields_ = [(n, i32) for n in ("index", "cin", "cout", "ksize", "stride", "has_bn", "in_h", "in_w", "out_h",
                                    "out_w", "is_head", "scope_index", "upsample2x")]
+
+
+class JpegInfo(C.Structure):       # yb_jpeg_info
+    _fields_ = [(n, i32) for n in ("height", "width", "src_height", "src_width", "components", "h_samp", "v_samp",
+                                   "restart_interval", "orientation", "mode")]
 
 
 class Optimizer(C.Structure):      # yb_optimizer
@@ -127,6 +133,11 @@ _SIGS = {
     "yb_kmeans_assign": ([vp, C.c_long, vp, i32, vp, vp, vp, vp, sz, vp], i32),
     "yb_kmeans_median": ([vp, C.c_long, vp, vp, i32, vp, vp, sz, vp], i32),
     "yb_kmeans_avg_iou": ([vp, C.c_long, vp, i32, vp, vp, sz, vp], i32),
+    "yb_jpeg_parse": ([vp, sz, C.POINTER(JpegInfo)], i32),
+    "yb_jpeg_pack_bytes": ([C.POINTER(vp), C.POINTER(sz), i32, C.POINTER(sz)], i32),
+    "yb_jpeg_pack": ([C.POINTER(vp), C.POINTER(sz), i32, vp, sz, vp], i32),
+    "yb_jpeg_workspace_bytes": ([vp, i32, C.POINTER(sz), C.POINTER(sz)], i32),
+    "yb_jpeg_decode": ([vp, vp, i32, vp, vp, vp, vp, sz, vp], i32),
     "yb_loss_workspace_bytes": ([i32, i32, i32, C.POINTER(sz)], i32),
     "yb_loss_layer": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32, i32, f32, f32, vp, sz, vp, vp, i32, i32, vp], i32),
     "yb_loss_finalize": ([vp, vp, vp], i32),

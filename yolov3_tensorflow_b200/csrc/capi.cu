@@ -55,7 +55,8 @@ struct Opt { const char* key; char val[32]; };
 static Opt g_opts[] = {{"YB_CONV_MODE", ""}, {"YB_CONV_MC", ""}, {"YB_CONV_MCAST", ""}, {"YB_CONV_RES", ""}, {"YB_CONV_EPI", ""}, {"YB_CONV_EG", ""}, {"YB_CONV_PP", ""}, {"YB_CONV_CTAS", ""}, {"YB_THIN", ""}, {"YB_STEM_DBG", ""},
                        {"YB_STEM_WGRAD", ""}, {"YB_WGRAD_TP", ""}, {"YB_DGRAD_S2", ""},
                        {"YB_HALO", ""}, {"YB_STEM_FUSE", ""},
-                       {"YB_BN_CPT", ""}, {"YB_BN_FIN", ""}, {"YB_PACK_MT", ""}, {"YB_WGRAD_EPI", ""}, {"YB_WGRAD_SPLITS", ""}, {"YB_STEM_TRAIN", ""}, {"YB_WGRAD_STREAM", ""}, {"YB_STEM_SPLIT", ""}, {"YB_HEAD_STREAM", ""}};
+                       {"YB_BN_CPT", ""}, {"YB_BN_FIN", ""}, {"YB_PACK_MT", ""}, {"YB_WGRAD_EPI", ""}, {"YB_WGRAD_SPLITS", ""}, {"YB_STEM_TRAIN", ""}, {"YB_WGRAD_STREAM", ""}, {"YB_STEM_SPLIT", ""}, {"YB_HEAD_STREAM", ""},
+                       {"YB_JPEG_SUBSEQ_BITS", ""}};
 static std::once_flag g_opt_once;
 static void seed_opts() {
   for (auto& o : g_opts) {

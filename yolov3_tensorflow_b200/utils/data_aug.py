@@ -3,7 +3,9 @@
 (test_single_image.py:44-46) into device kernels (libyolob200.so: yb_letterbox_normalize for one image, yb_resize_batch
 for a batch of images of different sizes, letterbox or stretch, nearest or bilinear), plus the detections' way back to
 the source image (test_single_image.py:64-70, yb_restore_boxes).  Bit-exact vs cv2.resize(..., interpolation=0 / 1) of
-OpenCV 4.13; the random augmentations of training are CPU image I/O and out of scope."""
+OpenCV 4.13; the random augmentations of training are CPU image I/O and out of scope.  `decode_jpeg_batch` replaces
+the cv2.imread in front of them (utils/data_utils.py:130, test_single_image.py:38): baseline JPEG files decoded on the
+device (yb_jpeg_decode), equal to cv2.imread byte for byte, straight into the PackedImages layout."""
 from __future__ import annotations
 
 import ctypes as C
@@ -11,6 +13,7 @@ import ctypes as C
 import numpy as np
 import torch
 
+from .. import _lib
 from .._lib import lib, check, ptr, stream_handle
 
 
@@ -75,6 +78,28 @@ class PackedImages:
         self.desc = desc
         self.data = pinned.to(dev, non_blocking=True)          # the one host -> device copy
         self.h2d_bytes = int(pinned.numel())
+        self.status = None
+
+    @classmethod
+    def from_device(cls, data, desc, status=None, h2d_bytes=0):
+        """A batch whose pixels are already on the device: data uint8 CUDA tensor holding the int64 [n, 4]
+        descriptor table and the pixels (the layout above), desc its int64 [n, 4] host copy.  No copy is made."""
+        self = cls.__new__(cls)
+        self.device = data.device
+        self.desc = np.ascontiguousarray(desc, np.int64)
+        self.n = int(self.desc.shape[0])
+        self.data = data
+        self.h2d_bytes = int(h2d_bytes)
+        self.status = status
+        return self
+
+    def __len__(self):
+        return self.n
+
+    def image(self, i):
+        """uint8 [H, W, 3] BGR view of image i on the device."""
+        off, h, w, pitch = (int(v) for v in self.desc[i])
+        return self.pixels[off: off + h * pitch].view(h, w, 3)
 
     @property
     def desc_dev(self):
@@ -103,7 +128,8 @@ def _resize_packed(packed, new_width, new_height, letterbox, interp, out=None):
 
 
 def preprocess_batch(images, new_width, new_height, letterbox=True, interp=1, out=None, device=None):
-    """images: list of uint8 [H, W, 3] BGR images of any sizes (numpy arrays or tensors) ->
+    """images: list of uint8 [H, W, 3] BGR images of any sizes (numpy arrays or tensors), or a PackedImages (from
+    decode_jpeg_batch: no second upload) ->
     (x float32 [n, new_height, new_width, 3] RGB in [0, 1] on the device, params float64 [n, 4] on the device).
 
     letterbox=True is letterbox_resize (utils/data_aug.py:274-293, 128-grey border), False a plain stretch to the
@@ -112,7 +138,7 @@ def preprocess_batch(images, new_width, new_height, letterbox=True, interp=1, ou
     params rows are (resize_ratio, dw, dh, 1) for letterbox, (ori_w / new_w, ori_h / new_h, 0, 0) for stretch: what
     restore_boxes needs.  The images are packed into one pinned buffer, copied with one H2D copy and resized in one
     launch; no host synchronisation."""
-    packed = PackedImages(images, device)
+    packed = images if isinstance(images, PackedImages) else PackedImages(images, device)
     return _resize_packed(packed, new_width, new_height, letterbox, interp, out)
 
 
@@ -149,3 +175,78 @@ def restore_boxes(out_boxes, counts, params, inplace=False):
             check(lib.yb_restore_boxes(ptr(b), ptr(counts.contiguous()), int(b.shape[0]), int(b.shape[1]), 4,
                                        ptr(params.contiguous()), stream_handle()), "yb_restore_boxes")
     return b
+
+
+def _jpeg_bytes(src):
+    if isinstance(src, (bytes, bytearray, memoryview)):
+        return bytes(src)
+    if isinstance(src, np.ndarray):
+        return src.tobytes()
+    with open(src, "rb") as f:
+        return f.read()
+
+
+def decode_jpeg_batch(sources, device=None, check=True):
+    """cv2.imread (IMREAD_COLOR, EXIF orientation applied) for a batch of baseline JPEG files, on the device:
+    sources are bytes-like objects or file paths -> PackedImages of uint8 BGR images equal to cv2.imread's, which
+    preprocess_batch / val_batch take without a second upload.
+
+    Headers are parsed on the host first: an unsupported or malformed file raises ValueError naming its index and
+    the reason before any device work.  Then one pinned blob (tables + compressed bytes) crosses PCIe and six launches
+    decode the whole batch.  Corrupt entropy-coded data gives the image a nonzero status (include/yolob200.h:
+    YB_JPEG_*) where libjpeg would warn and fill grey; other images are unaffected.  check=True reads the statuses
+    back once (a host synchronisation) and raises ValueError listing the corrupt images; check=False does not
+    synchronise, and `packed.status` (int32 [n] on the device) holds the codes."""
+    dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+    files = [_jpeg_bytes(s) for s in sources]
+    n = len(files)
+    if n == 0:
+        raise ValueError("no images")
+    bufs = [C.create_string_buffer(f, len(f)) for f in files]
+    ptrs = (C.c_void_p * n)(*[C.cast(b, C.c_void_p) for b in bufs])
+    sizes = (C.c_size_t * n)(*[len(f) for f in files])
+    blob_bytes = C.c_size_t()
+    check_rc(lib.yb_jpeg_pack_bytes(ptrs, sizes, n, C.byref(blob_bytes)), "decode_jpeg_batch")
+    host = torch.empty((blob_bytes.value,), dtype=torch.uint8, pin_memory=True)
+    desc = np.zeros((n, 4), np.int64)
+    check_rc(lib.yb_jpeg_pack(ptrs, sizes, n, C.c_void_p(host.data_ptr()), blob_bytes.value,
+                              desc.ctypes.data_as(C.c_void_p)), "decode_jpeg_batch")
+    ws_bytes, pix_bytes = C.c_size_t(), C.c_size_t()
+    check_rc(lib.yb_jpeg_workspace_bytes(C.c_void_p(host.data_ptr()), n, C.byref(ws_bytes), C.byref(pix_bytes)),
+             "decode_jpeg_batch")
+    with torch.cuda.device(dev):
+        blob = host.to(dev, non_blocking=True)                 # the one host -> device copy
+        ws = torch.empty((ws_bytes.value,), dtype=torch.uint8, device=dev)
+        data = torch.empty((n * 32 + max(pix_bytes.value, 1),), dtype=torch.uint8, device=dev)
+        status = torch.empty((n,), dtype=torch.int32, device=dev)
+        check_rc(lib.yb_jpeg_decode(ptr(blob), C.c_void_p(host.data_ptr()), n, ptr(data[n * 32:]), ptr(data),
+                                    ptr(status), ptr(ws), ws_bytes.value, stream_handle()), "yb_jpeg_decode")
+    packed = PackedImages.from_device(data, desc, status, h2d_bytes=blob_bytes.value)
+    if check:
+        bad = [(i, int(v)) for i, v in enumerate(status.cpu().tolist()) if v]
+        if bad:
+            raise ValueError("corrupt JPEG data: " + ", ".join(f"image {i}: {jpeg_status_text(v)}" for i, v in bad))
+    return packed
+
+
+def jpeg_status_text(code):
+    names = {_lib.YB_JPEG_BAD_MARKER: "unexpected marker", _lib.YB_JPEG_BAD_RST: "restart markers out of sequence",
+             _lib.YB_JPEG_BAD_CODE: "bad Huffman code", _lib.YB_JPEG_BAD_INDEX: "coefficient index past 63",
+             _lib.YB_JPEG_TRUNCATED: "data ends before the last MCU"}
+    return ", ".join(v for k, v in names.items() if code & k) or "ok"
+
+
+def jpeg_info(source):
+    """yb_jpeg_parse of one file: dict of the oriented height / width, stored size, components, luma sampling,
+    restart interval, orientation and mode (0 SOF0, 1 SOF1).  ValueError with the reason when it is not supported."""
+    f = _jpeg_bytes(source)
+    info = _lib.JpegInfo()
+    check_rc(lib.yb_jpeg_parse(f, len(f), C.byref(info)), "jpeg_info")
+    return {k: getattr(info, k) for k, _ in info._fields_}
+
+
+def check_rc(rc, what):
+    """check() for the JPEG entry points: an unsupported file is a ValueError as well."""
+    if rc == -3:
+        raise ValueError(f"{what}: {lib.yb_last_error_string().decode('utf-8', 'replace')}")
+    check(rc, what)

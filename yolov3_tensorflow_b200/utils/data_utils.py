@@ -62,7 +62,7 @@ def val_batch(images, boxes_list, labels_list, img_size, class_num, anchors, let
     """parse_data(mode='val') (utils/data_utils.py:166-182) for a batch, on the device: resize_with_bbox(interp=1,
     letterbox=letterbox_resize) + cvtColor(BGR2RGB) + float32 / 255 for the images (one H2D copy of the uint8 pixels,
     one launch), the same box transform, then process_box_batch.
-      images: uint8 [H, W, 3] BGR images of any sizes; boxes_list: per image float32 [V, 4] (x_min, y_min, x_max,
+      images: uint8 [H, W, 3] BGR images of any sizes, or a PackedImages (decode_jpeg_batch); boxes_list: per image float32 [V, 4] (x_min, y_min, x_max,
       y_max in source pixels) or [V, 5] with a mix-up weight (1 when absent, as parse_data adds); labels_list: per
       image [V] ints; img_size: [W, H], multiples of 32.
     -> (x [n, H, W, 3], y_true_13, y_true_26, y_true_52), float32 on the device, no host synchronisation."""
@@ -80,7 +80,7 @@ def val_batch(images, boxes_list, labels_list, img_size, class_num, anchors, let
             raise ValueError(f"val_batch: image {i}: boxes must be [V, 4] or [V, 5], got {b.shape}")
         bl.append(b)
     W, H = int(img_size[0]), int(img_size[1])
-    packed = PackedImages(images, device)
+    packed = images if isinstance(images, PackedImages) else PackedImages(images, device)
     dev = packed.device
     x, _ = _resize_packed(packed, W, H, letterbox_resize, 1)
     hb, hl, hc = pack_gt(bl, labels_list)
