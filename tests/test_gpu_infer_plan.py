@@ -32,6 +32,7 @@ import torch
 
 from oracle import yolov3_oracle as O
 from tests import conv_ref as R
+from tests import direct_ref as D
 from tests import infer_plan_ref as P
 from tests.synth import gen_inputs
 from tests.test_gpu_path import _train_case
@@ -39,7 +40,6 @@ from tests.test_gpu_path import _train_case
 pytestmark = pytest.mark.gpu
 CLASSES = 80
 NMS = (200, 0.3, 0.45)             # max_boxes, score_thresh, nms_thresh: bench.py's
-STEM_N16 = 2                       # the mma.sync stem: K = 27 padded to 32, two k16 steps
 EPS32 = float(np.float32(1e-5))    # the plan's BN epsilon (1e-5f)
 FOLD_ULPS = 3                      # yb_bn_fold: var + eps, sqrtf and the divide round once each (< 2.5 u relative)
 
@@ -60,12 +60,6 @@ def _bits(t):
 def _count(mask):
     """Number of True elements; the reduction to a count (int64) runs only when there is one."""
     return int(torch.count_nonzero(mask)) if bool(mask.any()) else 0
-
-
-def rn16(v, dtype):
-    """Round-to-nearest-even of float64 v into fp16 / bf16, as float64 (exact: scaled by the spacing at |v|)."""
-    q = R.ulp(v, dtype)
-    return torch.round(v / q) * q
 
 
 def ulp32(a):
@@ -192,15 +186,13 @@ class InferRun:
             sc0, sh0 = folds[0]
             v0 = R.epilogue(raw, sc0, sh0, leaky=True)
             if self.fused:
-                e0 = R.out_bound(v0, S, STEM_N16, torch.float32, scale=sc0, shift=sh0)
-                xs = rn16(v0, dt)
-                d = torch.maximum(rn16(v0 + e0, dt) - xs, xs - rn16(v0 - e0, dt))
+                xs, d = D.stem_interval(v0, S, dt, sc0, sh0)
                 shp = (1, infos[0].out_h, infos[0].out_w, infos[0].cout)
                 stem_in = (xs.reshape(shp), d.reshape(shp))
                 self.near_mid = max(self.near_mid, float((d > 0).double().mean()))
             else:
                 got = outs[0][im].reshape(-1, infos[0].cout)
-                b = R.out_bound(v0, S, STEM_N16, dt, scale=sc0, shift=sh0)
+                b = R.out_bound(v0, S, D.STEM_N16, dt, scale=sc0, shift=sh0)
                 self.worst.add("stem", f"layer 0 image {im}", R.check_out(got, v0, b, f"{self.cid} layer 0 image {im}"))
                 stem_in = None
             del raw, S, v0
@@ -211,10 +203,7 @@ class InferRun:
                 pad = f.ksize // 2
                 extra = 0.0
                 if i == 1 and stem_in is not None:
-                    xs, d = stem_in
-                    raw, _ = R.conv_raw(xs, w16[1], f.stride, pad)
-                    _, S = R.conv_raw(xs.abs() + d, w16[1], f.stride, pad)
-                    extra = folds[1][0].double().abs() * R.conv_raw(d, w16[1], f.stride, pad)[1]
+                    raw, S, extra = D.conv1_on_interval(*stem_in, w16[1], f.stride, folds[1][0])
                 else:
                     xin = ins[i][im:im + 1]
                     assert bool(torch.isfinite(xin).all()), f"{name}: its input holds the sentinel or a non-finite value"

@@ -10,6 +10,8 @@ flat gradient and the refresh of the 16-bit weights after an update are part of 
     padding rows zero; the stride-1 dgrad weights are the flip + transpose of RN16(master) bit for bit;
   - forward: each BN layer's raw z and batch sums [Σz | Σz²] against conv_ref.conv_raw of its own input view (concat
     slices included) and RN16(master), within conv_ref.out_bound / stats_bound; the heads' fp32 maps as conv + bias;
+    the split-precision stem's z against the float64 conv of the image and its float32 masters, and its sums against
+    float64 sums of the stored z (tests/direct_ref.py);
   - input gradient, checked right after each layer's backward GLOBAL phase: dX = conv_transpose(dz, RN16(master)) + R
     within out_bound, where R is dA(out_b) for the layer before a residual layer b, the gradient already there for a
     second consumer, and 0 otherwise; every channel and row outside the layer's slice keeps its bits;
@@ -27,6 +29,7 @@ import torch
 
 from oracle import yolov3_oracle as O
 from tests import conv_ref as R
+from tests import direct_ref as D
 from tests import train_plan_ref as T
 from tests import wgrad_ref as W
 from tests.test_gpu_path import _train_case
@@ -124,7 +127,7 @@ class PlanRun:
         after its launch."""
         L, m = self.L, self.m
         x, ys, plan, opt, _ = self.setup(lr)
-        self.plan = plan
+        self.plan, self.image = plan, x
         h, st, px = plan.handle, L.stream_handle(), L.ptr(x)
         nl = plan.num_layers
         for i in range(nl):
@@ -188,8 +191,43 @@ class PlanRun:
                 assert bad == 0, f"layer {i}: {bad} elements of the dgrad weights differ from flip + transpose of RN16(master)"
 
     # ------------------------------------------------------------------ forward
+    def check_stem_forward(self):
+        """Layer 0, the split-precision stem: z against the float64 conv of the image and the float32 master weights
+        within direct_ref.stem_split_bound, its [Σz | Σz²] against float64 sums of the stored z within sums_bound."""
+        plan, dt = self.plan, self.dtype
+        # the model of the split stem: YB_STEM_TRAIN=cuda runs the CUDA-core stem and yb_col_stats instead
+        assert self.L.get_option("YB_STEM_TRAIN")[:1] != "c" and self.L.get_option("YB_STEM_SPLIT")[:1] != "0"
+        info = plan.layer_info(0)
+        wt = plan.conv_params(0)["w"]
+        Aw = wt.double().abs().reshape(info.cout, -1).sum(1)
+        z = plan.train_buffer(0, "z")
+        zs = torch.zeros(info.cout, dtype=torch.float64, device="cuda")
+        zq, za = torch.zeros_like(zs), torch.zeros_like(zs)
+        worst = 0.0
+        for j in range(plan.n):
+            x = self.image[j:j + 1]
+            raw, S = R.conv_raw(x, wt, 1, 1)
+            zj = z[j].reshape(-1, info.cout)
+            b = D.stem_split_bound(raw, S, D.stem_patch_abs(x), Aw, dt)
+            worst = max(worst, R.check_out(zj, raw, b, f"{self.cid} layer 0 z image {j}"))
+            zd = zj.double()
+            zs += zd.sum(0); zq += (zd * zd).sum(0); za += zd.abs().sum(0)
+            del raw, S, b
+        self.worst.add("stem z", 0, worst)
+        tiles = plan.n * -(-plan.h // STEM_TH) * -(-plan.w // STEM_TW)
+        depth = D.sums_depth(tiles, _sms(self.L))
+        slab = plan.bn_exchange_buffer(0, False)
+        cp = slab.numel() // 2
+        name = f"{self.cid} layer 0"
+        fs = R.check_out(slab[:info.cout], zs, depth * D.U32 * za, name + " sum z")
+        fq = R.check_out(slab[cp:cp + info.cout], zq, depth * D.U32 * zq, name + " sum z^2")
+        self.worst.add("stem sum z", 0, fs)
+        self.worst.add("stem sum z^2", 0, fq)
+        print(f"PLAN {self.cid} layer 0: z worst err/bound {worst:.3f}, sum z {fs:.3f}, sum z^2 {fq:.3f} (depth {depth})")
+
     def check_forward(self):
         plan = self.plan
+        self.check_stem_forward()
         for i in range(1, plan.num_layers):
             info = plan.layer_info(i)
             p = plan.conv_params(i)
