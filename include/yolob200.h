@@ -441,6 +441,46 @@ int yb_jpeg_decode(const void* dev_blob, const void* host_blob, int n, uint8_t* 
                    int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------
+ * JPEG encode  (replaces cv2.imwrite / cv2.imencode('.jpg'), test_single_image.py:85): uint8 BGR or grey images on
+ * the device -> baseline JPEG files equal byte for byte to cv2.imencode of OpenCV 4.13 (libjpeg-turbo 3.1) with the
+ * same IMWRITE_JPEG_QUALITY, _SAMPLING_FACTOR, _RST_INTERVAL, _LUMA_QUALITY and _CHROMA_QUALITY.  Standard Huffman
+ * tables, one interleaved scan (one component for grey).  A bad image description is YB_ERR_INVALID_ARGUMENT with
+ * the reason; batch calls prefix it with "image <index>: ".
+ * --------------------------------------------------------------------------------- */
+enum {   /* sampling: OpenCV's IMWRITE_JPEG_SAMPLING_FACTOR_* values (luma h, v; chroma 1x1) */
+  YB_JPEG_SAMPLING_411 = 0x411111,
+  YB_JPEG_SAMPLING_420 = 0x221111,
+  YB_JPEG_SAMPLING_422 = 0x211111,
+  YB_JPEG_SAMPLING_440 = 0x121111,
+  YB_JPEG_SAMPLING_444 = 0x111111
+};
+typedef struct yb_jpeg_enc_image {
+  const void* pixels;          /* device address of row 0 (not read by the host-only calls)                    */
+  int64_t pitch;               /* bytes from one row to the next, >= width * channels                          */
+  int height, width;           /* 1..65535                                                                     */
+  int channels;                /* 3: BGR (three-component YCbCr file), 1: grey (one-component file)            */
+  int quality;                 /* IMWRITE_JPEG_QUALITY, clamped to 0..100 as OpenCV does                       */
+  int luma_quality;            /* IMWRITE_JPEG_LUMA_QUALITY, < 0: not given                                    */
+  int chroma_quality;          /* IMWRITE_JPEG_CHROMA_QUALITY, < 0: not given                                  */
+  int sampling;                /* YB_JPEG_SAMPLING_*; grey ignores it                                          */
+  int restart_interval;        /* IMWRITE_JPEG_RST_INTERVAL in MCUs, clamped to 0..65535; 0: none              */
+} yb_jpeg_enc_image;
+/* host only: the file's bytes up to and including SOS.  out NULL (or capacity too small: YB_ERR_WORKSPACE) only
+ * reports the length in *bytes. */
+int yb_jpeg_enc_header(const yb_jpeg_enc_image* image, uint8_t* out, size_t capacity, size_t* bytes);
+/* host only: the blob of n images that is the batch's one H2D copy: image geometry, quantisation reciprocals,
+ * Huffman code tables and headers. */
+int yb_jpeg_enc_pack_bytes(const yb_jpeg_enc_image* images, int n, size_t* blob_bytes);
+int yb_jpeg_enc_pack(const yb_jpeg_enc_image* images, int n, void* host_blob, size_t blob_bytes);
+/* host only: workspace bytes of yb_jpeg_enc_encode for this blob and the output capacity out must have (an upper
+ * bound on the n files together). */
+int yb_jpeg_enc_workspace_bytes(const void* host_blob, int n, size_t* workspace_bytes, size_t* out_bytes);
+/* dev_blob: the device copy of host_blob (16-byte aligned).  Writes the n files back to back from out[0] and
+ * out_desc int64 [n, 2] = (byte offset, length).  Eight launches for the whole batch, no host synchronisation. */
+int yb_jpeg_enc_encode(const void* dev_blob, const void* host_blob, int n, uint8_t* out, size_t out_bytes,
+                       int64_t* out_desc, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------
  * Loss  (replaces model.py:192-304 loss_layer, :307-345 box_iou, :348-365 compute_loss and
  * the part of TF autodiff (train.py:112) that differentiates them)
  * --------------------------------------------------------------------------------- */

@@ -5,7 +5,9 @@ for a batch of images of different sizes, letterbox or stretch, nearest or bilin
 the source image (test_single_image.py:64-70, yb_restore_boxes).  Bit-exact vs cv2.resize(..., interpolation=0 / 1) of
 OpenCV 4.13; the random augmentations of training are CPU image I/O and out of scope.  `decode_jpeg_batch` replaces
 the cv2.imread in front of them (utils/data_utils.py:130, test_single_image.py:38): baseline JPEG files decoded on the
-device (yb_jpeg_decode), equal to cv2.imread byte for byte, straight into the PackedImages layout."""
+device (yb_jpeg_decode), equal to cv2.imread byte for byte, straight into the PackedImages layout.
+`encode_jpeg_batch` / `write_jpeg_batch` are cv2.imencode('.jpg') / cv2.imwrite (test_single_image.py:85) for a batch
+on the device (yb_jpeg_enc_encode), byte for byte."""
 from __future__ import annotations
 
 import ctypes as C
@@ -250,3 +252,117 @@ def check_rc(rc, what):
     if rc == -3:
         raise ValueError(f"{what}: {lib.yb_last_error_string().decode('utf-8', 'replace')}")
     check(rc, what)
+
+
+def _per_image(name, value, n):
+    vals = list(value) if isinstance(value, (list, tuple)) else [value] * n
+    if len(vals) != n:
+        raise ValueError(f"{name}: {len(vals)} values for {n} images")
+    return vals
+
+
+def encode_jpeg_batch(images, quality=95, sampling="420", restart_interval=0, luma_quality=None, chroma_quality=None,
+                      to_host=True, optimize=False, progressive=False, device=None):
+    """cv2.imencode('.jpg', img, params) for a batch, on the device: baseline JPEG files equal to OpenCV 4.13's byte
+    for byte.  images: a PackedImages (decode_jpeg_batch's output: no upload), or a list of uint8 BGR [H, W, 3] or
+    grey [H, W] / [H, W, 1] images as numpy arrays or tensors (CUDA tensors are read in place; host images cross in
+    one pinned H2D copy).  Grey gives a one-component file.
+
+    quality, sampling ("411", "420", "422", "440", "444"), restart_interval, luma_quality and chroma_quality are
+    IMWRITE_JPEG_QUALITY, _SAMPLING_FACTOR, _RST_INTERVAL, _LUMA_QUALITY and _CHROMA_QUALITY (None: not given), each
+    a value for the batch or a list with one per image.  Progressive and optimised-Huffman files are not supported.
+
+    to_host=True returns a list of bytes; reading the lengths is the one synchronisation, then one D2H copy.
+    to_host=False returns (data, desc) without synchronising: data a uint8 CUDA tensor with the files back to back
+    from offset 0 (its size is an upper bound), desc an int64 [n, 2] CUDA tensor of (offset, length)."""
+    if optimize:
+        raise ValueError("encode_jpeg_batch: optimised Huffman tables (IMWRITE_JPEG_OPTIMIZE) are not supported")
+    if progressive:
+        raise ValueError("encode_jpeg_batch: progressive JPEG (IMWRITE_JPEG_PROGRESSIVE) is not supported")
+    keep = []                                        # tensors the launches read
+    if isinstance(images, PackedImages):
+        n, dev = images.n, images.device
+        base = images.pixels.data_ptr()
+        keep.append(images.data)
+        srcs = [(base + int(o), int(h), int(w), 3, int(p)) for o, h, w, p in images.desc.tolist()]
+    else:
+        images = list(images)
+        n = len(images)
+        srcs, host = [None] * n, []
+        for i, im in enumerate(images):
+            t = im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(im)))
+            if t.dtype != torch.uint8 or t.dim() not in (2, 3) or (t.dim() == 3 and t.shape[2] not in (1, 3)):
+                raise ValueError(f"image {i}: expected uint8 [H, W, 3] BGR or [H, W] / [H, W, 1] grey, got "
+                                 f"{t.dtype} {tuple(t.shape)}")
+            h, w = int(t.shape[0]), int(t.shape[1])
+            c = 1 if t.dim() == 2 else int(t.shape[2])
+            if not (1 <= h <= 65535 and 1 <= w <= 65535):
+                raise ValueError(f"image {i}: size {h} x {w} is outside 1..65535")
+            if t.is_cuda:
+                t = t.contiguous()
+                keep.append(t)
+                srcs[i] = (t.data_ptr(), h, w, c, w * c)
+            else:
+                host.append((i, t.contiguous(), h, w, c))
+        if n == 0:
+            raise ValueError("encode_jpeg_batch: no images")
+        on_dev = [t.device for t in keep]
+        dev = torch.device(device if device is not None else
+                           on_dev[0] if on_dev else f"cuda:{torch.cuda.current_device()}")
+        if host:
+            offs, total = [], 0
+            for _, t, *_ in host:
+                offs.append(total)
+                total += (t.numel() + 15) // 16 * 16
+            pinned = torch.empty((total,), dtype=torch.uint8, pin_memory=True)
+            for o, (_, t, *_) in zip(offs, host):
+                pinned[o: o + t.numel()] = t.reshape(-1)
+            with torch.cuda.device(dev):
+                up = pinned.to(dev, non_blocking=True)           # the one host -> device copy of the pixels
+            keep.append(up)
+            for o, (i, _, h, w, c) in zip(offs, host):
+                srcs[i] = (up.data_ptr() + o, h, w, c, w * c)
+    q = _per_image("quality", quality, n)
+    sm = _per_image("sampling", sampling, n)
+    ri = _per_image("restart_interval", restart_interval, n)
+    lq = _per_image("luma_quality", luma_quality, n)
+    cq = _per_image("chroma_quality", chroma_quality, n)
+    desc = (_lib.JpegEncImage * n)()
+    for i, (ptr_i, h, w, c, pitch) in enumerate(srcs):
+        if str(sm[i]) not in _lib.YB_JPEG_SAMPLING:
+            raise ValueError(f"image {i}: sampling must be one of {sorted(_lib.YB_JPEG_SAMPLING)}, got {sm[i]!r}")
+        desc[i] = _lib.JpegEncImage(ptr_i, pitch, h, w, c, int(q[i]), -1 if lq[i] is None else int(lq[i]),
+                                    -1 if cq[i] is None else int(cq[i]), _lib.YB_JPEG_SAMPLING[str(sm[i])], int(ri[i]))
+    blob_bytes = C.c_size_t()
+    check(lib.yb_jpeg_enc_pack_bytes(desc, n, C.byref(blob_bytes)), "encode_jpeg_batch")
+    hblob = torch.empty((blob_bytes.value,), dtype=torch.uint8, pin_memory=True)
+    check(lib.yb_jpeg_enc_pack(desc, n, C.c_void_p(hblob.data_ptr()), blob_bytes.value), "encode_jpeg_batch")
+    ws_bytes, out_bytes = C.c_size_t(), C.c_size_t()
+    check(lib.yb_jpeg_enc_workspace_bytes(C.c_void_p(hblob.data_ptr()), n, C.byref(ws_bytes), C.byref(out_bytes)),
+          "encode_jpeg_batch")
+    with torch.cuda.device(dev):
+        blob = hblob.to(dev, non_blocking=True)
+        ws = torch.empty((ws_bytes.value,), dtype=torch.uint8, device=dev)
+        data = torch.empty((out_bytes.value,), dtype=torch.uint8, device=dev)
+        out_desc = torch.empty((n, 2), dtype=torch.int64, device=dev)
+        check(lib.yb_jpeg_enc_encode(ptr(blob), C.c_void_p(hblob.data_ptr()), n, ptr(data), out_bytes.value,
+                                     ptr(out_desc), ptr(ws), ws_bytes.value, stream_handle()), "yb_jpeg_enc_encode")
+    if not to_host:
+        return data, out_desc
+    d = out_desc.cpu().numpy()                        # the one synchronisation
+    total = int(d[-1, 0] + d[-1, 1])
+    host = torch.empty((total,), dtype=torch.uint8, pin_memory=True)
+    host.copy_(data[:total])                          # the one D2H copy
+    buf = host.numpy().tobytes()
+    return [buf[o: o + ln] for o, ln in d.tolist()]
+
+
+def write_jpeg_batch(paths, images, **kw):
+    """cv2.imwrite(path, img, params) for a batch: encode_jpeg_batch(images, **kw) written to paths."""
+    paths = list(paths)
+    files = encode_jpeg_batch(images, **kw)
+    if len(paths) != len(files):
+        raise ValueError(f"write_jpeg_batch: {len(paths)} paths for {len(files)} images")
+    for p, f in zip(paths, files):
+        with open(p, "wb") as fh:
+            fh.write(f)
