@@ -481,6 +481,42 @@ int yb_jpeg_enc_encode(const void* dev_blob, const void* host_blob, int n, uint8
                        int64_t* out_desc, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------
+ * Detection drawing  (replaces utils/plot_utils.py plot_one_box and the loop of test_single_image.py:81-83 /
+ * video_test.py:91): cv2.rectangle + filled label box + cv2.putText(FONT_HERSHEY_SIMPLEX, LINE_AA) per detection,
+ * in order, equal to OpenCV 4.13's pixels, at every line thickness.
+ * --------------------------------------------------------------------------------- */
+enum { YB_PLOT_SUFFIX_MAX = 48 };            /* longest score suffix ", -<39 digits>.dd%" */
+enum { YB_PLOT_BAD_LABEL = 1, YB_PLOT_BAD_BOX = 2 };
+typedef struct yb_plot_layout {
+  int length;                  /* label characters (FONT_HERSHEY_SIMPLEX codes ' ' .. '~') written to text     */
+  int thickness;               /* font thickness max(tl - 1, 1)                                                */
+  int text_w, text_h;          /* cv2.getTextSize(text, 0, tl / 3, thickness)[0]                               */
+  int rect_x1, rect_y1;        /* the filled label rectangle runs from (x0, y0) to here                        */
+  int org_x, org_y;            /* putText origin                                                               */
+} yb_plot_layout;
+/* host only: the label of one detection at corner (x0, y0): name (UTF-8, 0..255 bytes, each byte outside
+ * ' ' .. '~' drawn as '?'), then with_score ? ", {:.2f}%" of the float32 score * 100 : nothing.  text needs
+ * name_len + YB_PLOT_SUFFIX_MAX bytes.  The device computes every label with this same function. */
+int yb_plot_label_layout(const unsigned char* name, int name_len, int with_score, float score, int tl, int x0,
+                         int y0, unsigned char* text, yb_plot_layout* layout);
+/* host only: bytes of the blob yb_plot_pack writes (the batch's one H2D copy), names_bytes the class names' total */
+int yb_plot_workspace_bytes(int n, int classes, size_t names_bytes, size_t* bytes);
+/* host only: tl [n] line thickness per image (0..1023), colors [classes, 3] (saturated
+ * to 0..255, channel order of the image), names the class names back to back with name_len [classes] bytes each
+ * (-1: no label, as plot_one_box(label=None)); with_score appends the score suffix to every label. */
+int yb_plot_pack(const int* tl, int n, const int* colors, const unsigned char* names, const int* name_len,
+                 int classes, int with_score, void* host_blob, size_t bytes);
+/* Draws in place into data, the PackedImages layout (int64 [n, 4] descriptors (offset, h, w, pitch), then the
+ * uint8 BGR pixels); max_h / max_w bound the images' sizes.  boxes [n, slots, 4] f32 (x0, y0, x1, y1), scores
+ * [n, slots] f32 (may be NULL without the score suffix), labels [n, slots] i32 and counts [n] i32: detections
+ * 0 .. counts[i] - 1 of image i are drawn in order.  Coordinates are truncated toward zero like int(); they are
+ * first clamped to +-2^24, which changes no pixel of an image up to 65535 pixels a side.  A detection with a label
+ * outside [0, classes) or a non-finite coordinate is skipped; status int32 [n, 2] gets (YB_PLOT_BAD_* flags, first
+ * bad slot or -1).  One launch, no host synchronisation. */
+int yb_plot_boxes(void* data, int n, int max_h, int max_w, const float* boxes, const float* scores,
+                  const int* labels, const int* counts, int slots, const void* dev_blob, int* status, void* stream);
+
+/* ---------------------------------------------------------------------------------
  * Loss  (replaces model.py:192-304 loss_layer, :307-345 box_iou, :348-365 compute_loss and
  * the part of TF autodiff (train.py:112) that differentiates them)
  * --------------------------------------------------------------------------------- */

@@ -19,6 +19,7 @@ YB_PHASE_LOCAL, YB_PHASE_GLOBAL = 0, 1
 YB_VOC_MAX_GT = 1024
 YB_KMEANS_MAX_K = 32
 YB_JPEG_BAD_MARKER, YB_JPEG_BAD_RST, YB_JPEG_BAD_CODE, YB_JPEG_BAD_INDEX, YB_JPEG_TRUNCATED = 1, 2, 4, 8, 16
+YB_PLOT_BAD_LABEL, YB_PLOT_BAD_BOX, YB_PLOT_SUFFIX_MAX = 1, 2, 48
 YB_JPEG_SAMPLING = {"411": 0x411111, "420": 0x221111, "422": 0x211111, "440": 0x121111, "444": 0x111111}
 YB_LAYER_IGEMM, YB_LAYER_HALO, YB_LAYER_FUSED_STEM, YB_LAYER_STEM, YB_LAYER_THIN = 1, 2, 3, 4, 5
 
@@ -77,6 +78,10 @@ class JpegInfo(C.Structure):       # yb_jpeg_info
 class JpegEncImage(C.Structure):   # yb_jpeg_enc_image
     _fields_ = [("pixels", vp), ("pitch", C.c_int64)] + [(n, i32) for n in (
         "height", "width", "channels", "quality", "luma_quality", "chroma_quality", "sampling", "restart_interval")]
+
+
+class PlotLayout(C.Structure):     # yb_plot_layout
+    _fields_ = [(n, i32) for n in ("length", "thickness", "text_w", "text_h", "rect_x1", "rect_y1", "org_x", "org_y")]
 
 
 class Optimizer(C.Structure):      # yb_optimizer
@@ -149,6 +154,10 @@ _SIGS = {
     "yb_jpeg_enc_pack": ([C.POINTER(JpegEncImage), i32, vp, sz], i32),
     "yb_jpeg_enc_workspace_bytes": ([vp, i32, C.POINTER(sz), C.POINTER(sz)], i32),
     "yb_jpeg_enc_encode": ([vp, vp, i32, vp, sz, vp, vp, sz, vp], i32),
+    "yb_plot_label_layout": ([C.c_char_p, i32, i32, f32, i32, i32, i32, vp, C.POINTER(PlotLayout)], i32),
+    "yb_plot_workspace_bytes": ([i32, i32, sz, C.POINTER(sz)], i32),
+    "yb_plot_pack": ([vp, i32, vp, C.c_char_p, vp, i32, i32, vp, sz], i32),
+    "yb_plot_boxes": ([vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp], i32),
     "yb_loss_workspace_bytes": ([i32, i32, i32, C.POINTER(sz)], i32),
     "yb_loss_layer": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32, i32, f32, f32, vp, sz, vp, vp, i32, i32, vp], i32),
     "yb_loss_finalize": ([vp, vp, vp], i32),
