@@ -197,6 +197,40 @@ int yb_resize_boxes(float* boxes, const int32_t* counts, int n, int vmax, int bo
 int yb_restore_boxes(float* boxes, const int32_t* counts, int n, int slots, int box_ld, const double* params,
                      void* stream);
 
+/* ---------------------------------------------------------------------------------
+ * Training augmentation  (replaces parse_data(mode='train')'s image work around the resize, utils/data_utils.py:
+ * 140-165: mix_up, random_color_distort, random_expand, the crop of random_crop_with_constraints and random_flip)
+ * --------------------------------------------------------------------------------- */
+/* One output image of yb_augment_batch.  All random draws are made on the host; this is what they decided. */
+typedef struct yb_augment_param {
+  int64_t out_offset;          /* byte offset of the output image in `out`                              */
+  int32_t out_h, out_w;        /* crop size = output size                                               */
+  int32_t crop_y, crop_x;      /* crop origin on the canvas                                             */
+  int32_t canvas_h, canvas_w;  /* expanded canvas; the mixed image's size when not expanded             */
+  int32_t off_y, off_x;        /* origin of the mixed image on the canvas                               */
+  int32_t src1, src2;          /* input images; src2 = -1: no mix-up                                    */
+  float w1, w2;                /* mix-up weights float32(r), float32(1 - r)                             */
+  int32_t color;               /* 1: brightness + BGR2HSV + hue / saturation / value + HSV2BGR          */
+  int32_t brightness;          /* delta added before BGR2HSV (0: not drawn)                             */
+  int32_t hue;                 /* delta added to H, mod 180 (0: not drawn)                              */
+  float saturation, value;     /* multipliers of S and V (1: not drawn)                                 */
+  int32_t fill;                /* canvas value outside the mixed image, 0..255                          */
+} yb_augment_param;
+/* mix-up -> brightness -> BGR2HSV -> hue / saturation / value -> clip -> HSV2BGR -> expand -> crop in one launch:
+ * images / desc_host / desc_dev as yb_resize_batch (n_in inputs), params_host and params_dev the same n records
+ * (host copy for validation, device copy for the kernel), out the output pixels, out_desc_dev the output's int64
+ * [n, 4] descriptor table (offset, h, w, 3 w), written by the kernel.  Pixels equal OpenCV 4.13's cvtColor (x86-64
+ * build: vector blocks of 32 pixels truncate in HSV2BGR, the scalar row tail rounds) and numpy's float32 arithmetic.
+ * Descriptors, image indices, expand offsets, crop windows and output ranges are checked before any device work. */
+int yb_augment_batch(const uint8_t* images, long images_bytes, const int64_t* desc_host, const int64_t* desc_dev,
+                     int n_in, const yb_augment_param* params_host, const yb_augment_param* params_dev, int n,
+                     uint8_t* out, long out_bytes, int64_t* out_desc_dev, void* stream);
+/* random_flip in place on n equal-size images x [n, h, w, 3] of uint8 (elem_bytes 1) or float32 (4): flags_dev int32
+ * [n], bit 0 horizontal (cv2.flip(img, 1)), bit 1 vertical (cv2.flip(img, 0)).  With boxes (float32 [n, vmax,
+ * box_ld], the first counts[i] of image i): x' = w - x, y' = h - y with min and max swapped, float32.  One launch. */
+int yb_flip_batch(void* x, int n, int h, int w, int elem_bytes, const int32_t* flags_dev, float* boxes,
+                  const int32_t* counts, int vmax, int box_ld, void* stream);
+
 /* Weight repack (utils/misc_utils.py:114-123 does (Cout,Cin,kh,kw) -> HWIO on the host):
  * src float32 in `layout` -> dst `dtype` (or float32) OHWI [cout_pad,k,k,cin], rows >= cout zeroed. */
 int yb_pack_conv_weights(const float* src, int layout, int cout, int cin, int ksize, int cout_pad, int dtype,

@@ -84,6 +84,13 @@ class PlotLayout(C.Structure):     # yb_plot_layout
     _fields_ = [(n, i32) for n in ("length", "thickness", "text_w", "text_h", "rect_x1", "rect_y1", "org_x", "org_y")]
 
 
+class AugmentParam(C.Structure):   # yb_augment_param
+    _fields_ = [("out_offset", C.c_int64)] + [(n, i32) for n in (
+        "out_h", "out_w", "crop_y", "crop_x", "canvas_h", "canvas_w", "off_y", "off_x", "src1", "src2")] + [
+        ("w1", f32), ("w2", f32), ("color", i32), ("brightness", i32), ("hue", i32), ("saturation", f32),
+        ("value", f32), ("fill", i32)]
+
+
 class Optimizer(C.Structure):      # yb_optimizer
     _fields_ = [("kind", i32)] + [(n, f32) for n in ("lr", "grad_scale", "momentum", "decay", "beta1", "beta2", "epsilon",
                                                       "weight_decay", "clip_norm")]
@@ -112,6 +119,8 @@ _SIGS = {
     "yb_resize_batch": ([vp, C.c_long, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
     "yb_resize_boxes": ([vp, vp, i32, i32, i32, vp, i32, i32, i32, vp], i32),
     "yb_restore_boxes": ([vp, vp, i32, i32, i32, vp, vp], i32),
+    "yb_augment_batch": ([vp, C.c_long, vp, vp, i32, vp, vp, i32, vp, C.c_long, vp, vp], i32),
+    "yb_flip_batch": ([vp, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp], i32),
     "yb_pack_conv_weights": ([vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
     "yb_pack_conv_weights_e4m3": ([vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
     "yb_amax": ([vp, C.c_long, C.c_long, i32, i32, vp, vp], i32),

@@ -3,7 +3,9 @@
 (test_single_image.py:44-46) into device kernels (libyolob200.so: yb_letterbox_normalize for one image, yb_resize_batch
 for a batch of images of different sizes, letterbox or stretch, nearest or bilinear), plus the detections' way back to
 the source image (test_single_image.py:64-70, yb_restore_boxes).  Bit-exact vs cv2.resize(..., interpolation=0 / 1) of
-OpenCV 4.13; the random augmentations of training are CPU image I/O and out of scope.  `decode_jpeg_batch` replaces
+OpenCV 4.13.  The training augmentations around the resize (`mix_up`, `random_color_distort`, `random_expand`,
+`random_crop_with_constraints`, `random_flip`, batched as `augment_train_batch` + `flip_batch`) draw on the host in the
+reference's order and run as device kernels (yb_augment_batch, yb_flip_batch).  `decode_jpeg_batch` replaces
 the cv2.imread in front of them (utils/data_utils.py:130, test_single_image.py:38): baseline JPEG files decoded on the
 device (yb_jpeg_decode), equal to cv2.imread byte for byte, straight into the PackedImages layout.
 `encode_jpeg_batch` / `write_jpeg_batch` are cv2.imencode('.jpg') / cv2.imwrite (test_single_image.py:85) for a batch
@@ -11,6 +13,7 @@ on the device (yb_jpeg_enc_encode), byte for byte."""
 from __future__ import annotations
 
 import ctypes as C
+import random
 
 import numpy as np
 import torch
@@ -366,3 +369,303 @@ def write_jpeg_batch(paths, images, **kw):
     for p, f in zip(paths, files):
         with open(p, "wb") as fh:
             fh.write(f)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Training augmentation: parse_data(mode='train') (utils/data_utils.py:140-165) around the resize.  The draws are made
+# here, on the host, from np.random and random in the reference's order; the pixels are one device launch
+# (yb_augment_batch) before the resize and one (yb_flip_batch) after it.
+# ---------------------------------------------------------------------------------------------------------------------
+
+def bbox_iou(bbox_a, bbox_b, offset=0):
+    """IoU matrix [N, M] of boxes (x_min, y_min, x_max, y_max, ...) [N, >=4] and [M, >=4]; `offset` is added to each
+    width and height (utils/data_aug.py:93-120)."""
+    if bbox_a.shape[1] < 4 or bbox_b.shape[1] < 4:
+        raise IndexError("Bounding boxes axis 1 must have at least length 4")
+    lo = np.maximum(bbox_a[:, None, :2], bbox_b[None, :, :2])
+    hi = np.minimum(bbox_a[:, None, 2:4], bbox_b[None, :, 2:4])
+    inter = np.prod(hi - lo + offset, axis=2) * (lo < hi).all(axis=2)
+    area_a = np.prod(bbox_a[:, 2:4] - bbox_a[:, :2] + offset, axis=1)
+    area_b = np.prod(bbox_b[:, 2:4] - bbox_b[:, :2] + offset, axis=1)
+    return inter / (area_a[:, None] + area_b[None, :] - inter)
+
+
+def bbox_crop(bbox, crop_box=None, allow_outside_center=True):
+    """Boxes [N, >=4] clipped to crop_box = (x, y, w, h) (None or 0 entries: unbounded) and shifted to its origin;
+    boxes left empty, and unless allow_outside_center those whose centre lies outside, are dropped.  Extra columns
+    are carried (utils/data_aug.py:39-91)."""
+    out = bbox.copy()
+    if crop_box is None:
+        return out
+    if len(crop_box) != 4:
+        raise ValueError(f"Invalid crop_box parameter, requires length 4, given {crop_box}")
+    if all(c is None for c in crop_box):
+        return out
+    x, y, w, h = crop_box
+    x, y = (x or 0), (y or 0)
+    win = np.array((x, y, x + (w if w else np.inf), y + (h if h else np.inf)))
+    keep = np.ones(len(out), bool)
+    if not allow_outside_center:
+        centre = (out[:, :2] + out[:, 2:4]) / 2
+        keep = ((win[:2] <= centre) & (centre < win[2:])).all(axis=1)
+    out[:, :2] = np.maximum(out[:, :2], win[:2])
+    out[:, 2:4] = np.minimum(out[:, 2:4], win[2:4])
+    out[:, :2] -= win[:2]
+    out[:, 2:4] -= win[:2]
+    keep &= (out[:, :2] < out[:, 2:4]).all(axis=1)
+    return out[keep]
+
+
+_SSD_CONSTRAINTS = ((0.1, None), (0.3, None), (0.5, None), (0.7, None), (0.9, None), (None, 1))
+
+
+def random_crop_with_constraints(bbox, size, min_scale=0.3, max_scale=1, max_aspect_ratio=2, constraints=None,
+                                 max_trial=50):
+    """SSD's constrained random crop (utils/data_aug.py:123-217): size = (w, h) -> (boxes, (x, y, w, h)).
+    Up to max_trial windows per (min_iou, max_iou) constraint are drawn with `random`; the first one whose IoU with
+    every box lies in range joins the candidates, then np.random picks candidates until one keeps a box centre.
+    An image without boxes takes the first window drawn.  A window as tall or wide as the image makes
+    random.randrange(0) raise ValueError, as in the reference."""
+    w, h = size
+    picks = [(0, 0, w, h)]
+    for lo, hi in (_SSD_CONSTRAINTS if constraints is None else constraints):
+        lo = -np.inf if lo is None else lo
+        hi = np.inf if hi is None else hi
+        for _ in range(max_trial):
+            scale = random.uniform(min_scale, max_scale)
+            ar = random.uniform(max(1 / max_aspect_ratio, scale * scale), min(max_aspect_ratio, 1 / (scale * scale)))
+            ch = int(h * scale / np.sqrt(ar))
+            cw = int(w * scale * np.sqrt(ar))
+            cy = random.randrange(h - ch)
+            cx = random.randrange(w - cw)
+            if len(bbox) == 0:
+                return bbox, (cx, cy, cw, ch)
+            iou = bbox_iou(bbox, np.array(((cx, cy, cx + cw, cy + ch),)))
+            if lo <= iou.min() and iou.max() <= hi:
+                picks.append((cx, cy, cw, ch))
+                break
+    while picks:
+        crop = picks.pop(np.random.randint(0, len(picks)))
+        kept = bbox_crop(bbox, crop, allow_outside_center=False)
+        if kept.size:
+            return kept, tuple(crop)
+    return bbox, (0, 0, w, h)
+
+
+def _draw_mix():
+    r = np.random.beta(1.5, 1.5)
+    return max(0, min(1, r))
+
+
+def _draw_color(brightness_delta=32, hue_vari=18, sat_vari=0.5, val_vari=0.5):
+    """random_color_distort's draws -> (brightness delta, hue delta, saturation and value multipliers); an op whose
+    coin does not land above 0.5 gets its identity.  Every coin is drawn, taken or not."""
+    bright = int(np.random.uniform(-brightness_delta, brightness_delta)) if np.random.uniform(0, 1) > 0.5 else 0
+    amount = {"hue": 0, "sat": 1.0, "val": 1.0}
+    draws = {"hue": lambda: int(np.random.randint(-hue_vari, hue_vari)),
+             "sat": lambda: 1 + np.random.uniform(-sat_vari, sat_vari),
+             "val": lambda: 1 + np.random.uniform(-val_vari, val_vari)}
+    for op in (("val", "sat", "hue") if np.random.randint(0, 2) else ("sat", "hue", "val")):
+        if np.random.uniform(0, 1) > 0.5:
+            amount[op] = draws[op]()
+    return bright, amount["hue"], amount["sat"], amount["val"]
+
+
+def _draw_expand(h, w, max_ratio=4, keep_ratio=True):
+    """random_expand's draws -> (canvas h, canvas w, off_y, off_x)."""
+    rx = random.uniform(1, max_ratio)
+    ry = rx if keep_ratio else random.uniform(1, max_ratio)
+    oh, ow = int(h * ry), int(w * rx)
+    return oh, ow, random.randint(0, oh - h), random.randint(0, ow - w)
+
+
+def _augment_param(src1, h, w, src2=-1, r=None, color=None, expand=None, crop=None, fill=0):
+    """The yb_augment_param of one output; h, w are the mixed image's size."""
+    p = _lib.AugmentParam()
+    p.src1, p.src2 = src1, src2
+    p.w1, p.w2 = (1.0, 0.0) if r is None else (np.float32(r), np.float32(1.0 - r))
+    p.canvas_h, p.canvas_w, p.off_y, p.off_x = expand if expand is not None else (h, w, 0, 0)
+    p.crop_x, p.crop_y, p.out_w, p.out_h = crop if crop is not None else (0, 0, p.canvas_w, p.canvas_h)
+    p.color = int(color is not None)
+    p.brightness, p.hue, p.saturation, p.value = color if color is not None else (0, 0, 1.0, 1.0)
+    p.fill = int(fill)
+    return p
+
+
+def _augment_launch(packed, params):
+    """One yb_augment_batch over `packed` with the records `params` -> PackedImages of the outputs."""
+    n = len(params)
+    table = (_lib.AugmentParam * n)(*params)
+    off = 0
+    for p in table:
+        p.out_offset = off
+        off += (3 * p.out_h * p.out_w + 15) // 16 * 16
+    dev = packed.device
+    nbytes = C.sizeof(table)
+    host = torch.empty((nbytes,), dtype=torch.uint8, pin_memory=True)
+    C.memmove(host.data_ptr(), C.addressof(table), nbytes)
+    desc = np.ascontiguousarray(packed.desc)
+    with torch.cuda.device(dev):
+        pdev = host.to(dev, non_blocking=True)                # the one host -> device copy
+        data = torch.empty((n * 32 + max(off, 1),), dtype=torch.uint8, device=dev)
+        check(lib.yb_augment_batch(ptr(packed.pixels), packed.pixels.numel(), desc.ctypes.data_as(C.c_void_p),
+                                   ptr(packed.desc_dev), packed.n, C.cast(table, C.c_void_p), ptr(pdev), n,
+                                   ptr(data[n * 32:]), data.numel() - n * 32, ptr(data), stream_handle()),
+              "yb_augment_batch")
+    out_desc = np.array([(p.out_offset, p.out_h, p.out_w, 3 * p.out_w) for p in table], np.int64).reshape(n, 4)
+    return PackedImages.from_device(data, out_desc, h2d_bytes=nbytes)
+
+
+def _one(img, device=None):
+    packed = img if isinstance(img, PackedImages) else PackedImages([img], device)
+    h, w = (int(v) for v in packed.desc[0, 1:3])
+    return packed, h, w
+
+
+def mix_up(img1, img2, bbox1, bbox2):
+    """utils/data_aug.py:12-36: img1 * r + img2 * (1 - r) on a canvas of the larger sides, r ~ Beta(1.5, 1.5) ->
+    (mixed image uint8 [H, W, 3] on the device, boxes float64 [N1 + N2, 5] with r / 1 - r as the last column)."""
+    packed = PackedImages([img1, img2])
+    (h1, w1), (h2, w2) = packed.desc[0, 1:3].tolist(), packed.desc[1, 1:3].tolist()
+    r = _draw_mix()
+    out = _augment_launch(packed, [_augment_param(0, max(h1, h2), max(w1, w2), 1, r)])
+    b1 = np.concatenate((bbox1, np.full((bbox1.shape[0], 1), r)), axis=-1)
+    b2 = np.concatenate((bbox2, np.full((bbox2.shape[0], 1), 1. - r)), axis=-1)
+    return out.image(0), np.concatenate((b1, b2), axis=0)
+
+
+def random_color_distort(img, brightness_delta=32, hue_vari=18, sat_vari=0.5, val_vari=0.5):
+    """utils/data_aug.py:220-271: random brightness, then value / saturation / hue in one of two drawn orders through
+    OpenCV's 8-bit HSV -> uint8 BGR [H, W, 3] on the device."""
+    packed, h, w = _one(img)
+    color = _draw_color(brightness_delta, hue_vari, sat_vari, val_vari)
+    return _augment_launch(packed, [_augment_param(0, h, w, color=color)]).image(0)
+
+
+def random_expand(img, bbox, max_ratio=4, fill=0, keep_ratio=True):
+    """utils/data_aug.py:349-380: the image placed at a random offset on a canvas up to max_ratio times larger,
+    filled with `fill` -> (uint8 [oh, ow, 3] on the device, bbox shifted in place, as the reference does)."""
+    packed, h, w = _one(img)
+    ex = _draw_expand(h, w, max_ratio, keep_ratio)
+    out = _augment_launch(packed, [_augment_param(0, h, w, expand=ex, fill=fill)]).image(0)
+    bbox[:, :2] += (ex[3], ex[2])
+    bbox[:, 2:4] += (ex[3], ex[2])
+    return out, bbox
+
+
+def _flip_launch(x, flags, boxes=None, counts=None):
+    n, h, w = (int(v) for v in x.shape[:3])
+    f = torch.as_tensor(np.asarray(flags, np.int32).reshape(-1)).pin_memory().to(x.device, non_blocking=True) \
+        if not isinstance(flags, torch.Tensor) else flags.to(x.device, torch.int32, non_blocking=True).contiguous()
+    if f.numel() != n:
+        raise ValueError(f"flip_batch: {f.numel()} flags for {n} images")
+    vmax, ld = (int(boxes.shape[1]), int(boxes.shape[2])) if boxes is not None else (0, 0)
+    with torch.cuda.device(x.device):
+        check(lib.yb_flip_batch(ptr(x), n, h, w, x.element_size(), ptr(f), ptr(boxes), ptr(counts), vmax, ld,
+                                stream_handle()), "yb_flip_batch")
+    return x
+
+
+def flip_batch(x, flags, boxes=None, counts=None):
+    """random_flip's horizontal flip after the resize, for a batch: x float32 [n, H, W, 3] (preprocess_batch's output)
+    flipped in place where flags[i] is true; boxes float32 [n, vmax, >=4] on the device (the first counts[i], int32,
+    of image i) get x' = W - x with min and max swapped.  flags: host booleans (e.g. augment_train_batch's) or a
+    device tensor.  One launch, no host synchronisation.  Returns x."""
+    if (not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.float32 or x.dim() != 4
+            or x.shape[3] != 3 or not x.is_contiguous()):
+        raise ValueError("flip_batch expects a contiguous float32 [n, H, W, 3] CUDA tensor")
+    if boxes is not None:
+        if (counts is None or boxes.dtype != torch.float32 or boxes.dim() != 3 or boxes.shape[0] != x.shape[0]
+                or boxes.shape[2] < 4 or not boxes.is_contiguous() or boxes.device != x.device
+                or counts.dtype != torch.int32 or tuple(counts.shape) != (x.shape[0],) or counts.device != x.device):
+            raise ValueError("flip_batch: boxes must be float32 [n, vmax, >=4] with counts int32 [n], on x's device")
+        if boxes.shape[1] == 0:
+            boxes = counts = None
+    return _flip_launch(x, flags, boxes, counts)
+
+
+def random_flip(img, bbox, px=0, py=0):
+    """utils/data_aug.py:323-346: horizontal flip with probability px, then vertical with py (both coins always
+    drawn).  img uint8 or float32 [H, W, 3] (numpy or CUDA tensor) -> (flipped copy on the device, bbox flipped in
+    place on the host in its own dtype)."""
+    t = torch.from_numpy(np.ascontiguousarray(img)) if isinstance(img, np.ndarray) else img
+    if t.dim() != 3 or t.shape[2] != 3 or t.dtype not in (torch.uint8, torch.float32):
+        raise ValueError(f"random_flip expects a uint8 or float32 [H, W, 3] image, got {t.dtype} {tuple(t.shape)}")
+    height, width = int(t.shape[0]), int(t.shape[1])
+    fx = np.random.uniform(0, 1) < px
+    fy = np.random.uniform(0, 1) < py
+    x = t.to(f"cuda:{torch.cuda.current_device()}" if not t.is_cuda else t.device, copy=True).contiguous()
+    if fx or fy:
+        _flip_launch(x[None], [int(fx) | 2 * int(fy)])
+    if fx:
+        bbox[:, 0], bbox[:, 2] = width - bbox[:, 2], width - bbox[:, 0].copy()
+    if fy:
+        bbox[:, 1], bbox[:, 3] = height - bbox[:, 3], height - bbox[:, 1].copy()
+    return x, bbox
+
+
+def augment_train_batch(images, boxes_list, labels_list, mix_with=None, device=None):
+    """parse_data(mode='train') (utils/data_utils.py:118-165) for a batch, up to its resize: for image i, drawing from
+    np.random and random exactly as the reference does, in this order: the mix-up weight (when mix_with[i] names
+    the partner image j, as get_batch_data's pairing would), the colour coins and amounts, the expand coin and
+    expand, every crop trial and pick, the interpolation, and both flip coins.
+      images: uint8 BGR [H, W, 3] images or a PackedImages (decode_jpeg_batch's output: no upload); boxes_list: per
+      image [V, 4] (x_min, y_min, x_max, y_max); labels_list: per image [V] ints; mix_with: None or, per image,
+      None or the index of its partner.
+    -> (PackedImages of the cropped uint8 images, boxes, labels, interp int64 [n], flip bool [n]).  boxes[i] is host
+    numpy as the reference holds it: float32 [N, 5] with a weight column of 1, float64 after a mix-up.  labels[i] is
+    labels[:len(boxes[i])]: the reference drops boxes in the crop but not their labels, and process_box pairs box k
+    with label k, so this keeps its pairing.  interp is drawn but not applied (preprocess_batch takes 0 or 1);
+    flip[i] is for flip_batch after the resize.  Pixels: one H2D copy of the parameter table and one launch, no
+    host synchronisation."""
+    packed = images if isinstance(images, PackedImages) else PackedImages(images, device)
+    n = packed.n
+    if len(boxes_list) != n or len(labels_list) != n:
+        raise ValueError(f"augment_train_batch: {n} images, {len(boxes_list)} box and {len(labels_list)} label arrays")
+    mix_with = [None] * n if mix_with is None else list(mix_with)
+    if len(mix_with) != n:
+        raise ValueError(f"augment_train_batch: mix_with has {len(mix_with)} entries for {n} images")
+    gt = []
+    for i, (b, l) in enumerate(zip(boxes_list, labels_list)):
+        b = np.asarray(b, np.float32)
+        b = b.reshape(0, 4) if b.size == 0 else b
+        l = np.asarray(l, np.int64).reshape(-1)
+        if b.ndim != 2 or b.shape[1] != 4 or len(b) != len(l):
+            raise ValueError(f"augment_train_batch: image {i}: boxes {b.shape} and labels {l.shape} do not pair")
+        gt.append((b, l))
+    sizes = packed.desc[:, 1:3].tolist()
+    params, boxes_out, labels_out = [], [], []
+    interp, flip = np.zeros(n, np.int64), np.zeros(n, bool)
+    for i in range(n):
+        j = mix_with[i]
+        b1, l1 = gt[i]
+        h, w = sizes[i]
+        if j is None:
+            r = None
+            boxes = np.concatenate((b1, np.ones((len(b1), 1), np.float32)), axis=-1)
+            labels = l1
+        else:
+            j = int(j)
+            if not 0 <= j < n:
+                raise ValueError(f"augment_train_batch: image {i} is paired with image {j} of {n}")
+            b2, l2 = gt[j]
+            h, w = max(h, sizes[j][0]), max(w, sizes[j][1])
+            r = _draw_mix()
+            boxes = np.concatenate((np.concatenate((b1, np.full((len(b1), 1), r)), -1),
+                                    np.concatenate((b2, np.full((len(b2), 1), 1. - r)), -1)), 0)
+            labels = np.concatenate((l1, l2))
+        color = _draw_color()
+        ex = None
+        if np.random.uniform(0, 1) > 0.5:
+            ex = _draw_expand(h, w)
+            boxes[:, :2] += (ex[3], ex[2])
+            boxes[:, 2:4] += (ex[3], ex[2])
+        ch, cw = ex[:2] if ex is not None else (h, w)
+        boxes, crop = random_crop_with_constraints(boxes, (cw, ch))
+        interp[i] = np.random.randint(0, 5)
+        flip[i] = np.random.uniform(0, 1) < 0.5
+        np.random.uniform(0, 1)                               # random_flip's vertical coin (py = 0)
+        params.append(_augment_param(i, h, w, -1 if j is None else j, r, color, ex, crop))
+        boxes_out.append(boxes)
+        labels_out.append(labels[:len(boxes)])
+    return _augment_launch(packed, params), boxes_out, labels_out, interp, flip
