@@ -187,6 +187,25 @@ int yb_letterbox_normalize(const uint8_t* bgr, int src_h, int src_w, long src_pi
  * sides in 1..2^20, and a letterbox whose int() truncation leaves an empty resize is rejected. */
 int yb_resize_batch(const uint8_t* images, long images_bytes, const int64_t* desc_host, const int64_t* desc_dev, int n,
                     int new_h, int new_w, int letterbox, int interp, float* out_rgb, double* params, void* stream);
+/* The training resize (parse_data(mode='train'), utils/data_utils.py:160-161: resize_with_bbox with the drawn
+ * interp): yb_resize_batch with one OpenCV interpolation per image, interp_host int32 [n] in 0..4 -- 0 nearest,
+ * 1 linear (both equal to yb_resize_batch's output), 2 INTER_CUBIC, 3 INTER_AREA, 4 INTER_LANCZOS4.  Each image's
+ * per-axis tap tables are built on the host as OpenCV builds them (Lanczos4 from the C library's sin / cos) into one
+ * 16-byte aligned buffer: yb_resize_tables_bytes gives its size, yb_resize_tables fills it (host only, no device
+ * work), the caller copies it to the device and passes both copies to yb_resize_batch_interp (the host copy is checked
+ * against the call).  A 608 x 608 cubic / Lanczos4 / upscaling area table is 24 kB; a shrinking area table holds
+ * 8 bytes per destination index and up to 16 per source index.
+ * Bit-exact vs cv2.resize of OpenCV 4.13 for INTER_AREA and INTER_LANCZOS4, and for INTER_CUBIC vs OpenCV's own code
+ * (cv2.ipp.setUseIPP(False)); default cv2 builds send uint8 INTER_CUBIC through Intel IPP, which differs by at most 1.
+ * Same size in and out is a copy.  Everything is validated before any device work. */
+int yb_resize_tables_bytes(const int64_t* desc_host, int n, int new_h, int new_w, int letterbox,
+                           const int32_t* interp_host, size_t* bytes);
+int yb_resize_tables(const int64_t* desc_host, int n, int new_h, int new_w, int letterbox, const int32_t* interp_host,
+                     void* tables_host, size_t bytes);
+int yb_resize_batch_interp(const uint8_t* images, long images_bytes, const int64_t* desc_host, const int64_t* desc_dev,
+                           int n, int new_h, int new_w, int letterbox, const int32_t* interp_host,
+                           const void* tables_host, const void* tables_dev, size_t tables_bytes, float* out_rgb,
+                           double* params, void* stream);
 /* resize_with_bbox's box transform (utils/data_aug.py:301-318), in place, float32 in the reference's order:
  * boxes float32 [n, vmax, box_ld] (columns 0-3 x_min, y_min, x_max, y_max; the rest untouched), counts int32 [n],
  * desc_dev the yb_resize_batch descriptor table of the same images. */

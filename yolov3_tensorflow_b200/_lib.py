@@ -117,6 +117,9 @@ _SIGS = {
     "yb_letterbox_params": ([i32, i32, i32, i32, C.POINTER(C.c_double), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
     "yb_letterbox_normalize": ([vp, i32, i32, C.c_long, i32, i32, vp, vp], i32),
     "yb_resize_batch": ([vp, C.c_long, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp], i32),
+    "yb_resize_tables_bytes": ([vp, i32, i32, i32, i32, vp, C.POINTER(sz)], i32),
+    "yb_resize_tables": ([vp, i32, i32, i32, i32, vp, vp, sz], i32),
+    "yb_resize_batch_interp": ([vp, C.c_long, vp, vp, i32, i32, i32, i32, vp, vp, vp, sz, vp, vp, vp], i32),
     "yb_resize_boxes": ([vp, vp, i32, i32, i32, vp, i32, i32, i32, vp], i32),
     "yb_restore_boxes": ([vp, vp, i32, i32, i32, vp, vp], i32),
     "yb_augment_batch": ([vp, C.c_long, vp, vp, i32, vp, vp, i32, vp, C.c_long, vp, vp], i32),

@@ -1,9 +1,10 @@
 """utils/data_aug.py of the reference, the functions on the inference and evaluation input path: `letterbox_resize`
 (:274-293) and `resize_with_bbox` (:296-318), fused with the caller's BGR->RGB + float32 / 255
 (test_single_image.py:44-46) into device kernels (libyolob200.so: yb_letterbox_normalize for one image, yb_resize_batch
-for a batch of images of different sizes, letterbox or stretch, nearest or bilinear), plus the detections' way back to
-the source image (test_single_image.py:64-70, yb_restore_boxes).  Bit-exact vs cv2.resize(..., interpolation=0 / 1) of
-OpenCV 4.13.  The training augmentations around the resize (`mix_up`, `random_color_distort`, `random_expand`,
+for a batch of images of different sizes, letterbox or stretch, nearest or bilinear; yb_resize_batch_interp for the
+training resize with every cv2.resize interpolation of the reference, 0..4, one per image), plus the detections' way
+back to the source image (test_single_image.py:64-70, yb_restore_boxes).  Bit-exact vs cv2.resize of OpenCV 4.13
+(INTER_CUBIC: OpenCV's own code, within 1 of its Intel IPP dispatch).  The training augmentations around the resize (`mix_up`, `random_color_distort`, `random_expand`,
 `random_crop_with_constraints`, `random_flip`, batched as `augment_train_batch` + `flip_batch`) draw on the host in the
 reference's order and run as device kernels (yb_augment_batch, yb_flip_batch).  `decode_jpeg_batch` replaces
 the cv2.imread in front of them (utils/data_utils.py:130, test_single_image.py:38): baseline JPEG files decoded on the
@@ -132,6 +133,58 @@ def _resize_packed(packed, new_width, new_height, letterbox, interp, out=None):
     return out, params
 
 
+def _resize_packed_interp(packed, new_width, new_height, letterbox, interp, out=None):
+    """yb_resize_batch_interp: one OpenCV interpolation (0..4) per image, the tap tables built on the host and sent
+    in one pinned H2D copy."""
+    n, dev = packed.n, packed.device
+    new_w, new_h = int(new_width), int(new_height)
+    it = np.asarray(interp, np.int64).reshape(-1)
+    if it.size == 1:
+        it = np.full(n, int(it[0]), np.int64)
+    if it.size != n:
+        raise ValueError(f"resize_train_batch: {it.size} interpolations for {n} images")
+    if ((it < 0) | (it > 4)).any():
+        i = int(np.argmax((it < 0) | (it > 4)))
+        raise ValueError(f"resize_train_batch: image {i}: interp must be in 0..4 (cv2.INTER_NEAREST .. INTER_LANCZOS4), "
+                         f"got {int(it[i])}")
+    it = np.ascontiguousarray(it, np.int32)
+    if out is None:
+        out = torch.empty((n, new_h, new_w, 3), dtype=torch.float32, device=dev)
+    elif (out.dtype != torch.float32 or tuple(out.shape) != (n, new_h, new_w, 3) or not out.is_contiguous()
+          or out.device != dev):
+        raise ValueError(f"out must be a contiguous float32 [{n}, {new_h}, {new_w}, 3] tensor on {dev}")
+    params = torch.empty((n, 4), dtype=torch.float64, device=dev)
+    desc = np.ascontiguousarray(packed.desc)
+    dp, ip, lb = desc.ctypes.data_as(C.c_void_p), it.ctypes.data_as(C.c_void_p), int(bool(letterbox))
+    nbytes = C.c_size_t()
+    check(lib.yb_resize_tables_bytes(dp, n, new_h, new_w, lb, ip, C.byref(nbytes)), "yb_resize_tables_bytes")
+    host = torch.empty((nbytes.value,), dtype=torch.uint8, pin_memory=True)
+    check(lib.yb_resize_tables(dp, n, new_h, new_w, lb, ip, C.c_void_p(host.data_ptr()), nbytes.value),
+          "yb_resize_tables")
+    with torch.cuda.device(dev):
+        tabs = host.to(dev, non_blocking=True)                # the one host -> device copy
+        check(lib.yb_resize_batch_interp(ptr(packed.pixels), packed.pixels.numel(), dp, ptr(packed.desc_dev), n, new_h,
+                                         new_w, lb, ip, C.c_void_p(host.data_ptr()), ptr(tabs), nbytes.value, ptr(out),
+                                         ptr(params), stream_handle()), "yb_resize_batch_interp")
+    return out, params
+
+
+def resize_train_batch(images, new_width, new_height, interp, letterbox=True, out=None, device=None):
+    """The resize of parse_data(mode='train') (utils/data_utils.py:160-161) for a batch: resize_with_bbox with each
+    image's drawn interpolation, fused with BGR->RGB + float32 / 255.
+      images: a PackedImages (augment_train_batch's or decode_jpeg_batch's output: no upload) or a list of uint8 BGR
+      [H, W, 3] images; interp: one int or one per image (augment_train_batch's int64 [n]), 0 INTER_NEAREST,
+      1 INTER_LINEAR, 2 INTER_CUBIC, 3 INTER_AREA, 4 INTER_LANCZOS4.
+    -> (x float32 [n, new_height, new_width, 3] RGB in [0, 1], params float64 [n, 4]) on the device, as
+    preprocess_batch returns them, so flip_batch, yb_resize_boxes and process_box_batch follow unchanged.
+    Equal to cv2.resize of OpenCV 4.13 byte for byte; for INTER_CUBIC that is OpenCV's own code
+    (cv2.ipp.setUseIPP(False)), within 1 of a default cv2 build, which sends it through Intel IPP.  Interp 0 / 1
+    images equal preprocess_batch's.  The per-image tap tables are built on the host (yb_resize_tables) and cross
+    in one H2D copy; one launch, no host synchronisation."""
+    packed = images if isinstance(images, PackedImages) else PackedImages(images, device)
+    return _resize_packed_interp(packed, new_width, new_height, letterbox, interp, out)
+
+
 def preprocess_batch(images, new_width, new_height, letterbox=True, interp=1, out=None, device=None):
     """images: list of uint8 [H, W, 3] BGR images of any sizes (numpy arrays or tensors), or a PackedImages (from
     decode_jpeg_batch: no second upload) ->
@@ -150,9 +203,13 @@ def preprocess_batch(images, new_width, new_height, letterbox=True, interp=1, ou
 def resize_with_bbox(img, bbox, new_width, new_height, interp=0, letterbox=False):
     """utils/data_aug.py:296-318 for one image, the reference's signature, with the caller's cvtColor(BGR2RGB) +
     float32 / 255 fused in: -> (x float32 [new_height, new_width, 3] RGB in [0, 1], bbox float32 [V, >=4] transformed
-    like the reference), both on the device.  Columns past the fourth (a mix-up weight) are carried unchanged."""
+    like the reference), both on the device.  Columns past the fourth (a mix-up weight) are carried unchanged.
+    interp 0 / 1 take preprocess_batch's path, 2..4 (cubic, area, Lanczos4) resize_train_batch's."""
     packed = PackedImages([img])
-    x, _ = _resize_packed(packed, new_width, new_height, letterbox, interp)
+    if interp in (0, 1):
+        x, _ = _resize_packed(packed, new_width, new_height, letterbox, interp)
+    else:
+        x, _ = _resize_packed_interp(packed, new_width, new_height, letterbox, interp)
     a = np.asarray(bbox, np.float32)
     if a.ndim != 2 or a.shape[1] < 4:
         raise ValueError(f"bbox must be [V, >=4], got {a.shape}")
@@ -615,8 +672,8 @@ def augment_train_batch(images, boxes_list, labels_list, mix_with=None, device=N
     -> (PackedImages of the cropped uint8 images, boxes, labels, interp int64 [n], flip bool [n]).  boxes[i] is host
     numpy as the reference holds it: float32 [N, 5] with a weight column of 1, float64 after a mix-up.  labels[i] is
     labels[:len(boxes[i])]: the reference drops boxes in the crop but not their labels, and process_box pairs box k
-    with label k, so this keeps its pairing.  interp is drawn but not applied (preprocess_batch takes 0 or 1);
-    flip[i] is for flip_batch after the resize.  Pixels: one H2D copy of the parameter table and one launch, no
+    with label k, so this keeps its pairing.  interp[i] (0..4) is for resize_train_batch; flip[i] is for flip_batch
+    after the resize.  Pixels: one H2D copy of the parameter table and one launch, no
     host synchronisation."""
     packed = images if isinstance(images, PackedImages) else PackedImages(images, device)
     n = packed.n
