@@ -746,6 +746,11 @@ int yb_net_train_backward_layer(yb_net* net, const float* images, int layer, int
 int yb_net_train_join(yb_net* net, void* stream);
 /* BN layer `layer`'s exchange slab, 2 x cout_pad floats: forward [Σz | Σz²], backward [Σdact·ẑ | Σdact]. */
 int yb_net_bn_exchange_buffer(yb_net* net, int layer, int backward, float** ptr, size_t* count);
+/* Read-only view of BN layer `layer`'s coefficients from the last training forward, fp32 [cout] each (activation
+ * arena): the mean it normalised with (the moving mean under YB_TRAIN_BN_FROZEN), invstd = rsqrtf(var + eps), and
+ * scale = gamma * invstd, shift = beta - mean * scale, which the activation and the backward read.  Needs a bound
+ * training plan and a layer with batch norm (YB_ERR_INVALID_ARGUMENT otherwise); a NULL output is skipped. */
+int yb_net_bn_batch_stats(yb_net* net, int layer, float** mean, float** invstd, float** scale, float** shift);
 /* the flat float32 gradient of all 222 trainable tensors (creation order: per conv w [OHWI], then gamma, beta
  * | bias; each padded to 4 floats) — the buffer a data-parallel wrapper all-reduces. */
 int yb_net_grad_buffer(yb_net* net, float** ptr, size_t* count);

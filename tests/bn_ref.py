@@ -31,6 +31,10 @@ shared-memory adds, one centring fma and the invstd product, `grid` atomic adds 
 BN_SLOTS final adds, each rounding once to at most the magnitude sum:
     |dbeta - ref| <= n_ops u A,   |dgamma - ref| <= n_ops u invstd (G + |mean| A),
     n_ops = rows_per_block / lanes + lanes + grid + BN_SLOTS + 4.
+The atomic adds are the one place subnormals do not survive: float atomicAdd (PTX atom / red .add.f32) flushes
+subnormal inputs and results to sign-preserving zero, so each of the `grid` atomic adds a value passes through may
+also drop less than 2^-126 twice, its input and its result.  Both bounds carry the absolute term 2 grid 2^-126 for it
+(it matters only for a channel whose sums are themselves near the subnormal range).
 
 bwd apply (bn_bwd_apply_kernel).  k1 = ga is, k2 = -k1 is dg inv_m, k3 = -k1 db inv_m - k2 mu with inv_m = fl32(1 / M),
 dz = fmaf(k1, dact, fmaf(k2, z, k3)).  Relative errors: inv_m 1 u, k1 1 u, k2 5 u, k1 db inv_m 4 u, k2 mu 6 u, k3's
@@ -47,6 +51,7 @@ from tests.conv_ref import SLOPE, U32, ulp
 RSQRT_ULP = 2          # rsqrtf, CUDA C Programming Guide (single-precision mathematical functions)
 EXACT_LIMIT = 2.0 ** 24
 BN_SLOTS = 16          # csrc/bn.cu
+FTZ32 = 2.0 ** -126    # smallest normal float32: what one flushing atomic add may drop, per input and per result
 _F32 = torch.float32
 
 
@@ -155,7 +160,8 @@ def reduce_ref(parts, mu, invstd):
 def reduce_bound(G, A, mu, invstd, rows_per_block, lanes, grid):
     """Float-operand bounds of (dgamma, dbeta) (module docstring)."""
     n_ops = -(-rows_per_block // lanes) + lanes + grid + BN_SLOTS + 4
-    return (n_ops * U32 * invstd.double().abs() * (G + mu.double().abs() * A), n_ops * U32 * A)
+    ftz = 2 * grid * FTZ32
+    return (n_ops * U32 * invstd.double().abs() * (G + mu.double().abs() * A) + ftz, n_ops * U32 * A + ftz)
 
 
 def bwd_apply_ref(da, z, ga, invstd, mu, dg, db, count, dtype):

@@ -197,6 +197,7 @@ _SIGS = {
     "yb_net_train_backward_layer": ([vp, vp, i32, i32, i32, i32, vp], i32),
     "yb_net_train_join": ([vp, vp], i32),
     "yb_net_bn_exchange_buffer": ([vp, i32, i32, C.POINTER(vp), C.POINTER(sz)], i32),
+    "yb_net_bn_batch_stats": ([vp, i32] + [C.POINTER(vp)] * 4, i32),
     "yb_net_grad_buffer": ([vp, C.POINTER(vp), C.POINTER(sz)], i32),
     "yb_net_train_update": ([vp, C.POINTER(Optimizer), vp], i32),
     "yb_net_train_reset_state": ([vp, i32, vp], i32),

@@ -593,6 +593,19 @@ extern "C" int yb_net_bn_exchange_buffer(yb_net* net, int layer, int backward, f
   return YB_OK;
 }
 
+extern "C" int yb_net_bn_batch_stats(yb_net* net, int layer, float** mean, float** invstd, float** scale,
+                                     float** shift) {
+  YB_REQUIRE(net && net->training && layer >= 0 && layer < (int)net->layers.size(), "bn_batch_stats: bad argument");
+  const Layer& L = net->layers[layer];
+  YB_REQUIRE(L.info.has_bn, "bn_batch_stats: layer %d has no batch norm", layer);
+  YB_REQUIRE(net->act, "bn_batch_stats: not a bound training plan");
+  if (mean) *mean = fact(net, L.st_mean);
+  if (invstd) *invstd = fact(net, L.st_invstd);
+  if (scale) *scale = fact(net, L.st_scale);
+  if (shift) *shift = fact(net, L.st_shift);
+  return YB_OK;
+}
+
 extern "C" int yb_net_train_reset_state(yb_net* net, int optimizer_kind, void* stream) {
   YB_REQUIRE(net && net->training && net->par, "train_reset_state: not a bound training plan");
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -135,6 +135,18 @@ class _Plan:
         off = p.value - self.act.data_ptr()
         return self.act[off: off + n.value * 4].view(torch.float32)
 
+    def bn_batch_stats(self, i):
+        """BN layer i's coefficients from the last training forward (include/yolob200.h: yb_net_bn_batch_stats):
+        dict(mean, invstd, scale, shift) of float32 [cout] views into the activation arena."""
+        ps = [C.c_void_p() for _ in range(4)]
+        check(lib.yb_net_bn_batch_stats(self.handle, int(i), *[C.byref(q) for q in ps]), "yb_net_bn_batch_stats")
+        c = self.layer_info(i).cout
+        out = {}
+        for name, q in zip(("mean", "invstd", "scale", "shift"), ps):
+            off = q.value - self.act.data_ptr()
+            out[name] = self.act[off: off + c * 4].view(torch.float32)
+        return out
+
     def opt_norms(self):
         """Per-tensor squared norms of the last update, float32 [222] view (include/yolob200.h: yb_net_opt_norms)."""
         p, n = C.c_void_p(), C.c_int()
